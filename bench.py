@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py - measurement harness of the OrientedRepPoints B200 hot path (contract in the task brief).
+"""bench.py - measurement harness of the OrientedRepPoints hot path on an H100.
 
     python bench.py --gpus 1 --steps 20 --warmup 5                 # our arm, one JSON line
+    python bench.py --gpus 1 --steps 3 --warmup 1 --dump-outputs DIR   # + the last timed step's outputs as DIR/<name>.npy
     python bench.py --impl reference --gpus 1 --steps 3 --warmup 1 # reference CPU arm, one JSON line
     torchrun ... bench.py --gpus N ...                             # one rank per GPU (weak scaling)
 
@@ -43,12 +44,32 @@ def parse_args():
     ap.add_argument("--backbone", default=None, help="r50_tile workload backbone: r50 (default) | r101 | swin_tiny")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-graph", dest="no_graph", action="store_true", help="r50_tile: eager launches instead of a CUDA graph")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", dest="dump_outputs", default=None, metavar="DIR",
+                    help="write what the timed path returned in its last timed step as DIR/<name>.npy (float32 / float64)")
+    args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    return args
+
+
+def dump_outputs(out_dir, arrays, limit=64 << 20):
+    """arrays: name -> numpy array.  Integer arrays are stored as float64 (exact below 2^53), floating ones as float32 /
+    float64; together at most `limit` bytes.  Inputs are seeded, so two builds run with the same arguments can be compared
+    file for file."""
+    os.makedirs(out_dir, exist_ok=True)
+    total = 0
+    for name, a in arrays.items():
+        a = np.asarray(a)
+        a = a.astype(np.float64) if (a.dtype.kind in "iub" or a.dtype == np.float64) else a.astype(np.float32)
+        total += a.nbytes
+        if total > limit:
+            raise SystemExit("--dump-outputs: the outputs exceed %d bytes" % limit)
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 # ----------------------------------------------------------------------------------------------- clocks
 class ClockSampler:
-    """nvidia-smi sampling DURING the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi sampling DURING the timed region: SM clock, its maximum and active throttle reasons."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -140,7 +161,8 @@ def peaks():
                     "bf16_tflops_sustained": d.get("bf16_tflops_sustained", d["bf16_tflops"]), "source": "measured"}
         except Exception:
             pass
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "source": "fallback"}
+    # NVIDIA's data sheet for the H100 SXM (dense, 700 W card): a bound, never a measured figure
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "source": "H100 SXM data sheet"}
 
 
 # ----------------------------------------------------------------------------------------------- NMS workload
@@ -153,11 +175,12 @@ def nms_bitmatrix_bytes(n):
 # per-candidate-pair arithmetic of the exact decision (fp32 Sutherland-Hodgman of two quadrilaterals in pair-local
 # coordinates with a running error bound: 4 clip edges x <=8 ring vertices x ~14 flops + areas), counted from the source
 CLIP_FLOPS = 700.0
-FP32_PEAK_TFLOPS = 148 * 128 * 2 * 1.965e9 / 1e12      # 148 SMs x 128 FMA lanes x 2 x 1.965 GHz = 74.4 (nominal, no measured figure)
+FP32_PEAK_TFLOPS = 67.0                                 # H100 SXM data sheet, FP32 (nominal, no measured figure)
 
 
 def time_nms(dets_h, local, steps, warm, world, flush, thr=0.1):
-    """device-timed rotated NMS of one box set resident in HBM: (ms per call, sweep-kernel ms, kept, stats)"""
+    """device-timed rotated NMS of one box set resident in HBM: (ms per call, sweep-kernel ms, kept, stats, kept indices
+    of the last call)"""
     import torch
     from orientedreppoints_b200 import _lib
     from orientedreppoints_b200.ops import rnms_indices
@@ -178,7 +201,7 @@ def time_nms(dets_h, local, steps, warm, world, flush, thr=0.1):
         sweep.append(_lib.last_sweep_ms())
     _lib.set_timing(False)
     ms = max_over_ranks(sum(a.elapsed_time(b) for a, b in ev) / steps, world)
-    return ms, float(np.mean(sweep)), int(cnt.item()), _lib.last_nms_stats()
+    return ms, float(np.mean(sweep)), int(cnt.item()), _lib.last_nms_stats(), keep[:int(cnt.item())].cpu().numpy()
 
 
 def nms_sweep(args, rank, world, local, sizes=(10000, 20000, 50000, 100000, 200000)):
@@ -196,7 +219,7 @@ def nms_sweep(args, rank, world, local, sizes=(10000, 20000, 50000, 100000, 2000
     for n in sizes:
         for dense in (False, True):
             d = gen_rotated_boxes(n, seed=100 + rank, extent=1024.0 if dense else const_density_extent(n))
-            ms, sweep_ms, kept, st = time_nms(d, local, 5, 3, world, flush)
+            ms, sweep_ms, kept, st, _ = time_nms(d, local, 5, 3, world, flush)
             pairs = n * (n - 1) / 2.0
             row = {"n": n, "variant": "dense_1024" if dense else "const_density", "ms": ms, "Mpairs_per_s": world * pairs / (ms * 1e-3) / 1e6,
                    "kept": kept, "sweep_kernel_ms": sweep_ms, "pairs_swept": st["pairs_total"], "pairs_aabb": st["pairs_aabb"],
@@ -221,12 +244,6 @@ def nms_sweep(args, rank, world, local, sizes=(10000, 20000, 50000, 100000, 2000
         torch.cuda.synchronize()
         e2e_ms = max_over_ranks((time.perf_counter() - t0) * 1e3 / reps, world)
         pairs = 100000 * 99999 / 2.0
-        traffic = None
-        try:
-            tj = json.load(open(os.path.join(ROOT, "profiles", "r2_nms_traffic_dense100k.json")))
-            traffic = tj                                                  # ncu dram bytes of the kernels of one call
-        except Exception:
-            pass
         out["headline_100k_dense"] = {
             "value": row["Mpairs_per_s"], "unit": "Mpairs/s", "ms": row["ms"], "kept": row["kept"],
             "e2e": {"value": world * pairs / (e2e_ms * 1e-3) / 1e6, "unit": "Mpairs/s", "ms": e2e_ms,
@@ -239,7 +256,7 @@ def nms_sweep(args, rank, world, local, sizes=(10000, 20000, 50000, 100000, 2000
                         "latency and by the divergent clip" % (nms_bitmatrix_bytes(100000) / 1e9),
                 "reference_formulation_bytes": nms_bitmatrix_bytes(100000),
                 "reference_formulation_GBps_equiv": nms_bitmatrix_bytes(100000) / (row["ms"] * 1e-3) / 1e9,
-                "hbm_peak_GBps": pk["hbm_gbs"], "dram_traffic_ncu": traffic,
+                "hbm_peak_GBps": pk["hbm_gbs"],
                 "clip_tflops": row["clip_tflops"], "fp32_peak_tflops_nominal": FP32_PEAK_TFLOPS,
                 "clip_frac_of_fp32_peak": row["clip_tflops"] / FP32_PEAK_TFLOPS}}
     return out
@@ -260,7 +277,9 @@ def run_nms(args, rank, world, local, dense=True):
     if rank == 0:
         sampler.start()
     _lib.reset_launch_count()
-    ms, sweep_avg, kept, stats = time_nms(dets_h, local, args.steps, max(args.warmup, 3), world, flush, thr)
+    ms, sweep_avg, kept, stats, keep_last = time_nms(dets_h, local, args.steps, max(args.warmup, 3), world, flush, thr)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"keep": keep_last})
     launches = _lib.launch_count()
     clocks = sampler.stop() if rank == 0 else None
     pairs = n * (n - 1) / 2.0
@@ -295,7 +314,7 @@ def run_nms(args, rank, world, local, dense=True):
         "roofline": {"bound": "hbm", "kernel": "nms_sweep_kernel", "achieved": None, "peak": pk["hbm_gbs"], "unit": "GB/s",
                      "frac": None, "traffic": None, "peak_source": pk["source"],
                      "note": "HBM is not the binding roof of this formulation (no N^2 bit matrix): see clip_tflops and "
-                             "reference_formulation_GBps_equiv; dram bytes of a call are in profiles/ (ncu)",
+                             "reference_formulation_GBps_equiv",
                      "reference_formulation_bytes": nms_bitmatrix_bytes(n),
                      "reference_formulation_GBps_equiv": nms_bitmatrix_bytes(n) / (ms * 1e-3) / 1e9,
                      "clip_tflops": clip_tf, "clip_frac_of_fp32_peak": clip_tf / FP32_PEAK_TFLOPS,

@@ -1,5 +1,5 @@
 /*
- * orp_b200.h - C ABI of liborp_b200.so: the B200 (sm_100a) implementation of the
+ * orp_b200.h - C ABI of liborp_b200.so: the H100 (sm_90a) implementation of the
  * OrientedRepPoints dense-inference hot path (SURVEY.md section 8).
  *
  * Plain pointers and sizes only - no torch types.  Every entry point cites the reference
@@ -27,7 +27,7 @@ extern "C" {
 #define ORP_OK 0
 #define ORP_EINVAL (-1)   /* bad argument                                  */
 #define ORP_ECUDA (-2)    /* CUDA runtime error (see orp_last_error)        */
-#define ORP_ENOGPU (-3)   /* no sm_100 device / wrong architecture          */
+#define ORP_ENOGPU (-3)   /* no sm_90 device / wrong architecture           */
 #define ORP_EOVERFLOW (-4) /* internal capacity exceeded after retries       */
 
 const char *orp_last_error(void);
@@ -241,7 +241,7 @@ int orp_gn_apply_f32(const float *x, int N, int H, int W, int C, const double *s
 int orp_maxpool3x3s2_f32(const float *x, int N, int H, int W, int C, float *y, void *stream);
 
 /* ------------------------------------------------------------------------------------------
- * Dense layers, bf16 on the 5th-generation tensor cores (tcgen05.mma, fp32 accumulation in TMEM,
+ * Dense layers, bf16 on the Hopper tensor cores (wgmma.mma_async, fp32 accumulation in registers,
  * operands staged by TMA).  Activations NHWC bf16; weights bf16 [Cout_padded][KH*KW*Cin] (K index =
  * (kh*KW + kw)*Cin + ci; rows >= Cout are zero; Cout_padded a multiple of 32).
  * ---------------------------------------------------------------------------------------- */
@@ -274,7 +274,7 @@ int orp_conv2d_bf16(int nprob, const orp_tc_problem *probs, const void *w, int C
  * reference computes nn.Conv2d / DeformConv in fp32 (resnet.py:203-239, fpn.py:138-178,
  * orientedreppoints_head.py:148-171; torch 1.4: no TF32).  Here every fp32 value travels as an fp16
  * pair x = hi + lo (hi = fp16(x), lo = fp16(x - hi): 22 significand bits) and every product is
- * hi*hi + lo*hi + hi*lo: three tcgen05 MMAs into one fp32 TMEM accumulator (dropped lo*lo term 2^-22).
+ * hi*hi + lo*hi + hi*lo: three wgmma MMAs into one fp32 accumulator (dropped lo*lo term 2^-22).
  * Activations: fp16 [N,H,W,2,C] (per pixel: C hi values, then C lo values).  Weights: fp16
  * [Cout_padded][KH*KW][2][Cin_padded to 64] holding (hi, lo) of w * 2^wscale_log2 - the power-of-two
  * scale (0..15, chosen by the caller so the scaled weights have rms ~ 1) keeps the lo halves out of the
@@ -287,7 +287,7 @@ int orp_conv2d_f16x3(int nprob, const orp_tc_problem *probs, const void *w_split
                      int out_f32, int deform, void *stream);
 /* Split-K form of one plain convolution (no residual / deformation) for launches whose 128 x BN tiling leaves most SMs idle
  * (P6: 3x3/2 over 2048 channels on a 16^2 map; layer4 and layer3 at one tile per step): the KH*KW taps are divided into
- * `ksplit` groups (KH*KW % ksplit == 0), every (tile, group) is a CTA-sized unit of the same tcgen05 kernel writing its partial
+ * `ksplit` groups (KH*KW % ksplit == 0), every (tile, group) is a CTA-sized unit of the same wgmma kernel writing its partial
  * sums to its own slab of `workspace` (fp32 [ksplit, N,Ho,Wo,Cout]), and a finishing pass adds the slabs in a fixed order
  * (bit-reproducible), applies bias / ReLU and writes
  * bf16 (f16x3 == 0) or split fp16 (f16x3 != 0) to prob->out (+ GroupNorm statistics when prob->gn_stats is set).  Shorter

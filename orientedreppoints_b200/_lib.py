@@ -1,7 +1,7 @@
 """ctypes binding of liborp_b200.so (include/orp_b200.h).
 
 There is NO fallback: if the shared library is missing or a call fails, an exception is raised.
-The library is built in-tree by `python -m orientedreppoints_b200.build` (nvcc, sm_100a).
+The library is built in-tree by `python -m orientedreppoints_b200.build` (nvcc, sm_90a).
 """
 import ctypes
 import os

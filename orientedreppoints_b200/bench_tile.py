@@ -81,16 +81,20 @@ def build_detector(backbone, precision, dev, reference_init=True):
     return depth, OrientedRepPointsDetector(sd, depth, dev, precision, test_cfg=dict(score_thr=0.0))
 
 
-def _device_steps(det, img, steps, warm, world, flush, benchmod, use_graph, sampler=None):
+def _device_steps(det, img, steps, warm, world, flush, benchmod, use_graph, sampler=None, last_out=None):
     """`steps` device-resident steps (dense graph -> fused post-processing -> packed detections -> all-gather), CUDA events
     around every step, L2 flush between steps.  The collective is asynchronous: step s waits for the gather of step s-1
     (the last step also for its own), so the ranks are not forced into lockstep and the gather overlaps the next step's
-    dense graph.  Returns (ms per step as max over ranks, per-tile detection counts, launches counted by the library)."""
+    dense graph.  Returns (ms per step as max over ranks, per-tile detection counts, launches counted by the library).
+    last_out (dict): receives host copies of what the last timed step returned (dets, labels, counts)."""
     from . import gather as G
     pending = [None]
 
+    outs = [None]
+
     def step(last=False):
         dets, labels, counts = det.simple_test(img, return_tensors="padded")
+        outs[0] = (dets, labels, counts)
         buf, _ = G.pack(dets, labels, counts)
         h = G.all_gather_detections(buf, async_op=True)
         res = pending[0].wait() if pending[0] is not None else None
@@ -120,6 +124,9 @@ def _device_steps(det, img, steps, warm, world, flush, benchmod, use_graph, samp
             _, all_cnt = got
     benchmod.barrier(world)
     launches = _lib.launch_count()
+    if last_out is not None:
+        for k, t in zip(("dets", "labels", "counts"), outs[0]):
+            last_out[k] = t.cpu().numpy()
     total_ms = benchmod.max_over_ranks(sum(a.elapsed_time(b) for a, b in ev), world)
     return total_ms / steps, [int(v) for v in all_cnt.reshape(-1).tolist()], launches
 
@@ -146,7 +153,7 @@ def _roofline_pass(det, img, steps, flush):
     return tc_ms / n, tc_launches // n, tc_flops / n, launches_dense
 
 
-def _roofline_obj(precision, kernel_ms, tc_launches, flops_step, ms_step, pk, batch, fl_tile, traffic=None, traffic_note=None):
+def _roofline_obj(precision, kernel_ms, tc_launches, flops_step, ms_step, pk, batch, fl_tile):
     """`achieved` = ALGORITHMIC flops (2*MACs of the convolutions, no padded / identity / extra-term MMAs) / kernel time.
     The f16x3 mode executes three MMAs per algorithmic product, so its tensor pipe is three times as busy as `frac` says:
     `tensor_pipe_frac` (executed MMA flops / peak) is the utilisation north_star's 70 % target speaks of."""
@@ -155,7 +162,7 @@ def _roofline_obj(precision, kernel_ms, tc_launches, flops_step, ms_step, pk, ba
     return {"bound": "tensor", "kernel": "conv_tc_kernel (all %d launches per step)" % tc_launches,
             "achieved": ach, "peak": pk["bf16_tflops_sustained"], "unit": "TFLOP/s", "frac": ach / pk["bf16_tflops_sustained"],
             "mma_per_product": mult, "executed_tflops": ach * mult, "tensor_pipe_frac": ach * mult / pk["bf16_tflops_sustained"],
-            "traffic": traffic, "traffic_note": traffic_note, "peak_source": pk["source"] + " (sustained, dense bf16/fp16)",
+            "peak_source": pk["source"] + " (sustained, dense bf16/fp16)",
             "algorithmic_flops_per_step": flops_step, "kernel_ms_per_step": kernel_ms,
             "kernel_share_of_step": kernel_ms / ms_step,
             "whole_step_tflops": batch * fl_tile / (ms_step * 1e-3) / 1e12}
@@ -227,8 +234,13 @@ def run(args, rank, world, local, benchmod):
 
     use_graph = not getattr(args, "no_graph", False)
     sampler = benchmod.ClockSampler(local)
+    last_out = {}
     ms_step, ndet, launches = _device_steps(det, img, args.steps, warm, world, flush, benchmod, use_graph,
-                                            sampler=sampler if rank == 0 else None)
+                                            sampler=sampler if rank == 0 else None, last_out=last_out)
+    if getattr(args, "dump_outputs", None) and rank == 0:
+        # the padded per-tile detections [tiles, max_per_img, 27] (8 box corners, 18 reppoint coordinates, score), their
+        # labels [tiles, max_per_img] and counts [tiles]: rows past a tile's count are padding
+        benchmod.dump_outputs(args.dump_outputs, last_out)
     clocks = sampler.stop() if rank == 0 else None
     # roofline pass
     tc_ms, tc_launches, tc_flops, launches_dense = _roofline_pass(det, img, args.steps, flush)
@@ -335,23 +347,12 @@ def run(args, rank, world, local, benchmod):
         "e2e": {"value": world * batch / (e2e_ms * 1e-3), "unit": "tiles/s", "h2d_bytes_per_step": int(img_host.nbytes),
                 "d2h_bytes_per_step": int(d2h), "api": "OrientedRepPointsDetector.simple_test(uint8 HWC tiles) -> rbbox2result lists", "input": "uint8 HWC tiles, Normalize fused into the stem input transform"},
     }
-    traffic, traffic_note = None, None
-    try:
-        import json as _json
-        import os as _os
-        name = "r2_conv_tc_traffic_%s_b%d.json" % (precision, batch)
-        tj = _json.load(open(_os.path.join(_os.path.dirname(_os.path.dirname(_os.path.abspath(__file__))), "profiles", name)))
-        if depth == 50 and batch == tj["tiles"]:
-            traffic = tj["dram_bytes_read"] + tj["dram_bytes_write"]      # ncu, all conv launches of one step (cold L2 per launch)
-            traffic_note = "dram bytes read+written by the same launches under ncu (profiles/%s)" % name
-    except Exception:
-        pass
     if tc_ms > 0:
-        line["roofline"] = _roofline_obj(precision, tc_ms, tc_launches, tc_flops, ms_step, pk, batch, fl_tile, traffic, traffic_note)
+        line["roofline"] = _roofline_obj(precision, tc_ms, tc_launches, tc_flops, ms_step, pk, batch, fl_tile)
     if hasattr(det.eng, "overflow_count"):
         line["f16_overflow_events"] = det.eng.overflow_count()
-    line["parity"] = ("f16x3: every fp32 product as fp16 hi/lo pairs, three tcgen05 MMAs into one fp32 accumulator; dense outputs within "
-                      "1e-4 of the fp64 reference graph at 1024x1024 (tests/test_f16x3_gpu.py, measured 2.4e-5 R-50 / 2.8e-5 R-101)"
+    line["parity"] = ("f16x3: every fp32 product as fp16 hi/lo pairs, three wgmma MMAs into one fp32 accumulator; dense outputs within "
+                      "1e-4 of the fp64 reference graph at 1024x1024 (tests/test_f16x3_gpu.py)"
                       if precision == "f16x3" else "bf16 operands: ~1e-2 of max, NOT the parity arithmetic")
     if clocks is not None:
         line["clocks"] = clocks

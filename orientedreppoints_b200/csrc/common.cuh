@@ -1,5 +1,5 @@
 // common.cuh - error plumbing, launch accounting and stream-ordered scratch memory shared by
-// every translation unit of liborp_b200.so (sm_100a only).
+// every translation unit of liborp_b200.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -35,7 +35,7 @@ inline int fail(int code, const char *fmt, const char *a = "", const char *b = "
 
 inline void count_launches(int n) { __atomic_add_fetch(&g_launches, n, __ATOMIC_RELAXED); }
 
-// one-time per-device setup: refuse anything that is not compute capability 10.x, and keep
+// one-time per-device setup: refuse anything that is not compute capability 9.x, and keep
 // freed scratch in the stream-ordered pool so repeated calls do not hit the driver allocator.
 int ensure_device();
 
@@ -63,5 +63,8 @@ int run_nms(const float *dets, const int32_t *segments, int n, double thr, int i
             int32_t *overflow_out /* optional device int: set to 1 when the candidate list overflowed (no_sync callers) */);
 
 static inline int ceil_div(long long a, long long b) { return (int)((a + b - 1) / b); }
+
+// streaming multiprocessors of an H100 SXM: caps of grid-stride launches are multiples of it
+constexpr int kNumSMs = 132;
 
 }  // namespace orp

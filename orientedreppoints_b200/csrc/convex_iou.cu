@@ -99,7 +99,7 @@ extern "C" int orp_convex_iou(const float *pts18, int n, const float *quads8, in
     const size_t total = (size_t)n * k;
     if (total == 0) return ORP_OK;
     size_t g = (total + 127) / 128;
-    if (g > 148 * 32) g = 148 * 32;
+    if (g > kNumSMs * 32) g = kNumSMs * 32;
     convex_iou_kernel<<<(int)g, 128, 0, static_cast<cudaStream_t>(stream)>>>(pts18, n, quads8, k, out);
     ORP_LAUNCHED();
     return ORP_OK;

@@ -220,7 +220,7 @@ gn_apply_bf16_kernel(const __grid_constant__ GnApplyParams P)
 int grid_for(size_t items, int threads)
 {
     size_t g = (items + threads - 1) / threads;
-    const size_t cap = 148 * 16;
+    const size_t cap = kNumSMs * 16;
     return (int)(g < cap ? (g ? g : 1) : cap);
 }
 
@@ -380,7 +380,7 @@ extern "C" int orp_gn_stats_bf16(const void *x, int N, int HW, int C, int groups
     int rc = ensure_device();
     if (rc) return rc;
     int slabs = ceil_div(HW, 64);
-    const int maxs = (148 * 4 + N - 1) / N;
+    const int maxs = (kNumSMs * 4 + N - 1) / N;
     if (slabs > maxs) slabs = maxs;
     const int slab = ceil_div(HW, slabs);
     slabs = ceil_div(HW, slab);

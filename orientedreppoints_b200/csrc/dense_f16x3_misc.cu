@@ -45,7 +45,7 @@ __device__ __forceinline__ void split8(const float (&v)[8], uint4 &h, uint4 &l)
 int grid_for(size_t items, int threads)
 {
     size_t g = (items + threads - 1) / threads;
-    const size_t cap = 148 * 16;
+    const size_t cap = kNumSMs * 16;
     return (int)(g < cap ? (g ? g : 1) : cap);
 }
 
@@ -398,7 +398,7 @@ extern "C" int orp_gn_stats_f16x3(const void *x, int N, int HW, int C, int group
     int rc = ensure_device();
     if (rc) return rc;
     int slabs = ceil_div(HW, 64);
-    const int maxs = (148 * 4 + N - 1) / N;
+    const int maxs = (kNumSMs * 4 + N - 1) / N;
     if (slabs > maxs) slabs = maxs;
     const int slab = ceil_div(HW, slabs);
     slabs = ceil_div(HW, slab);

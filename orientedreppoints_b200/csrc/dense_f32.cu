@@ -4,7 +4,7 @@
 // fp32 cuDNN/cuBLAS convolutions (mmdet/models/backbones/resnet.py:203-239,495-506,
 // necks/fpn.py:138-178, anchor_heads/orientedreppoints_head.py:148-171) and its deformable im2col +
 // SGEMM (mmdet/ops/dcn/src/deform_conv_cuda_kernel.cu:84-115,190-243, deform_conv_cuda.cpp:152-260).
-// The bf16 tcgen05 kernels in dense_tc.cu compute the same layers on the tensor pipe; tests compare
+// The bf16 wgmma kernels in dense_tc.cu compute the same layers on the tensor pipe; tests compare
 // the two against each other and against a PyTorch fp32 re-declaration of the reference graph.
 //
 // One implicit-GEMM kernel serves ordinary and deformable convolutions: M = output pixels of one
@@ -318,7 +318,7 @@ extern "C" int orp_gn_apply_f32(const float *x, int N, int H, int W, int C, cons
     if (rc) return rc;
     const size_t total4 = (size_t)N * H * W * C / 4;
     int grid = (int)((total4 + 255) / 256);
-    if (grid > 148 * 16) grid = 148 * 16;
+    if (grid > kNumSMs * 16) grid = kNumSMs * 16;
     gn_apply_f32_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(x, N, H, W, C, stats, groups, gamma, beta, eps,
                                                                              relu, up_src, y);
     ORP_LAUNCHED();
@@ -333,7 +333,7 @@ extern "C" int orp_maxpool3x3s2_f32(const float *x, int N, int H, int W, int C, 
     const int Ho = (H + 2 - 3) / 2 + 1, Wo = (W + 2 - 3) / 2 + 1;
     const size_t total4 = (size_t)N * Ho * Wo * C / 4;
     int grid = (int)((total4 + 255) / 256);
-    if (grid > 148 * 16) grid = 148 * 16;
+    if (grid > kNumSMs * 16) grid = kNumSMs * 16;
     maxpool3x3s2_f32_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(x, N, H, W, C, Ho, Wo, y);
     ORP_LAUNCHED();
     return ORP_OK;

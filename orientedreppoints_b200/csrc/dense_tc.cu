@@ -1,4 +1,4 @@
-// dense_tc.cu - tensor-core (tcgen05 / TMEM / TMA) implicit-GEMM convolution for sm_100a, NHWC bf16.
+// dense_tc.cu - tensor-core (wgmma / TMA / mbarrier) implicit-GEMM convolution for sm_90a (H100), NHWC bf16.
 //
 // Replaces the cuDNN convolutions of the reference's backbone / FPN / head towers
 // (mmdet/models/backbones/resnet.py:203-239,495-506; necks/fpn.py:138-178;
@@ -7,34 +7,33 @@
 //
 // GEMM view: D[M = 128 output pixels, N = BN output channels] += A[M, K] * B[N, K]^T with
 // K = taps x Cin walked in 64-channel blocks.  One persistent CTA per SM, warp-specialised:
-//   warp 0      TMA producer: the A tile of one (tap, channel block) is ONE 4-D box {64 ch, BW, BH, BI}
+//   warps 0-7   two consumer warpgroups.  Warpgroup g issues wgmma.mma_async m64nBNk16 x 4 per stage for the
+//               output rows [64 g, 64 g + 64), accumulating fp32 in registers, and releases the stage once the
+//               MMAs that read it have retired.  After the last K block the same warps run the epilogue: the
+//               accumulator is staged in shared memory 64 columns at a time (fp32, one row per pixel), then
+//               bias / residual / ReLU and bf16, split-fp16 or fp32 NHWC stores.
+//   warp 8      TMA producer (plain variant): the A tile of one (tap, channel block) is ONE box {64 ch, BW, BH, BI}
 //               of the NHWC activation (tensor-map element strides = conv stride; out-of-bounds
 //               coordinates are zero-filled by the TMA unit = the convolution's zero padding), landing in
 //               shared memory as 128 rows x 128 B with the 128-byte swizzle - exactly the canonical
-//               K-major operand layout of tcgen05.mma; the B tile is a 2-D box of the [Cout, K] weights.
-//   warp 1      MMA issuer: one elected lane issues tcgen05.mma.cta_group::1.kind::f16 (M=128, N=BN,
-//               K=16) x 4 per stage, accumulating fp32 in TMEM; tcgen05.commit releases the stage and,
-//               after the last K block, publishes the accumulator.
-//   warps 2-5   epilogue: tcgen05.ld (32 lanes x 32 columns), bias / residual / ReLU, bf16 or fp32 NHWC
-//               stores.  TMEM holds two accumulators so the epilogue of tile i overlaps the main loop
-//               of tile i+1.
-//   warps 6-13  (deformable variant only) A-operand producers: per output pixel and tap the 4-corner
+//               K-major operand layout of wgmma; the B tile is a 2-D box of the [Cout, K] weights.
+//   warps 8-15  (deformable variant only) A-operand producers: per output pixel and tap the 4-corner
 //               bilinear sample of the reference (deform_conv_cuda_kernel.cu:84-115) is computed in
-//               fp32 from bf16 features and written to shared memory in the same swizzled layout.
+//               fp32 from bf16 features and written to shared memory in the same swizzled layout; their first
+//               thread also issues the TMA loads of the B tiles.
 // Several "problems" (the five FPN levels, which share the head weights) are served by ONE launch.
 //
 // Two operand modes share the kernel.  bf16: activations / weights rounded to bf16, one MMA per K step.
 // f16x3 ("split"): every fp32 value is carried as an fp16 pair x = hi + lo (22 significand bits, activations
 // stored [N,H,W,2,C]: hi channels then lo channels per pixel) and every product is evaluated as
-// hi*hi + lo*hi + hi*lo with three MMAs into the same fp32 TMEM accumulator (the dropped lo*lo term is 2^-22
+// hi*hi + lo*hi + hi*lo with three MMAs into the same fp32 accumulator (the dropped lo*lo term is 2^-22
 // relative) - fp32-faithful arithmetic at 1/3 of the tensor-pipe rate; this is the parity mode.  The K loop
 // simply runs three "terms" per (tap, channel block); weights are stored [Cout][tap][channel block][2][64] = (hi, lo).
-// A tcgen05.mma with M = 128 takes the same ~100 ns whatever N <= 256 (measured: 87 / 97 / 115 ns at N = 64 / 128 / 256), so
-// layers with 64 or 128 output channels are issue-bound at a quarter / half of the tensor rate.  For those (BN <= 128) the
-// terms are concatenated along N instead of K ("ncat"): per K step  x_hi * [w_hi | w_lo]  is ONE MMA of width 2 BN (main
-// product into accumulator columns [0, BN), cross term into [BN, 2 BN)) and  x_lo * w_hi  a second one into [BN, 2 BN) -
-// two instructions instead of three, the x_hi / x_lo tiles of a (tap, channel block) are loaded once, and the small cross
-// terms own an accumulator (their sum never meets the large main sum before the epilogue adds the two in fp32).
+// For layers with BN <= 128 output channels per tile the terms are concatenated along N instead of K ("ncat"): per K
+// step  x_hi * [w_hi | w_lo]  is ONE MMA of width 2 BN (main product into accumulator columns [0, BN), cross term into
+// [BN, 2 BN)) and  x_lo * w_hi  a second one into [BN, 2 BN) - two instructions instead of three, the x_hi / x_lo tiles
+// of a (tap, channel block) are loaded once, and the small cross terms own an accumulator (their sum never meets the
+// large main sum before the epilogue adds the two in fp32).
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -44,6 +43,7 @@
 #include <unordered_map>
 
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace orp {
 namespace {
@@ -99,7 +99,6 @@ struct alignas(64) TcParams {
     long long ks_stride;                      // elements between the partial-sum slabs of consecutive K splits
     int b_resident;                           // short-K layers: the whole weight slab of this CTA's N tile stays in shared memory
     int res_mma;                              // residual added by the tensor core: extra K blocks  R[128x64] * I[64x64]
-    int epi_split;                            // epilogue-bound layers: the two epilogue warpgroups work on alternate tiles (one per accumulator buffer)
     int gn_fused;                             // GroupNorm statistics accumulated in the TMA epilogue (Cout == 256)
     int dcat;                                 // deformable split mode: one stage = sampled x_hi | x_lo | w_hi | w_lo of a K block
     int stem;                                 // producers build conv1's 7x7/2 im2col rows from the NCHW fp32 image
@@ -169,30 +168,15 @@ __device__ __forceinline__ void tma_load_2d(void *smem, const CUtensorMap *tm, u
         "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
         ::"r"(smem_u32(smem)), "l"(tm), "r"(smem_u32(bar)), "r"(c0), "r"(c1) : "memory");
 }
-__device__ __forceinline__ void tcgen05_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tcgen05_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void umma_commit(uint64_t *bar)
-{
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate)
-{
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}" ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
-}
-// K-major, 128-byte swizzle: start address >> 4, LBO = 1 (ignored), SBO = 1024 B >> 4, version 1, layout 2
+// wgmma matrix descriptor, K-major with the 128-byte swizzle: start address >> 4, LBO = 1 (ignored), SBO = 1024 B >> 4
+// (eight 128-byte rows), layout type 1 = SWIZZLE_128B in bits 62-63.  Operand tiles start on 1024-byte boundaries.
 __device__ __forceinline__ uint64_t make_desc_sw128(uint32_t smem_addr)
 {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
     d |= (uint64_t)1 << 16;
     d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
+    d |= (uint64_t)1 << 62;
     return d;
 }
 __device__ __forceinline__ uint4 lds128(uint32_t addr)
@@ -210,43 +194,19 @@ __device__ __forceinline__ void named_bar()
 {
     asm volatile("bar.sync %0, %1;" ::"n"(ID), "n"(N) : "memory");
 }
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32])
+// 32 consecutive fp32 columns of one staged accumulator row (conflict-free: 16-byte loads, row pitch 68 words)
+__device__ __forceinline__ void acc_ld32(uint32_t addr, uint32_t (&r)[32])
 {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+        const uint4 v = lds128(addr + (uint32_t)j * 16u);
+        r[4 * j] = v.x; r[4 * j + 1] = v.y; r[4 * j + 2] = v.z; r[4 * j + 3] = v.w;
+    }
 }
 
-// split form: issue the load, do independent work, then tmem_ld_wait() before touching the registers
-__device__ __forceinline__ void tmem_ld32_issue(uint32_t taddr, uint32_t (&r)[32])
-{
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait(uint32_t (&r)[32])
-{
-    // the registers are tied to the wait so that no use can be scheduled above it
-    asm volatile("tcgen05.wait::ld.sync.aligned;"
-                 : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]), "+r"(r[8]),
-                   "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15]), "+r"(r[16]),
-                   "+r"(r[17]), "+r"(r[18]), "+r"(r[19]), "+r"(r[20]), "+r"(r[21]), "+r"(r[22]), "+r"(r[23]), "+r"(r[24]),
-                   "+r"(r[25]), "+r"(r[26]), "+r"(r[27]), "+r"(r[28]), "+r"(r[29]), "+r"(r[30]), "+r"(r[31])
-                 :: "memory");
-}
+// two fp32 lanes, each rounded once (sm_90 has no packed fp32 FMA / add)
+__device__ __forceinline__ float2 ffma2_rn(float2 a, float2 b, float2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
+__device__ __forceinline__ float2 fadd2_rn(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
 
 // epilogue activation: 0 none, 1 ReLU, 2 exact (erf) GELU as nn.GELU (swin_transformer.py:24-29)
 __device__ __forceinline__ float act_fn(float v, int act)
@@ -344,22 +304,67 @@ __device__ unsigned int g_f16_overflow = 0;
 // ----------------------------------------------------------------------------------------------- kernel
 // BN: accumulator width (32..256).  OUT_F32: fp32 output (head predictions) instead of bf16.
 constexpr int kStemPatchBytes = 24576;             // conv1's input patch in dynamic shared memory (5632 floats used)
-constexpr int kDP = 256;                           // deformable A-operand producer threads (warps 6 .. 6 + kDP/32 - 1)
+constexpr int kConsumers = 256;                    // two consumer warpgroups: MMA, then epilogue (warps 0-7)
+constexpr int kDP = 256;                           // deformable A-operand producer threads (warps 8 .. 8 + kDP/32 - 1)
 constexpr int kDItems = 1024 / kDP;                // (pixel row, 8-channel chunk) items of one 128 x 64 A block per thread
 constexpr int kDRound = kDItems / 2;               // items gathered together (two rounds per K block)
-// DEFORM: A operand produced by the warps from 6 on (bilinear gather) instead of TMA.
+constexpr int kAccPitch = 68;                      // words per staged accumulator row: 64 columns + 4 (conflict-free 16-byte reads)
+constexpr int kAccBytes = 128 * kAccPitch * 4;     // one 64-column pass of the 128 x BN accumulator, fp32 (34 KiB)
+
+// Columns [64 pass, 64 pass + 64) of this thread's accumulator fragment -> the staged rows (ncat: main + cross columns,
+// added here in fp32 with round-to-nearest).  The pass loop is unrolled with a compile-time index so that the fragment
+// stays in registers.  row0 / col0: the fragment's first row and column (wgmma.cuh).
+template <int BN, int R>
+__device__ __forceinline__ void stage_acc(const float (&acc)[R], int pass, bool ncat, float *s_acc, int row0, int col0)
+{
+    constexpr int kGroups = (BN < 64 ? BN : 64) / 8;         // 8-column groups per pass
+#pragma unroll
+    for (int p = 0; p < (BN + 63) / 64; ++p) {
+        if (p != pass) continue;
+#pragma unroll
+        for (int i = 0; i < kGroups; ++i) {
+            const int g = p * 8 + i;
+            float2 a = make_float2(acc[4 * g], acc[4 * g + 1]), b = make_float2(acc[4 * g + 2], acc[4 * g + 3]);
+            if constexpr (R >= BN) {
+                if (ncat) {                                   // cross columns: BN further on, BN / 2 registers further
+                    a.x += acc[BN / 2 + 4 * g]; a.y += acc[BN / 2 + 4 * g + 1];
+                    b.x += acc[BN / 2 + 4 * g + 2]; b.y += acc[BN / 2 + 4 * g + 3];
+                }
+            }
+            *reinterpret_cast<float2 *>(s_acc + row0 * kAccPitch + i * 8 + col0) = a;
+            *reinterpret_cast<float2 *>(s_acc + (row0 + 8) * kAccPitch + i * 8 + col0) = b;
+        }
+    }
+}
+
+// accumulator columns [64 g, 64 g + 64) += A * B (the residual K blocks: residual tile x identity)
+template <int BN, int R>
+__device__ __forceinline__ void wgmma_cols64(float (&acc)[R], int g, uint64_t da, uint64_t db, bool bf16)
+{
+    if (g == 0) wgmma_n<64>(acc_view<0, 32>(acc), da, db, 1u, bf16);
+    if constexpr (BN >= 128) { if (g == 1) wgmma_n<64>(acc_view<32, 32>(acc), da, db, 1u, bf16); }
+    if constexpr (BN >= 256) {
+        if (g == 2) wgmma_n<64>(acc_view<64, 32>(acc), da, db, 1u, bf16);
+        if (g == 3) wgmma_n<64>(acc_view<96, 32>(acc), da, db, 1u, bf16);
+    }
+}
+
+// DEFORM: A operand produced by the warps from 8 on (bilinear gather) instead of TMA.
 template <int BN, bool OUT_F32, bool DEFORM>
-__global__ void __launch_bounds__(DEFORM ? 192 + kDP : 320, 1)
+__global__ void __launch_bounds__(DEFORM ? kConsumers + kDP : kConsumers + 128, 1)
 conv_tc_kernel(const __grid_constant__ TcParams P, int stages)
 {
-    // warp roles.  plain: 0 TMA | 1 MMA | 2-9 epilogue (two warps per TMEM lane quarter, splitting the columns).
-    // deformable / stem: 0 TMA(B) | 1 MMA | 2-5 epilogue | 6-13 A-operand producers.
-    constexpr int kEpiWarps = DEFORM ? 4 : 8;
-    constexpr int kEpiThreads = kEpiWarps * 32;
-    constexpr int kWG = kEpiWarps / 4;                 // epilogue warps per lane quarter
+    // warp roles.  0-7: consumer warpgroups (wgmma main loop, then epilogue).  plain: 8 TMA producer (9-11 idle).
+    // deformable / stem: 8-15 A-operand producers, their thread 0 also loads the B tiles.
+    constexpr int kEpiThreads = kConsumers;
+    constexpr int kWG = 2;                             // epilogue warps per 32-row quarter (one per 32-column half)
+    // accumulator columns per thread group: the ncat layout (BN <= 128) keeps main | cross columns side by side
+    constexpr int kAccN = (!DEFORM && BN <= 128) ? 2 * BN : BN;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
-    // dynamic: [stages][A 16K | B BN*128]  then the epilogue staging tile [128 rows][HC*2 + 16 B]
+    // dynamic: [staged accumulator pass][identity][stem patch][resident B][stages: A 16K | B BN*128] then the output staging tile
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    float *s_acc = reinterpret_cast<float *>(smem);
+    smem += kAccBytes;
     constexpr int kBBytes = BN * kBK * 2;
     // b_resident: [B slab: kblocks x kBBytes] then A-only stages; otherwise every stage carries A | B
     const int kStageBytes = (P.ncat || P.dcat) ? (P.b_resident ? 2 * kABytes : 2 * kABytes + 2 * kBBytes)
@@ -374,124 +379,61 @@ conv_tc_kernel(const __grid_constant__ TcParams P, int stages)
     constexpr int HC = BN < 64 ? BN : 64;              // columns staged per epilogue pass
     constexpr int kPitch = HC * 2 + 16;                // bytes per staged row (+16: conflict-free 16-byte accesses)
     uint8_t *stage_out = smem + (size_t)stages * kStageBytes;
-    __shared__ uint64_t bars[2 * kStagesMax + 4];
-    __shared__ __align__(16) float s_bias_all[2][256];
+    __shared__ uint64_t bars[2 * kStagesMax];
+    __shared__ __align__(16) float s_bias[256];
     __shared__ uint64_t bres_bar;                // resident weight slab landed
-    __shared__ uint32_t tmem_slot_s;
     uint64_t *full = bars;                       // [stages]  TMA bytes landed (+ producer arrivals when DEFORM)
-    uint64_t *empty = bars + kStagesMax;         // [stages]  MMA finished reading the stage
-    uint64_t *tfull = bars + 2 * kStagesMax;     // [2] accumulator ready
-    uint64_t *tempty = tfull + 2;                // [2] accumulator drained
-    uint32_t *tmem_slot = &tmem_slot_s;
+    uint64_t *empty = bars + kStagesMax;         // [stages]  both consumer warpgroups' MMAs finished reading the stage
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    // two accumulator buffers; BN <= 128 leaves room for the ncat layout (main | cross columns per buffer)
-    constexpr uint32_t kAccCols = BN <= 128 ? 4 * BN : 2 * BN;
-    constexpr uint32_t kTmemCols = (kAccCols <= 32) ? 32 : (kAccCols <= 64) ? 64 : (kAccCols <= 128) ? 128 : (kAccCols <= 256) ? 256 : 512;
 
-    if (warp == 0 && elect_one()) {
+    if (warp == kConsumers / 32 && elect_one()) {
+        if (!DEFORM) {
 #pragma unroll 1
-        for (int p = 0; p < P.nprob; ++p)
-            asm volatile("prefetch.tensormap [%0];" ::"l"(&P.tmA[p]) : "memory");
+            for (int p = 0; p < P.nprob; ++p)
+                asm volatile("prefetch.tensormap [%0];" ::"l"(&P.tmA[p]) : "memory");
+        }
         asm volatile("prefetch.tensormap [%0];" ::"l"(&P.tmB) : "memory");
     }
-    if (warp == 1) {
+    if (warp == 0) {
         if (elect_one()) {
             for (int s = 0; s < stages; ++s) {
                 mbar_init(&full[s], DEFORM ? 1 + (P.stem ? 8 : kDP / 32) : 1);          // TMA expect_tx arrival (+ one arrival per producer warp)
-                mbar_init(&empty[s], 1);
+                mbar_init(&empty[s], kConsumers / 128);                                 // one arrival per consumer warpgroup
             }
-            for (int a = 0; a < 2; ++a) { mbar_init(&tfull[a], 1); mbar_init(&tempty[a], (kWG == 2 && P.epi_split) ? 4 : kEpiWarps); }
             mbar_init(&bres_bar, 1);
             asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         }
         __syncwarp();
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(kTmemCols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
     }
-    tcgen05_fence_before();
     __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     const int taps_per = (P.KH * P.KW) / (P.ksplit > 1 ? P.ksplit : 1);              // taps of one K split
     const int kblocks = taps_per * P.cin_blocks * ((P.split && !P.ncat && !P.dcat) ? 3 : 1);     // main-loop K blocks (stages) per tile
-    // Programmatic dependent launch: the next kernel in the stream may start its CTAs (barrier init, TMEM allocation,
-    // descriptor prefetch - the code above) on SMs this grid has already left; nothing above touches global memory,
+    // Programmatic dependent launch: the next kernel in the stream may start its CTAs (barrier init, descriptor
+    // prefetch - the code above) on SMs this grid has already left; nothing above touches global memory,
     // and everything below (loads AND stores) comes after the wait for the preceding grid to complete and flush.
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
     asm volatile("griddepcontrol.wait;" ::: "memory");
 
-    if (warp == 0) {
-        // ===================================================== TMA producer
-        if (elect_one()) {
-            Ring r(stages);
-            if ((P.b_resident || P.res_mma) && (int)blockIdx.x < P.num_tiles) {
-                // gridDim.x is a multiple of n_tiles_n, so every tile of this CTA has the same N tile
-                const int nt0 = blockIdx.x % P.n_tiles_n;
-                mbar_expect_tx(&bres_bar, (uint32_t)((P.b_resident ? kblocks_all * kBBytes : 0) + (P.res_mma ? 8192 : 0)));   // kblocks_all counts weight blocks
-                if (P.res_mma) tma_load_2d(ident, &P.tmI, &bres_bar, 0, 0);
-                if (P.b_resident)
-                    for (int kb = 0; kb < kblocks_all; ++kb)
-                        tma_load_2d(bres + (size_t)kb * kBBytes, &P.tmB, &bres_bar, kb * kBK, nt0 * BN);
-            }
-            const int wterms = P.split ? 2 : 1, rterms = P.split ? 2 : 1;
-            for (int tile = blockIdx.x; tile < P.num_tiles; tile += gridDim.x) {
-                int pi, wb, hb, ib, nt;
-                decode_tile(P, tile, pi, wb, hb, ib, nt);
-                const Problem &pr = P.prob[pi];
-                const int w0 = wb * pr.BW * P.stride - P.pad, h0 = hb * pr.BH * P.stride - P.pad, i0 = ib * pr.BI;
-                const int tap_lo = ksplit_of(P, tile) * taps_per;
-                KIter it(tap_lo + taps_per, P.cin_blocks, (P.split && !P.ncat && !P.dcat) ? 1 : 0, tap_lo);
-                for (int j = 0; j < kblocks; ++j, it.next()) {
-                    const int kh = it.tap / P.KW, kw = it.tap - kh * P.KW;
-                    mbar_wait(&empty[r.stage], r.phase ^ 1);
-                    uint8_t *sa = smem + (size_t)r.stage * kStageBytes;
-                    const int wblk = ((it.tap * P.cin_blocks + it.cb) * wterms) * kBK;      // K offset of the (hi, lo) weight blocks
-                    if (P.ncat || P.dcat) {
-                        // one stage = x_hi tile | x_lo tile | w_hi block | w_lo block of this (tap, channel block); the
-                        // deformable variant's x halves come from the producer warps
-                        mbar_expect_tx(&full[r.stage], (DEFORM ? 0 : 2 * kABytes) + (P.b_resident ? 0 : 2 * kBBytes));
-                        if (!DEFORM) {
-                            tma_load_5d(sa, &P.tmA[pi], &full[r.stage], it.cb * kBK, 0, w0 + kw, h0 + kh, i0);
-                            tma_load_5d(sa + kABytes, &P.tmA[pi], &full[r.stage], it.cb * kBK, 1, w0 + kw, h0 + kh, i0);
-                        }
-                        if (!P.b_resident) {
-                            tma_load_2d(sa + 2 * kABytes, &P.tmB, &full[r.stage], wblk, nt * BN);
-                            tma_load_2d(sa + 2 * kABytes + kBBytes, &P.tmB, &full[r.stage], wblk + kBK, nt * BN);
-                        }
-                    } else {
-                        mbar_expect_tx(&full[r.stage], DEFORM ? kBBytes : (P.b_resident ? kABytes : kABytes + kBBytes));
-                        if (!DEFORM) tma_load_5d(sa, &P.tmA[pi], &full[r.stage], it.cb * kBK, it.term == 1 ? 1 : 0, w0 + kw, h0 + kh, i0);
-                        if (!P.b_resident)
-                            tma_load_2d(sa + kABytes, &P.tmB, &full[r.stage], wblk + (it.term == 2 ? kBK : 0), nt * BN);
-                    }
-                    r.next();
-                }
-                if (!DEFORM && P.res_mma) {
-                    // residual: one extra K block per 64 output channels (two in split mode: hi and lo), the A operand
-                    // is the residual tile itself
-                    for (int g = 0; g < BN / 64 && nt * BN + g * 64 < P.Cout; ++g)
-                        for (int t = 0; t < rterms; ++t) {
-                            mbar_wait(&empty[r.stage], r.phase ^ 1);
-                            mbar_expect_tx(&full[r.stage], kABytes);
-                            tma_load_5d(smem + (size_t)r.stage * kStageBytes, &P.tmRes[pi], &full[r.stage], nt * BN + g * 64, t,
-                                        wb * pr.BW, hb * pr.BH, ib * pr.BI);
-                            r.next();
-                        }
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // ===================================================== MMA issuer
-        // instruction descriptor: D fp32 (bit 4), A/B format (bits 7-9 / 10-12: 0 = fp16, 1 = bf16), N >> 3, M >> 4
-        const uint32_t fmt = P.split ? 0u : 1u;
-        const uint32_t idesc = (1u << 4) | (fmt << 7) | (fmt << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(kBM >> 4) << 24);
-        const uint32_t idesc64 = (1u << 4) | (fmt << 7) | (fmt << 10) | ((uint32_t)(64 >> 3) << 17) | ((uint32_t)(kBM >> 4) << 24);
-        const uint32_t idesc2 = (1u << 4) | (fmt << 7) | (fmt << 10) | ((uint32_t)((2 * BN > 256 ? 256 : 2 * BN) >> 3) << 17) | ((uint32_t)(kBM >> 4) << 24);   // N = 2 BN (ncat)
-        Ring r(stages);
-        int acc = 0;
-        uint32_t acc_phase = 0;
+    if (warp < kConsumers / 32) {
+        // ===================================================== consumers: main loop
+        const int cw = warp >> 2;                          // consumer warpgroup: accumulator rows [64 cw, 64 cw + 64)
+        const uint32_t a_off = (uint32_t)cw * 8192u;       // its 64 rows of a 128-row A tile (64 x 128 B)
+        const bool leader = (threadIdx.x & 127) == 0;
+        const bool bf16 = !P.split;
         const int wterms = P.split ? 2 : 1, rterms = P.split ? 2 : 1;
+        float acc[kAccN / 2];
+        Ring r(stages);
+        // epilogue geometry: thread -> staged row rrow = q * 32 + lane, 32-column half wg of every 64-column pass
+        const int q = warp & 3, wg = warp >> 2;
+        const int et = threadIdx.x, nthr = kEpiThreads;
+        const int bar_a = 1, bar_b = 3;                    // named barriers of the consumers; 2 = deformable producers
+        const int ch0 = wg, chs = kWG;
+        const int frow = cw * 64 + (warp & 3) * 16 + (lane >> 2), fcol = 2 * (lane & 3);   // fragment's first row / column
+        const uint32_t s_acc_u = smem_u32(s_acc);
+        auto bar_sync = [](int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); };
+        int ob = 0;                                        // staging ring position (TMA epilogue)
+        int bias_nt = -1;                                  // N tile whose bias slice is staged in s_bias
         if ((P.b_resident || P.res_mma) && (int)blockIdx.x < P.num_tiles) mbar_wait(&bres_bar, 0);
         for (int tile = blockIdx.x; tile < P.num_tiles; tile += gridDim.x) {
             int res_groups = 0;
@@ -499,89 +441,73 @@ conv_tc_kernel(const __grid_constant__ TcParams P, int stages)
                 const int nt = tile - (int)P.fd_ntn.div((uint32_t)tile) * P.n_tiles_n;
                 for (int g = 0; g < BN / 64 && nt * BN + g * 64 < P.Cout; ++g) ++res_groups;
             }
-            mbar_wait(&tempty[acc], acc_phase ^ 1);
-            tcgen05_fence_after();
-            const uint32_t accw = P.ncat ? 2u * BN : (uint32_t)BN;          // TMEM columns of one accumulator buffer
-            const uint32_t d_tmem = tmem_base + (uint32_t)acc * accw;
             const int tap_lo = ksplit_of(P, tile) * taps_per;
             KIter it(tap_lo + taps_per, P.cin_blocks, (P.split && !P.ncat && !P.dcat) ? 1 : 0, tap_lo);   // same walk as the producer
+            // A stage is released once the MMAs reading it have retired: with one commit group in flight, the stage
+            // before the current one.
+            int held = -1;
+            auto release = [&](int next) {
+                if (held >= 0 && leader) mbar_arrive(&empty[held]);
+                held = next;
+            };
             for (int kb = 0; kb < kblocks; ++kb, it.next()) {
                 mbar_wait(&full[r.stage], r.phase);
-                tcgen05_fence_after();
-                if (elect_one()) {
-                    const uint32_t sa = smem_u32(smem + (size_t)r.stage * kStageBytes);
-                    const uint64_t da = make_desc_sw128(sa);
-                    const int slab = (it.tap * P.cin_blocks + it.cb) * wterms + (it.term == 2 ? 1 : 0);
-                    if (P.ncat) {
+                const uint32_t sa = smem_u32(smem + (size_t)r.stage * kStageBytes);
+                const uint64_t da = make_desc_sw128(sa + a_off);
+                const int slab = (it.tap * P.cin_blocks + it.cb) * wterms + (it.term == 2 ? 1 : 0);
+                wgmma_fence();
+                if (P.ncat) {
+                    if constexpr (kAccN == 2 * BN) {
                         // [w_hi | w_lo] are adjacent in the stage (and in the resident slab): one operand of 2 BN rows
-                        const uint64_t dl = make_desc_sw128(sa + kABytes);
+                        const uint64_t dl = make_desc_sw128(sa + kABytes + a_off);
                         const uint64_t db = make_desc_sw128(P.b_resident ? smem_u32(bres + (size_t)slab * kBBytes) : sa + 2 * kABytes);
 #pragma unroll
                         for (int k = 0; k < kBK / 16; ++k) {
-                            umma_bf16(d_tmem, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), idesc2, (kb | k) ? 1u : 0u);        // x_hi * [w_hi | w_lo]
-                            umma_bf16(d_tmem + (uint32_t)BN, dl + (uint64_t)(k * 2), db + (uint64_t)(k * 2), idesc, 1u);          // x_lo * w_hi -> cross columns
+                            wgmma_n<2 * BN>(acc, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (kb | k) ? 1u : 0u, bf16);   // x_hi * [w_hi | w_lo]
+                            wgmma_n<BN>(acc_view<BN / 2, BN / 2>(acc), dl + (uint64_t)(k * 2), db + (uint64_t)(k * 2), 1u, bf16);  // x_lo * w_hi -> cross columns
                         }
-                    } else if (P.dcat) {
-                        const uint64_t dl = make_desc_sw128(sa + kABytes);
-                        const uint64_t dbh = make_desc_sw128(sa + 2 * kABytes), dbl = make_desc_sw128(sa + 2 * kABytes + kBBytes);
-#pragma unroll
-                        for (int k = 0; k < kBK / 16; ++k) {
-                            umma_bf16(d_tmem, dl + (uint64_t)(k * 2), dbh + (uint64_t)(k * 2), idesc, (kb | k) ? 1u : 0u);   // x_lo * w_hi
-                            umma_bf16(d_tmem, da + (uint64_t)(k * 2), dbl + (uint64_t)(k * 2), idesc, 1u);                   // x_hi * w_lo
-                            umma_bf16(d_tmem, da + (uint64_t)(k * 2), dbh + (uint64_t)(k * 2), idesc, 1u);                   // x_hi * w_hi
-                        }
-                    } else {
-                        const uint64_t db = make_desc_sw128(P.b_resident ? smem_u32(bres + (size_t)slab * kBBytes) : sa + kABytes);
-#pragma unroll
-                        for (int k = 0; k < kBK / 16; ++k)
-                            umma_bf16(d_tmem, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), idesc, (kb | k) ? 1u : 0u);
                     }
-                    umma_commit(&empty[r.stage]);
-                    if (kb == kblocks - 1 && res_groups == 0) umma_commit(&tfull[acc]);
-                }
-                __syncwarp();
-                r.next();
-            }
-            for (int g = 0; g < res_groups * rterms; ++g) {
-                // accumulator columns [64 g, 64 g + 64) += residual tile * (scaled) identity
-                mbar_wait(&full[r.stage], r.phase);
-                tcgen05_fence_after();
-                if (elect_one()) {
-                    const uint64_t da = make_desc_sw128(smem_u32(smem + (size_t)r.stage * kStageBytes));
-                    const uint64_t db = make_desc_sw128(smem_u32(ident));
+                } else if (P.dcat) {
+                    const uint64_t dl = make_desc_sw128(sa + kABytes + a_off);
+                    const uint64_t dbh = make_desc_sw128(sa + 2 * kABytes), dbl = make_desc_sw128(sa + 2 * kABytes + kBBytes);
+#pragma unroll
+                    for (int k = 0; k < kBK / 16; ++k) {
+                        wgmma_n<BN>(acc_view<0, BN / 2>(acc), dl + (uint64_t)(k * 2), dbh + (uint64_t)(k * 2), (kb | k) ? 1u : 0u, bf16);   // x_lo * w_hi
+                        wgmma_n<BN>(acc_view<0, BN / 2>(acc), da + (uint64_t)(k * 2), dbl + (uint64_t)(k * 2), 1u, bf16);                   // x_hi * w_lo
+                        wgmma_n<BN>(acc_view<0, BN / 2>(acc), da + (uint64_t)(k * 2), dbh + (uint64_t)(k * 2), 1u, bf16);                   // x_hi * w_hi
+                    }
+                } else {
+                    const uint64_t db = make_desc_sw128(P.b_resident ? smem_u32(bres + (size_t)slab * kBBytes) : sa + kABytes);
 #pragma unroll
                     for (int k = 0; k < kBK / 16; ++k)
-                        umma_bf16(d_tmem + (uint32_t)((g / rterms) * 64), da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), idesc64, 1u);
-                    umma_commit(&empty[r.stage]);
-                    if (g == res_groups * rterms - 1) umma_commit(&tfull[acc]);
+                        wgmma_n<BN>(acc_view<0, BN / 2>(acc), da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (kb | k) ? 1u : 0u, bf16);
                 }
-                __syncwarp();
+                wgmma_commit();
+                wgmma_wait<1>();
+                release(r.stage);
                 r.next();
             }
-            if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-        }
-    } else if (warp < 2 + kEpiWarps) {
-        // ===================================================== epilogue (TMEM lane quarter = warp % 4)
-        const int q = warp & 3;
-        const int wg = (warp - 2) >> 2;                    // epilogue warpgroup (0 or 1)
-        // Two ways to use eight epilogue warps.  Default: both warpgroups work on the same tile, each warp owning one
-        // 32-column half of a 64-column pass.  Split (epilogue-bound layers): the warpgroups are independent, group g
-        // drains accumulator buffer g (= every second tile of this CTA) with its own staging tiles, barriers and bias
-        // copy, so the fixed latencies of one group's pass (barriers, TMEM load, store issue) overlap the other's.
-        const bool split = (kWG == 2) && P.epi_split;
-        const int grp = split ? wg : 0;
-        const int et = split ? ((threadIdx.x - 64) & 127) : (threadIdx.x - 64);   // thread index inside the group
-        const int nthr = split ? 128 : kEpiThreads;
-        const int bar_a = 1 + 3 * grp, bar_b = 3 + 2 * grp;                     // named barriers (1,3) / (4,5); 2 = producers
-        const int ch0 = split ? 0 : wg, chs = split ? 1 : kWG;
-        float *s_bias = s_bias_all[grp];
-        auto bar_sync = [](int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); };
-        int ob = 0;                                        // staging ring position (TMA epilogue)
-        int bias_nt = -1;                                  // N tile whose bias slice is staged in s_bias
-        int acc = split ? wg : 0;
-        uint32_t acc_phase = 0;
-        for (int tile = blockIdx.x + (split ? wg * (int)gridDim.x : 0); tile < P.num_tiles;
-             tile += (split ? 2 : 1) * (int)gridDim.x) {
+            if constexpr (!DEFORM && BN >= 64) {
+                for (int g = 0; g < res_groups * rterms; ++g) {
+                    // accumulator columns [64 g', 64 g' + 64) += residual tile * (scaled) identity, g' = g / rterms
+                    mbar_wait(&full[r.stage], r.phase);
+                    const uint64_t da = make_desc_sw128(smem_u32(smem + (size_t)r.stage * kStageBytes) + a_off);
+                    const uint64_t db = make_desc_sw128(smem_u32(ident));
+                    wgmma_fence();
+#pragma unroll
+                    for (int k = 0; k < kBK / 16; ++k)
+                        wgmma_cols64<BN>(acc, g / rterms, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), bf16);
+                    wgmma_commit();
+                    wgmma_wait<1>();
+                    release(r.stage);
+                    r.next();
+                }
+            }
+            wgmma_wait<0>();
+            wgmma_fence_acc(acc);
+            release(-1);
+
+            // ===================================================== epilogue
             int pi, wb, hb, ib, nt;
             decode_tile(P, tile, pi, wb, hb, ib, nt);
             const Problem &pr = P.prob[pi];
@@ -595,14 +521,17 @@ conv_tc_kernel(const __grid_constant__ TcParams P, int stages)
             size_t pix;
             const bool valid = row_pixel(rrow, pix);
             if (OUT_F32) {
-                // small fp32 outputs (head predictions, Cout <= 32): straight from registers
-                mbar_wait(&tfull[acc], acc_phase);
-                tcgen05_fence_after();
+                // fp32 outputs (head predictions, split-K partial sums): straight from the staged rows
 #pragma unroll 1
-                for (int ch = wg; ch < BN / 32; ch += kWG) {
+                for (int pass = 0; pass < BN / HC; ++pass) {
+                bar_sync(bar_a, nthr);                               // the previous pass's reads of the staged rows are done
+                stage_acc<BN>(acc, pass, false, s_acc, frow, fcol);
+                bar_sync(bar_a, nthr);
+#pragma unroll 1
+                for (int ch = wg; ch < HC / 32; ch += kWG) {
                     uint32_t v[32];
-                    tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * BN + ch * 32), v);
-                    const int c0 = nt * BN + ch * 32;
+                    acc_ld32(s_acc_u + (uint32_t)(rrow * kAccPitch + ch * 32) * 4u, v);
+                    const int c0 = nt * BN + pass * HC + ch * 32;
                     if (valid && c0 < P.Cout) {
                         float *op = reinterpret_cast<float *>(pr.out) + pix * P.Cout + c0;
                         const float *rp = pr.res32 ? pr.res32 + pix * P.Cout + c0 : nullptr;
@@ -627,18 +556,19 @@ conv_tc_kernel(const __grid_constant__ TcParams P, int stages)
                         }
                     }
                 }
+                }
             } else if (P.tma_epi) {
                 // bf16 outputs through the TMA unit, in 64-channel passes: results go to a 128-byte-swizzled staging
                 // tile and leave with cp.async.bulk.tensor (coalescing and partial-tile clipping by hardware).  A
-                // residual is already in the accumulator (added by the tensor core, see the MMA warp).
-                // With eight epilogue warps each warp owns one 32-column half of the pass.
+                // residual is already in the accumulator (added by the tensor core, see the main loop).
+                // Each of the two warps of a row quarter owns one 32-column half of the pass.
                 const uint32_t slot = P.epi_merge ? 32768u : 16384u;     // a staging slot: one 16 KiB tile (hi | lo when merged)
-                const uint32_t obuf_u = smem_u32(stage_out) + (uint32_t)(grp * P.epi_bufs) * slot;   // [epi_bufs][slot] per group
+                const uint32_t obuf_u = smem_u32(stage_out);             // [epi_bufs][slot]
                 const uint32_t bias_u = smem_u32(s_bias);
                 const bool io = (et == 0);
                 constexpr int kPasses = BN / 64;
                 // split mode: a hi pass and a lo pass per 64 columns (compute-bound layers: one 16 KiB staging tile), or both
-                // halves in one pass (memory-bound layers: half the TMEM reads, barriers and fp32 work per output value)
+                // halves in one pass (memory-bound layers: half the staged-row reads, barriers and fp32 work per output value)
                 const int oterms = (P.split && !P.epi_merge) ? 2 : 1;
                 if (nt != bias_nt) {                                     // bias slice changes only with the N tile
                     bar_sync(bar_a, nthr);                               // previous tile's bias reads are done
@@ -653,39 +583,28 @@ conv_tc_kernel(const __grid_constant__ TcParams P, int stages)
                         if (P.epi_bufs == 2) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
                         else asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
                     }
-                    bar_sync(bar_a, nthr);                               // staging buffer `ob` is free, bias staged
-                    if (pass == 0) {
-                        mbar_wait(&tfull[acc], acc_phase);
-                        tcgen05_fence_after();
+                    bar_sync(bar_a, nthr);                               // staging buffer `ob` is free, bias staged, staged rows read
+                    if (oterm == 0) {                                    // the lo pass of a half reads the rows its hi pass staged
+                        stage_acc<BN>(acc, half, P.ncat != 0, s_acc, frow, fcol);
+                        bar_sync(bar_a, nthr);
                     }
                     float gn_s = 0.f, gn_q = 0.f;
                     const uint32_t orow = obuf_u + (uint32_t)ob * slot + (uint32_t)rrow * 128u;
 #pragma unroll 1
                     for (int ch = ch0; ch < 2; ch += chs) {
-                        uint32_t v[32];
-                        const uint32_t accw = P.ncat ? 2u * BN : (uint32_t)BN;
-                        const uint32_t tcol = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)acc * accw + (uint32_t)(half * 64 + ch * 32);
-                        tmem_ld32_issue(tcol, v);
-                        // bias slice of these 32 columns: eight back-to-back shared loads, in flight with the TMEM load
-                        uint4 bu[8];
-#pragma unroll
-                        for (int j8 = 0; j8 < 8; ++j8) bu[j8] = lds128(bias_u + (uint32_t)(half * 64 + ch * 32 + j8 * 4) * 4u);
-                        tmem_ld_wait(v);
-                        if (P.ncat) {
-                            // main + cross accumulators meet here, in fp32 with round-to-nearest
-                            uint32_t vc[32];
-                            tmem_ld32(tcol + (uint32_t)BN, vc);
-#pragma unroll
-                            for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(__uint_as_float(v[j]) + __uint_as_float(vc[j]));
-                        }
+                        const uint32_t arow = s_acc_u + (uint32_t)(rrow * kAccPitch + ch * 32) * 4u;
 #pragma unroll
                         for (int j4 = 0; j4 < 4; ++j4) {
                             const int c16 = ch * 4 + j4;                  // 16-byte chunk inside the 128-byte row
                             const uint32_t sw = (uint32_t)(c16 ^ (rrow & 7)) << 4;
+                            const uint4 a0 = lds128(arow + (uint32_t)j4 * 32u), a1 = lds128(arow + (uint32_t)j4 * 32u + 16u);
+                            const float f0[8] = {__uint_as_float(a0.x), __uint_as_float(a0.y), __uint_as_float(a0.z), __uint_as_float(a0.w),
+                                                 __uint_as_float(a1.x), __uint_as_float(a1.y), __uint_as_float(a1.z), __uint_as_float(a1.w)};
                             float f[8];
 #pragma unroll
-                            for (int j = 0; j < 8; ++j) f[j] = __uint_as_float(v[j4 * 8 + j]);
-                            const uint4 b0 = bu[2 * j4], b1 = bu[2 * j4 + 1];
+                            for (int j = 0; j < 8; ++j) f[j] = f0[j];
+                            const uint32_t bb = bias_u + (uint32_t)(half * 64 + ch * 32 + j4 * 8) * 4u;
+                            const uint4 b0 = lds128(bb), b1 = lds128(bb + 16u);
                             if (P.split) {
 #pragma unroll
                                 for (int j = 0; j < 8; ++j) f[j] *= P.oscale;      // exact: power of two
@@ -796,18 +715,13 @@ conv_tc_kernel(const __grid_constant__ TcParams P, int stages)
                         }
                         asm volatile("cp.async.commit_group;" ::: "memory");
                     }
-                    if (half == 0) {
-                        mbar_wait(&tfull[acc], acc_phase);
-                        tcgen05_fence_after();
-                    }
-                    if (pr.res && vec_ok) {
-                        asm volatile("cp.async.wait_group 0;" ::: "memory");
-                        named_bar<1, kEpiThreads>();
-                    }
+                    if (pr.res && vec_ok) asm volatile("cp.async.wait_group 0;" ::: "memory");
+                    stage_acc<BN>(acc, half, false, s_acc, frow, fcol);
+                    named_bar<1, kEpiThreads>();                         // residual tile and accumulator pass staged
 #pragma unroll 1
                     for (int ch = wg; ch < HC / 32; ch += kWG) {
                         uint32_t v[32];
-                        tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * BN + half * HC + ch * 32), v);
+                        acc_ld32(s_acc_u + (uint32_t)(rrow * kAccPitch + ch * 32) * 4u, v);
                         const int c0 = cbase + ch * 32;
                         uint4 *sp = reinterpret_cast<uint4 *>(stage_out + (size_t)rrow * kPitch + ch * 64);
 #pragma unroll
@@ -867,15 +781,67 @@ conv_tc_kernel(const __grid_constant__ TcParams P, int stages)
                     named_bar<1, kEpiThreads>();
                 }
             }
-            tcgen05_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&tempty[acc]);
-            if (split) acc_phase ^= 1;                       // this group always drains the same accumulator buffer
-            else if (++acc == 2) { acc = 0; acc_phase ^= 1; }
         }
         if (P.tma_epi && et == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // stores drained before exit
+    } else if (!DEFORM) {
+        // ===================================================== TMA producer
+        if (warp == kConsumers / 32 && elect_one()) {
+            Ring r(stages);
+            if ((P.b_resident || P.res_mma) && (int)blockIdx.x < P.num_tiles) {
+                // gridDim.x is a multiple of n_tiles_n, so every tile of this CTA has the same N tile
+                const int nt0 = blockIdx.x % P.n_tiles_n;
+                mbar_expect_tx(&bres_bar, (uint32_t)((P.b_resident ? kblocks_all * kBBytes : 0) + (P.res_mma ? 8192 : 0)));   // kblocks_all counts weight blocks
+                if (P.res_mma) tma_load_2d(ident, &P.tmI, &bres_bar, 0, 0);
+                if (P.b_resident)
+                    for (int kb = 0; kb < kblocks_all; ++kb)
+                        tma_load_2d(bres + (size_t)kb * kBBytes, &P.tmB, &bres_bar, kb * kBK, nt0 * BN);
+            }
+            const int wterms = P.split ? 2 : 1, rterms = P.split ? 2 : 1;
+            for (int tile = blockIdx.x; tile < P.num_tiles; tile += gridDim.x) {
+                int pi, wb, hb, ib, nt;
+                decode_tile(P, tile, pi, wb, hb, ib, nt);
+                const Problem &pr = P.prob[pi];
+                const int w0 = wb * pr.BW * P.stride - P.pad, h0 = hb * pr.BH * P.stride - P.pad, i0 = ib * pr.BI;
+                const int tap_lo = ksplit_of(P, tile) * taps_per;
+                KIter it(tap_lo + taps_per, P.cin_blocks, (P.split && !P.ncat && !P.dcat) ? 1 : 0, tap_lo);
+                for (int j = 0; j < kblocks; ++j, it.next()) {
+                    const int kh = it.tap / P.KW, kw = it.tap - kh * P.KW;
+                    mbar_wait(&empty[r.stage], r.phase ^ 1);
+                    uint8_t *sa = smem + (size_t)r.stage * kStageBytes;
+                    const int wblk = ((it.tap * P.cin_blocks + it.cb) * wterms) * kBK;      // K offset of the (hi, lo) weight blocks
+                    if (P.ncat || P.dcat) {
+                        // one stage = x_hi tile | x_lo tile | w_hi block | w_lo block of this (tap, channel block)
+                        mbar_expect_tx(&full[r.stage], 2 * kABytes + (P.b_resident ? 0 : 2 * kBBytes));
+                        tma_load_5d(sa, &P.tmA[pi], &full[r.stage], it.cb * kBK, 0, w0 + kw, h0 + kh, i0);
+                        tma_load_5d(sa + kABytes, &P.tmA[pi], &full[r.stage], it.cb * kBK, 1, w0 + kw, h0 + kh, i0);
+                        if (!P.b_resident) {
+                            tma_load_2d(sa + 2 * kABytes, &P.tmB, &full[r.stage], wblk, nt * BN);
+                            tma_load_2d(sa + 2 * kABytes + kBBytes, &P.tmB, &full[r.stage], wblk + kBK, nt * BN);
+                        }
+                    } else {
+                        mbar_expect_tx(&full[r.stage], P.b_resident ? kABytes : kABytes + kBBytes);
+                        tma_load_5d(sa, &P.tmA[pi], &full[r.stage], it.cb * kBK, it.term == 1 ? 1 : 0, w0 + kw, h0 + kh, i0);
+                        if (!P.b_resident)
+                            tma_load_2d(sa + kABytes, &P.tmB, &full[r.stage], wblk + (it.term == 2 ? kBK : 0), nt * BN);
+                    }
+                    r.next();
+                }
+                if (P.res_mma) {
+                    // residual: one extra K block per 64 output channels (two in split mode: hi and lo), the A operand
+                    // is the residual tile itself
+                    for (int g = 0; g < BN / 64 && nt * BN + g * 64 < P.Cout; ++g)
+                        for (int t = 0; t < rterms; ++t) {
+                            mbar_wait(&empty[r.stage], r.phase ^ 1);
+                            mbar_expect_tx(&full[r.stage], kABytes);
+                            tma_load_5d(smem + (size_t)r.stage * kStageBytes, &P.tmRes[pi], &full[r.stage], nt * BN + g * 64, t,
+                                        wb * pr.BW, hb * pr.BH, ib * pr.BI);
+                            r.next();
+                        }
+                }
+            }
+        }
     } else if (DEFORM) {
-        // ===================================================== deformable A-operand producers (warps 6-13)
+        // ===================================================== deformable A-operand producers (warps 8-15)
         // Per tap: threads 0-127 compute the bilinear parameters of their output pixel (4 weights + 4 element
         // offsets, deform_conv_cuda_kernel.cu:84-115 + the validity test of :229) into a shared table; then all
         // 256 threads gather: 8 consecutive lanes fetch the 8 x 16 B of one pixel's 64-channel block for each of
@@ -884,7 +850,15 @@ conv_tc_kernel(const __grid_constant__ TcParams P, int stages)
         __shared__ float4 s_w[2][128];
         __shared__ uint2 s_wh[2][128];                     // the same four weights as fp16 (split mode: blend of the lo halves)
         __shared__ int4 s_o[2][128];
-        const int pt = threadIdx.x - 192;                  // 0..kDP-1 (the stem transform uses the first 256)
+        const int pt = threadIdx.x - kConsumers;           // 0..kDP-1 (the stem transform uses the first 256)
+        // the B tile(s) of a stage: thread 0 of the producers adds their bytes to the stage's barrier and issues the TMA loads
+        auto load_b = [&](int stage, int tap, int cb, int nt) {
+            uint8_t *sb = smem + (size_t)stage * kStageBytes + (P.dcat ? 2 * kABytes : kABytes);
+            const int wblk = (tap * P.cin_blocks + cb) * (P.split ? 2 : 1) * kBK;
+            mbar_expect_tx(&full[stage], P.dcat ? 2 * kBBytes : kBBytes);
+            tma_load_2d(sb, &P.tmB, &full[stage], wblk, nt * BN);
+            if (P.dcat) tma_load_2d(sb + kBBytes, &P.tmB, &full[stage], wblk + kBK, nt * BN);
+        };
         Ring r(stages);
         int tb = 0;
         if (P.stem && pt >= 256) {
@@ -940,6 +914,7 @@ conv_tc_kernel(const __grid_constant__ TcParams P, int stages)
                 const int c16 = pt & 7;
                 for (int kb = 0; kb < 3; ++kb) {
                     mbar_wait(&empty[r.stage], r.phase ^ 1);
+                    if (pt == 0) load_b(r.stage, 0, kb, nt);
                     uint8_t *sa = smem + (size_t)r.stage * kStageBytes;
                     const int4 o0 = *reinterpret_cast<const int4 *>(&s_koff[kb * 64 + c16 * 8]);
                     const int4 o1 = *reinterpret_cast<const int4 *>(&s_koff[kb * 64 + c16 * 8 + 4]);
@@ -1017,6 +992,7 @@ conv_tc_kernel(const __grid_constant__ TcParams P, int stages)
                 for (int cb = 0; cb < P.cin_blocks; ++cb) {
                     if (!P.split) {
                         mbar_wait(&empty[r.stage], r.phase ^ 1);
+                        if (pt == 0) load_b(r.stage, tap, cb, nt);
                         uint8_t *sa = smem + (size_t)r.stage * kStageBytes;
                         uint4 u[kDItems][4];
 #pragma unroll
@@ -1051,7 +1027,7 @@ conv_tc_kernel(const __grid_constant__ TcParams P, int stages)
                             }
                             *reinterpret_cast<uint4 *>(sa + (size_t)row * 128 + ((c16 ^ (row & 7)) << 4)) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
                         }
-                        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic -> async proxy (UMMA reads smem)
+                        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic -> async proxy (wgmma reads smem)
                         __syncwarp();                                                   // every lane has fenced its own stores
                         if ((pt & 31) == 0) mbar_arrive(&full[r.stage]);
                         r.next();
@@ -1094,13 +1070,13 @@ conv_tc_kernel(const __grid_constant__ TcParams P, int stages)
                                     for (int c = 0; c < 4; ++c) {
                                         const uint32_t uh = reinterpret_cast<const uint32_t *>(&u[i1][c][0])[k];
                                         const uint32_t ul = reinterpret_cast<const uint32_t *>(&u[i1][c][1])[k];
-                                        acc = __ffma2_rn(wc[c], __half22float2(*reinterpret_cast<const __half2 *>(&uh)), acc);
+                                        acc = ffma2_rn(wc[c], __half22float2(*reinterpret_cast<const __half2 *>(&uh)), acc);
                                         accl = __hfma2(wl[c], *reinterpret_cast<const __half2 *>(&ul), accl);
                                     }
-                                    acc = __fadd2_rn(acc, __half22float2(accl));
+                                    acc = fadd2_rn(acc, __half22float2(accl));
                                     const __half2 h2 = __floats2half2_rn(acc.x, acc.y);
                                     const float2 hf = __half22float2(h2);
-                                    const float2 rem = __fadd2_rn(acc, make_float2(-hf.x, -hf.y));
+                                    const float2 rem = fadd2_rn(acc, make_float2(-hf.x, -hf.y));
                                     const __half2 l2 = __floats2half2_rn(rem.x, rem.y);
                                     phi[it][k] = *reinterpret_cast<const uint32_t *>(&h2);
                                     plo[it][k] = *reinterpret_cast<const uint32_t *>(&l2);
@@ -1109,6 +1085,7 @@ conv_tc_kernel(const __grid_constant__ TcParams P, int stages)
                         }
                         {
                             mbar_wait(&empty[r.stage], r.phase ^ 1);
+                            if (pt == 0) load_b(r.stage, tap, cb, nt);
                             uint8_t *sa = smem + (size_t)r.stage * kStageBytes;
 #pragma unroll
                             for (int it = 0; it < kDItems; ++it) {
@@ -1127,12 +1104,6 @@ conv_tc_kernel(const __grid_constant__ TcParams P, int stages)
                 tb ^= 1;
             }
         }
-    }
-    tcgen05_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tcgen05_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(kTmemCols) : "memory");
     }
 }
 
@@ -1169,7 +1140,7 @@ int launch_tc(const TcParams &P, int stages, int grid, cudaStream_t st, int stag
 {
     const size_t stage_b = (P.ncat || P.dcat) ? (P.b_resident ? 2 * kABytes : 2 * kABytes + 2 * BN * kBK * 2)
                                   : (P.b_resident ? kABytes : kABytes + BN * kBK * 2);
-    const size_t smem = 1024 + (size_t)stages * stage_b + (size_t)staging_bytes;
+    const size_t smem = 1024 + (size_t)kAccBytes + (size_t)stages * stage_b + (size_t)staging_bytes;
     auto kern = conv_tc_kernel<BN, OUT_F32, DEFORM>;
     static bool attr_set = false;
     if (!attr_set) {
@@ -1200,7 +1171,7 @@ int launch_tc(const TcParams &P, int stages, int grid, cudaStream_t st, int stag
         cudaLaunchConfig_t cfg;
         memset(&cfg, 0, sizeof(cfg));
         cfg.gridDim = dim3((unsigned)grid);
-        cfg.blockDim = dim3(DEFORM ? (unsigned)(192 + kDP) : 320u);
+        cfg.blockDim = dim3(DEFORM ? (unsigned)(kConsumers + kDP) : (unsigned)(kConsumers + 128));
         cfg.dynamicSmemBytes = smem;
         cfg.stream = st;
         cudaLaunchAttribute at[1];
@@ -1385,7 +1356,7 @@ extern "C" int orp_conv2d_tc_splitk(const orp_tc_problem *prob, const void *w, i
     ORP_CUDA(cudaGetSymbolAddress(&ovf, g_f16_overflow));
     const size_t items = pixels * (Cout / 8);
     size_t g = (items + 255) / 256;
-    if (g > 148 * 16) g = 148 * 16;
+    if (g > kNumSMs * 16) g = kNumSMs * 16;
     splitk_finish_kernel<<<(unsigned)(g ? g : 1), 256, 0, st>>>(workspace, ksplit, pixels, Cout, bias, relu, f16x3 ? 1 : 0, prob->out,
                                                                 static_cast<unsigned int *>(ovf));
     ORP_LAUNCHED();
@@ -1428,6 +1399,9 @@ static int conv2d_bf16_impl(int nprob, const orp_tc_problem *probs, const void *
         }
         while (BN > 64 && mtiles * (Cout_padded / BN) * ksplit < 120) BN /= 2;
     }
+    // the deformable variant's 512 threads leave 128 registers each: a 64 x 128 fp32 accumulator fragment (64 per thread)
+    // fits beside the epilogue, a 64 x 256 one does not
+    if (deform && BN > 128) BN = 128;
     TcParams P;
     memset(&P, 0, sizeof(P));
     // a partial last channel block is zero-filled by TMA (A operand) and by the weight layout (B operand)
@@ -1531,13 +1505,6 @@ static int conv2d_bf16_impl(int nprob, const orp_tc_problem *probs, const void *
     // the K-concatenated walk
     P.dcat = (split && deform && stem != 1) ? 1 : 0;
     P.ncat = (split && P.tma_epi && BN <= 128 && !deform && !any_res && stem != 1 && !getenv("ORP_TC_NO_NCAT")) ? 1 : 0;
-    // epilogue-bound layers (at most 6 K blocks per tile incl. the residual's; measured: 7-15 lose a little to the
-    // smaller staging/stage budget): independent epilogue warpgroups
-    {
-        const int kb_total = (KH * KW * P.cin_blocks) * ((split && !P.ncat) ? 3 : 1) + (any_res ? (BN / 64) * T : 0);
-        P.epi_split = (P.tma_epi && !deform && !stem && kb_total <= 6 && !getenv("ORP_TC_NO_SPLIT")) ? 1 : 0;
-        if (P.epi_split) P.epi_bufs = 2;
-    }
     // residual through the tensor core (TMA epilogue only; the staged epilogue adds it itself)
     P.res_mma = (P.tma_epi && any_res) ? 1 : 0;
     if (P.res_mma) {
@@ -1581,7 +1548,7 @@ static int conv2d_bf16_impl(int nprob, const orp_tc_problem *probs, const void *
             }
         }
     }
-    int sms = 148;
+    int sms = kNumSMs;
     {
         int dev = 0;
         ORP_CUDA(cudaGetDevice(&dev));
@@ -1590,8 +1557,8 @@ static int conv2d_bf16_impl(int nprob, const orp_tc_problem *probs, const void *
     int grid = P.num_tiles < sms ? P.num_tiles : sms;
     if (P.b_resident && grid >= P.n_tiles_n) grid -= grid % P.n_tiles_n;       // fixed N tile per CTA
     else if (P.b_resident) P.b_resident = 0;
-    // shared-memory budget: output staging + resident weights + main-loop stages.  When the extras leave fewer than three
-    // stages they are given up in order of least value: the second epilogue group, the second staging slot, the resident slab.
+    // shared-memory budget: staged accumulator pass + output staging + resident weights + main-loop stages.  When the extras
+    // leave fewer than three stages they are given up in order of least value: the second staging slot, the resident slab.
     int stage_bytes = 0, bres_bytes = 0, staging = 0, stages = 0;
     for (;;) {
         stage_bytes = (P.ncat || P.dcat) ? (P.b_resident ? 2 * kABytes : 2 * kABytes + 2 * BN * kBK * 2)
@@ -1599,10 +1566,9 @@ static int conv2d_bf16_impl(int nprob, const orp_tc_problem *probs, const void *
         bres_bytes = (P.b_resident ? KH * KW * T * P.cin_blocks * BN * kBK * 2 : 0) + (P.res_mma ? 8192 : 0) + (stem == 1 ? kStemPatchBytes : 0);
         const int hc = BN < 64 ? BN : 64;
         staging = out_f32 ? 0 : 128 * (hc * 2 + 16);
-        if (P.tma_epi) staging = P.epi_bufs * (P.epi_merge ? 32768 : 16384) * (P.epi_split ? 2 : 1);
-        stages = (int)((227 * 1024 - (deform || stem == 1 ? 14336 : 4096) - 1024 - staging - bres_bytes) / stage_bytes);   // static shared memory of the variant
+        if (P.tma_epi) staging = P.epi_bufs * (P.epi_merge ? 32768 : 16384);
+        stages = (int)((227 * 1024 - (deform || stem == 1 ? 14336 : 4096) - 1024 - kAccBytes - staging - bres_bytes) / stage_bytes);   // static shared memory of the variant
         if (stages >= 3) break;
-        if (P.epi_split) { P.epi_split = 0; P.epi_bufs = mem_bound ? 2 : 1; continue; }
         if (P.epi_bufs == 2) { P.epi_bufs = 1; continue; }
         if (P.b_resident) { P.b_resident = 0; continue; }
         if (stages >= 2) break;
@@ -1616,7 +1582,10 @@ static int conv2d_bf16_impl(int nprob, const orp_tc_problem *probs, const void *
 #define ORP_TC_DISPATCH(BNV)                                                                     \
     if (!launched && BN == BNV) {                                                                \
         launched = true;                                                                         \
-        if (deform) lrc = out_f32 ? launch_tc<BNV, true, true>(P, stages, grid, st, staging + bres_bytes) : launch_tc<BNV, false, true>(P, stages, grid, st, staging + bres_bytes); \
+        if (deform) {                                                                            \
+            if constexpr (BNV <= 128)                                                            \
+                lrc = out_f32 ? launch_tc<BNV, true, true>(P, stages, grid, st, staging + bres_bytes) : launch_tc<BNV, false, true>(P, stages, grid, st, staging + bres_bytes); \
+        }                                                                                        \
         else lrc = out_f32 ? launch_tc<BNV, true, false>(P, stages, grid, st, staging + bres_bytes) : launch_tc<BNV, false, false>(P, stages, grid, st, staging + bres_bytes);       \
     }
     ORP_TC_DISPATCH(256)

@@ -1,4 +1,4 @@
-// geom.cuh - device-side rotated-quadrilateral geometry for sm_100a.
+// geom.cuh - device-side rotated-quadrilateral geometry for sm_90a.
 //
 // Two IoU evaluators live here:
 //

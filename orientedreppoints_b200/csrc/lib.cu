@@ -15,9 +15,9 @@ int ensure_device()
     if (dev == checked_dev) return ORP_OK;
     cudaDeviceProp prop;
     ORP_CUDA(cudaGetDeviceProperties(&prop, dev));
-    if (prop.major != 10) {
+    if (prop.major != 9) {
         snprintf(g_err, sizeof(g_err),
-                 "liborp_b200 is built for sm_100a only; device %d is sm_%d%d (no fallback path exists)", dev,
+                 "liborp_b200 is built for sm_90a (H100) only; device %d is sm_%d%d (no fallback path exists)", dev,
                  prop.major, prop.minor);
         return ORP_ENOGPU;
     }
@@ -35,6 +35,6 @@ int ensure_device()
 extern "C" const char *orp_last_error(void) { return orp::g_err; }
 extern "C" void orp_set_timing(int on) { orp::g_timing = on; }
 extern "C" int orp_version(void) { return 100; }
-extern "C" int orp_compiled_sm(void) { return 100; }
+extern "C" int orp_compiled_sm(void) { return 90; }
 extern "C" int64_t orp_launch_count(void) { return __atomic_load_n(&orp::g_launches, __ATOMIC_RELAXED); }
 extern "C" void orp_reset_launch_count(void) { __atomic_store_n(&orp::g_launches, 0, __ATOMIC_RELAXED); }

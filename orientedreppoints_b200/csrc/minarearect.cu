@@ -1,4 +1,4 @@
-// minarearect.cu - 9-point sets -> minimum-area rectangles on sm_100a (SURVEY.md section 8 row a8).
+// minarearect.cu - 9-point sets -> minimum-area rectangles on sm_90a (SURVEY.md section 8 row a8).
 //
 // Replaces minareabbox_cuda (mmdet/ops/minarearect/src/minarearect_kernel.cu:470-505), which runs one
 // thread per set on the legacy stream, then copies the result to the host, loops over it and uploads it

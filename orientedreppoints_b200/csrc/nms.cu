@@ -1,4 +1,4 @@
-// nms.cu - rotated / polygon greedy NMS for sm_100a (SURVEY.md section 8 rows a9, a10, a14, a15).
+// nms.cu - rotated / polygon greedy NMS for sm_90a (SURVEY.md section 8 rows a9, a10, a14, a15).
 //
 // Replaces rnms_cuda (mmdet/ops/nms/src/rnms_kernel.cu:204-265) and _poly_nms
 // (DOTA_devkit/poly_nms_gpu/poly_nms_kernel.cu:277-329).  The reference materialises an
@@ -917,7 +917,7 @@ int run_nms(const float *dets, const int32_t *segments, int n, double thr, int i
             }
             SweepParams P{aabb, meta_s, v01, v23, nvalid, glob, R, edges, indeg, pending, cap, ctr, thr, union_mode};
             int grid = ceil_div(m, kSweepWarps);
-            const int maxgrid = 148 * 8 * 4;
+            const int maxgrid = kNumSMs * 8 * 4;
             if (grid > maxgrid) grid = maxgrid;
             if (g_timing) {
                 if (!g_ev[0]) { ORP_CUDA(cudaEventCreate(&g_ev[0])); ORP_CUDA(cudaEventCreate(&g_ev[1])); }
@@ -964,7 +964,7 @@ int run_nms(const float *dets, const int32_t *segments, int n, double thr, int i
     int32_t *adj = S.get<int32_t>(cap);
     if (!adj) return fail(ORP_ECUDA, "orp_rnms: adjacency allocation failed");
     {
-        int grid = 148 * 8;
+        int grid = kNumSMs * 8;
         nms_scatter_kernel<<<grid, 256, 0, st>>>(edges, ctr, cap, offs, cursor, adj);
         ORP_LAUNCHED();
     }

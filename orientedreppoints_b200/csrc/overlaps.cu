@@ -1,4 +1,4 @@
-// overlaps.cu - pairwise rotated IoU matrices for sm_100a (SURVEY.md section 8 rows a13, a15, n2).
+// overlaps.cu - pairwise rotated IoU matrices for sm_90a (SURVEY.md section 8 rows a13, a15, n2).
 //
 //   orp_poly_overlaps(_host)   DOTA_devkit/poly_nms_gpu/poly_overlaps_kernel.cu:280-427
 //   orp_quad_iou_matrix        N x K over 8-coordinate quads (rnms/poly_nms IoU as a matrix)

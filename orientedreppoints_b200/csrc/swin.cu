@@ -551,7 +551,7 @@ subsample2_kernel(const uint16_t *__restrict__ x, int B, int H, int W, int C /* 
 int grid_for(long long items, int threads)
 {
     long long g = (items + threads - 1) / threads;
-    const long long cap = 148 * 16;
+    const long long cap = kNumSMs * 16;
     return (int)(g < cap ? (g ? g : 1) : cap);
 }
 

@@ -8,8 +8,8 @@ Mirrors mmdet/models/detectors/orientedreppoints_detector.py:37-46:
 
 Host code is Python; every layer is a kernel of this repository called through the C ABI
 (include/orp_b200.h) on torch-owned device memory and the current torch stream.  Activations are NHWC.
-Three arithmetic engines: 'f16x3' (tcgen05 tensor cores on fp16 hi/lo operand pairs, three MMAs per product,
-fp32 accumulation in TMEM - fp32-faithful, the parity AND benchmark arithmetic), 'bf16' (tcgen05, single-pass bf16
+Three arithmetic engines: 'f16x3' (wgmma tensor cores on fp16 hi/lo operand pairs, three MMAs per product,
+fp32 accumulation - fp32-faithful, the parity AND benchmark arithmetic), 'bf16' (wgmma, single-pass bf16
 operands - 3x the rate, ~1e-2 accuracy) and 'fp32' (CUDA-core FMAs).  There is no PyTorch/cuDNN fallback for any layer.
 """
 import numpy as np

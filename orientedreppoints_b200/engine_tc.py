@@ -1,4 +1,4 @@
-"""Tensor-core engines of the dense path: tcgen05 implicit-GEMM convolutions (csrc/dense_tc.cu) plus their
+"""Tensor-core engines of the dense path: wgmma implicit-GEMM convolutions (csrc/dense_tc.cu) plus their
 memory-bound companions (csrc/dense_bf16_misc.cu, csrc/dense_f16x3_misc.cu).  EngineTC: bf16 operands (fast, ~1e-2);
 EngineTCSplit: f16x3 split operands (fp32-faithful, the parity mode).  Same interface as detector.EngineF32."""
 import ctypes
@@ -130,14 +130,14 @@ class EngineTC:
 
     @staticmethod
     def _ksplit(n, ho, wo, L, nprob, relu, residual, out_f32, residual_f32):
-        """split-K factor for a launch whose tiling would leave most of the 148 SMs idle (3x3 layers on small maps)"""
+        """split-K factor for a launch whose tiling would leave most of the 132 SMs idle (3x3 layers on small maps)"""
         if nprob != 1 or L.kh * L.kw != 9 or residual is not None or residual_f32 is not None or out_f32 or relu == 2 or L.cout % 8:
             return 1
         mt = -(-(n * ho * wo) // 128)
-        if mt * -(-L.cout // 64) > 74:           # the narrow-tile (BN = 64) launch already fills half the machine: measured faster
-            return 1                             # than split-K there (64^2 x 256 -> 256: 45 us vs 76 us)
+        if mt * -(-L.cout // 64) > 66:           # the narrow-tile (BN = 64) launch already fills half the machine: no split-K
+            return 1
         tiles = mt * -(-L.cout // 256)
-        return 9 if tiles * 9 <= 2 * 148 else 3
+        return 9 if tiles * 9 <= 2 * 132 else 3
 
     def _conv_splitk(self, x, y, tc, L, relu, ks, stats, f16x3):
         ws = torch.empty((ks, y.shape[0], y.shape[1], y.shape[2], L.cout), dtype=torch.float32, device=self.device)
@@ -251,8 +251,8 @@ class EngineTC:
 
 
 class EngineTCSplit(EngineTC):
-    """f16x3 arithmetic on the same tcgen05 kernels - the PARITY mode (include/orp_b200.h, "split" section): every fp32
-    value is an fp16 pair hi + lo, every product hi*hi + lo*hi + hi*lo in one fp32 TMEM accumulator.  Activations are
+    """f16x3 arithmetic on the same wgmma kernels - the PARITY mode (include/orp_b200.h, "split" section): every fp32
+    value is an fp16 pair hi + lo, every product hi*hi + lo*hi + hi*lo in one fp32 accumulator.  Activations are
     fp16 tensors [N,H,W,2,C] (hi channels, then lo channels)."""
     name = "f16x3"
     act_dtype = torch.float16

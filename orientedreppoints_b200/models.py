@@ -231,7 +231,7 @@ class OrientedRepPointsDetector(nn.Module):
             from .detector import OrientedRepPointsDetector as Engine
             dev = torch.device(device) if device is not None else next(self.parameters()).device
             if dev.type != 'cuda':
-                raise NotImplementedError("OrientedRepPointsDetector inference needs a CUDA (sm_100a) device: there is no CPU path")
+                raise NotImplementedError("OrientedRepPointsDetector inference needs a CUDA (sm_90a) device: there is no CPU path")
             depth = self.backbone.depth if isinstance(self.backbone, ResNet) else "swin_tiny"
             self._engine = Engine({k: v.detach() for k, v in self.state_dict().items()}, depth, dev, self.precision,
                                   test_cfg=dict(self.test_cfg) if self.test_cfg else None)

@@ -1,5 +1,5 @@
 """`mmdet.ops.conv` surface (mmdet/ops/conv.py:6-40): config strings -> convolution layer classes; 'DCN' / 'DCNv2' resolve to
-this repository's tcgen05-backed deformable convolutions (ops/dcn.py)."""
+this repository's tensor-core (wgmma) deformable convolutions (ops/dcn.py)."""
 from torch import nn as nn
 
 from .dcn import DeformConvPack, ModulatedDeformConvPack

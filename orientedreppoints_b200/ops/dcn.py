@@ -7,7 +7,7 @@ fp32 tensors in and out, and the same error behaviour (`assert not bias`, ValueE
 NotImplementedError, `RuntimeError` for an offset of the wrong shape as deform_conv_cuda.cpp:130-136 raises).
 
 What runs underneath is NOT the reference's im2col + SGEMM (deform_conv_cuda.cpp:152-260: a 151 MB `columns` buffer per
-level): the sampling happens inside the tcgen05 implicit-GEMM kernel's A-operand producers (csrc/dense_tc.cu), in f16x3
+level): the sampling happens inside the wgmma implicit-GEMM kernel's A-operand producers (csrc/dense_tc.cu), in f16x3
 arithmetic by default (fp32-faithful: |err| ~1e-5 of max, see include/orp_b200.h) or single-pass bf16
 (`set_precision('bf16')`).  Shapes the tensor-core kernel does not cover (Cin % 64, dilation > 1, bias-free fp32 path)
 run on the fp32 CUDA-core kernel `orp_deform_conv2d_f32`.  groups / deformable_groups > 1 are not built (the reference's

@@ -12,7 +12,7 @@ absent), so its plumbing is stubbed: `mmcv.cnn` initialisers (weights are overwr
 `auto_fp16`, loss builders; the ONE compute stub is `DeformConv` (CUDA-only extension in the reference), replaced by
 oracle/torch_reference.py::deform_conv_ref (itself an im2col restatement of deform_conv_cuda_kernel.cu).
 
-    python tests/golden/gen_golden_dense.py     # needs /root/reference; writes tests/golden/dense_r50.npz
+    python tests/golden/gen_golden_dense.py     # needs the reference source tree; writes tests/golden/dense_ref_r50.npz, dense_ref_r101.npz
 """
 import importlib
 import os
@@ -162,8 +162,9 @@ def main():
             out["%s_init%d" % (tag, l)] = init[l].numpy()
             out["%s_refine%d" % (tag, l)] = refine[l].numpy()
         print(tag, [tuple(f.shape) for f in feats], float(feats[0].abs().max()), float(cls[0].abs().max()))
-    np.savez_compressed(os.path.join(HERE, "dense_ref.npz"), **out)
-    print("wrote dense_ref.npz")
+    for tag in ("r50", "r101"):                                                        # one file per depth: each under 1 MB
+        np.savez_compressed(os.path.join(HERE, "dense_ref_%s.npz" % tag), **{k: v for k, v in out.items() if k.startswith(tag + "_")})
+        print("wrote dense_ref_%s.npz" % tag)
 
 
 if __name__ == "__main__":

@@ -4,7 +4,7 @@ mmdet/models/backbones/swin_transformer.py::SwinTransformer (arguments of config
 run on the CPU in float64 (eval mode: DropPath is the identity).  Stubs: timm.models.layers (DropPath / to_2tuple /
 trunc_normal_ - initialisers only, weights come from the state dict), mmcv_custom.load_checkpoint, registries.
 
-    python tests/golden/gen_golden_swin.py     # needs /root/reference; writes tests/golden/swin_ref.npz
+    python tests/golden/gen_golden_swin.py     # needs the reference source tree; writes tests/golden/swin_ref_c0.npz, swin_ref_c1.npz
 """
 import importlib
 import os
@@ -71,8 +71,9 @@ def main():
         for i, t in enumerate(f):
             out["c%d_fpn%d" % (case, i)] = t.numpy()
         print(case, [tuple(t.shape) for t in c], [tuple(t.shape) for t in f])
-    np.savez_compressed(os.path.join(HERE, "swin_ref.npz"), **out)
-    print("wrote swin_ref.npz")
+    for case in range(2):                                                               # one file per case: each under 1 MB
+        np.savez_compressed(os.path.join(HERE, "swin_ref_c%d.npz" % case), **{k: v for k, v in out.items() if k.startswith("c%d_" % case)})
+        print("wrote swin_ref_c%d.npz" % case)
 
 
 if __name__ == "__main__":

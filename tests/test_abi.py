@@ -27,11 +27,11 @@ def test_library_exports_every_declared_symbol():
 def test_version_and_arch():
     l = _lib.lib()
     assert l.orp_version() >= 100
-    assert l.orp_compiled_sm() == 100
+    assert l.orp_compiled_sm() == 90
 
 
-def test_sass_is_sm100a_only():
+def test_sass_is_sm90a_only():
     import subprocess
     out = subprocess.run(["cuobjdump", "--list-elf", _lib.LIB_PATH], capture_output=True, text=True).stdout
     archs = set(re.findall(r"sm_(\d+a?)", out))
-    assert archs == {"100a"}, archs
+    assert archs == {"90a"}, archs

@@ -1,4 +1,4 @@
-"""GPU parity tests (run with -m gpu on the B200 box): the CUDA path through the C-ABI against the
+"""GPU parity tests (run with -m gpu on an H100): the CUDA path through the C-ABI against the
 CPU oracle and the committed golden vectors.  Integer/index results bit-exact; fp64 IoU bit-exact;
 fp32 'compat32' IoU bit-exact; fp32 'exact64' IoU values within 1e-5 of the fp64 reference."""
 import numpy as np

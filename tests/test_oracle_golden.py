@@ -1,6 +1,6 @@
 """CPU: the oracle (oracle/*.c) against the golden vectors minted from the reference itself
-(tests/golden/gen_golden.py) and, where /root/reference was compiled into oracle/_ref, against the
-live reference.  Bit-exact: the oracle restates the reference's arithmetic operation for operation."""
+(tests/golden/gen_golden*.py, oracle/build_ref.py).  Bit-exact: the oracle restates the reference's arithmetic
+operation for operation."""
 import os
 
 import numpy as np
@@ -43,16 +43,17 @@ def test_fp32_reference_is_unstable_far_from_origin(golden):
     assert len(far["keep64_thr01"]) == 660 and len(far["keep32_thr01"]) == 511
 
 
-def test_live_reference_if_present(po):
-    if not po.ref_available():
-        pytest.skip("oracle/_ref not built (no /root/reference on this machine)")
+def test_clustered_iou_pairs_bit_exact_vs_reference(po, golden):
+    """4000 pairs drawn from clustered boxes (gen_clustered_boxes(40, 12, seed=11)): what the reference's polyiou.cpp (fp64)
+    and rnms_cpu.cpp rotate_iou (fp32), compiled by oracle/build_ref.py, returned for them"""
+    g = golden("iou_pairs_clustered.npz")
     d = po.gen_clustered_boxes(40, 12, seed=11)
     rng = np.random.RandomState(5)
     i, j = rng.randint(0, len(d), 4000), rng.randint(0, len(d), 4000)
     p, q = d[i, :8], d[j, :8]
-    assert np.array_equal(po.iou_poly_f64(p, q), po.ref_iou_poly_pairs(p, q), equal_nan=True)
-    if os.path.exists(os.path.join(po.REF_DIR, "ref_rnms_cpu.so")):
-        assert np.array_equal(po.iou_rnms_f32(p, q), po.ref_rotate_iou_pairs(p, q), equal_nan=True)
+    assert np.array_equal(p, g["p"]) and np.array_equal(q, g["q"])     # the generator still yields the stored pairs
+    assert np.array_equal(po.iou_poly_f64(p, q), g["ref64"], equal_nan=True)
+    assert np.array_equal(po.iou_rnms_f32(p, q), g["ref32"], equal_nan=True)
 
 
 def test_guard_and_nan_conventions(po):
@@ -198,16 +199,16 @@ def test_postprocess_restatement_equals_reference_python(case):
 
 @pytest.mark.parametrize("depth", [50, 101])
 def test_dense_graph_restatement_equals_reference_modules(depth):
-    """SURVEY 8 a1/a3/a4/a5: tests/golden/dense_ref.npz holds the outputs of the reference's OWN ResNet, FPN and
-    OrientedRepPointsHead modules (imported from /root/reference by tests/golden/gen_golden_dense.py with mmcv/registry
+    """SURVEY 8 a1/a3/a4/a5: tests/golden/dense_ref_r{50,101}.npz hold the outputs of the reference's OWN ResNet, FPN and
+    OrientedRepPointsHead modules (imported from the reference's source tree by tests/golden/gen_golden_dense.py with mmcv/registry
     plumbing stubbed and DeformConv replaced by the oracle's deform_conv_ref), loaded with strict=True from
     weights.random_state_dict (same key names) and run in float64.  The functional restatement the GPU engines are checked
     against (oracle/torch_reference.py::forward_dense) agrees to rounding noise on every FPN level and head output."""
     import torch
     from oracle import torch_reference as tr
     from orientedreppoints_b200.weights import STAGE_BLOCKS, random_state_dict
-    g = np.load(os.path.join(os.path.dirname(__file__), "golden", "dense_ref.npz"))
     tag = "r%d" % depth
+    g = np.load(os.path.join(os.path.dirname(__file__), "golden", "dense_ref_%s.npz" % tag))
     d, seed, h, w = [int(v) for v in g[tag + "_meta"]]
     sd = {k: v.double() for k, v in random_state_dict(d, seed=seed, reference_init=False).items()}
     img = torch.from_numpy(g[tag + "_img"])
@@ -223,15 +224,15 @@ def test_dense_graph_restatement_equals_reference_modules(depth):
 
 @pytest.mark.parametrize("case", [0, 1])
 def test_swin_restatement_equals_reference_module(case):
-    """SURVEY 8 a2: tests/golden/swin_ref.npz holds the outputs of the reference's OWN SwinTransformer
+    """SURVEY 8 a2: tests/golden/swin_ref_c{0,1}.npz hold the outputs of the reference's OWN SwinTransformer
     (backbones/swin_transformer.py, arguments of configs/dota/orientedrepoints_swin_tiny_demo.py:9-25) and FPN
-    (in_channels [192,384,768], num_outs 5, GN), imported from /root/reference by tests/golden/gen_golden_swin.py (timm /
+    (in_channels [192,384,768], num_outs 5, GN), imported from the reference's source tree by tests/golden/gen_golden_swin.py (timm /
     mmcv plumbing stubbed) and run in float64; case 1 exercises the window padding.  The functional restatement the GPU
     Swin path is checked against (oracle/torch_swin.py) agrees to rounding noise."""
     import torch
     from oracle import torch_swin as ts
     from orientedreppoints_b200.swin import random_swin_state_dict
-    g = np.load(os.path.join(os.path.dirname(__file__), "golden", "swin_ref.npz"))
+    g = np.load(os.path.join(os.path.dirname(__file__), "golden", "swin_ref_c%d.npz" % case))
     sd = {k: (v.double() if v.is_floating_point() else v) for k, v in random_swin_state_dict(0).items()}
     img = torch.from_numpy(g["c%d_img" % case])
     with torch.no_grad():
@@ -277,12 +278,12 @@ def _quad_area(b):
 
 
 def test_minarearect_oracle_vs_reference_device_code(po):
-    """SURVEY 8 a8: tests/golden/device_ops_ref.npz holds what the reference's OWN __device__ code of
+    """SURVEY 8 a8: tests/golden/minarearect_ref.npz holds what the reference's OWN __device__ code of
     minarearect_kernel.cu (Findminbox / Jarvis_and_index, compiled as host C++ by oracle/build_ref.py) returns.
     Hull index maps: identical.  Rectangles: identical or within 2e-6 (the reference calls cosf, the oracle and the CUDA
     kernel evaluate cos in double and round - DESIGN deviation 3), except near-ties of the min-area argmin (< 0.1 % of the
     sets) where the other, equally small rectangle is chosen: same area to 1e-6."""
-    g = np.load(os.path.join(os.path.dirname(__file__), "golden", "device_ops_ref.npz"))
+    g = np.load(os.path.join(os.path.dirname(__file__), "golden", "minarearect_ref.npz"))
     boxes, maps, hull_n = po.minarearect(g["mar_pts"])
     assert np.array_equal(hull_n, g["mar_hull_n"])
     for i in range(len(hull_n)):
@@ -307,11 +308,11 @@ def test_convex_iou_oracle_bit_identical_to_reference_device_code(po):
 def test_poly_nms_and_poly_overlaps_oracles_bit_identical_to_reference_device_code(po):
     """SURVEY 8 a15: DOTA_devkit/poly_nms_gpu has CUDA sources only; their __device__ functions compiled as host C++
     (oracle/build_ref.py) give tests/golden/device_ops_ref.npz.  The restatements reproduce every float: devPolyIoU of
-    poly_nms_kernel.cu on 20 000 clustered quad pairs, RotBox2Poly and devPolyIoU of poly_overlaps_kernel.cu on 300 x 40
+    poly_nms_kernel.cu on 4000 clustered quad pairs, RotBox2Poly and devPolyIoU of poly_overlaps_kernel.cu on 300 x 40
     (cx, cy, w, h, theta) boxes."""
     g = np.load(os.path.join(os.path.dirname(__file__), "golden", "device_ops_ref.npz"))
-    mine = np.array([po.iou_polynms_f32_one(p, q) for p, q in zip(g["pn_p"][:4000], g["pn_q"][:4000])], dtype=np.float32)
-    assert np.array_equal(mine.view(np.uint32), g["pn_iou"][:4000].view(np.uint32))
+    mine = np.array([po.iou_polynms_f32_one(p, q) for p, q in zip(g["pn_p"], g["pn_q"])], dtype=np.float32)
+    assert len(mine) == 4000 and np.array_equal(mine.view(np.uint32), g["pn_iou"].view(np.uint32))
     assert np.array_equal(po.rotbox_to_quad_f32(g["po_boxes"]), g["po_quads"])
     ov = po.poly_overlaps_f32(g["po_boxes"], g["po_query"])
     assert np.array_equal(ov.view(np.uint32), g["po_iou"].view(np.uint32)) and (ov > 0).mean() > 0.1

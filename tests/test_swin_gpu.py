@@ -100,7 +100,7 @@ def test_swin_backbone_and_detector_vs_torch(cuda, swin_sd):
 
 
 def test_swin_f16x3_kernels_and_backbone_vs_fp64(cuda, swin_sd):
-    """Swin-T in the parity arithmetic (f16x3 Linear layers on tcgen05, LayerNorm / window attention / gathers on split fp16
+    """Swin-T in the parity arithmetic (f16x3 Linear layers on the wgmma kernels, LayerNorm / window attention / gathers on split fp16
     tokens): component kernels vs torch in fp64, whole backbone + FPN + head vs the fp64 evaluation of the reference graph
     (oracle/torch_swin.py, pinned to the reference's own SwinTransformer), tolerance = north_star's 1e-4"""
     from oracle import torch_reference as tr
