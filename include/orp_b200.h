@@ -122,6 +122,29 @@ int orp_rnms_last_sweep_ms(float *ms);
  * resets) the summed device time, the number of launches and their algorithmic FLOPs (2*MACs) since
  * the previous collect on this thread */
 int orp_tc_timing_collect(float *total_ms, int *launches, double *flops);
+/* The launch plan of this thread's most recent tensor-core convolution (orp_conv2d_bf16 / orp_conv2d_f16x3 /
+ * orp_conv2d_tc_splitk / orp_stem_conv_*), as launched: the host code picks it from the shapes.  An observation point
+ * for tests and traces (there is no way to request a plan).  ORP_EINVAL before the first launch on the thread. */
+typedef struct {
+    int BN;                  /* accumulator width: 256, 128, 64 or 32 output channels per tile              */
+    int stages;              /* main-loop pipeline stages                                                    */
+    int grid;                /* persistent CTAs                                                              */
+    int num_tiles;           /* (m tile, n tile, k split) units; num_tiles > grid: a CTA runs several        */
+    int n_tiles_n;           /* N tiles (Cout_padded / BN)                                                   */
+    int ksplit;              /* split-K factor (1: none)                                                     */
+    int nprob;               /* problems served by the launch                                                */
+    int Cout, Cout_padded;
+    int split;               /* f16x3 operands                                                               */
+    int deform;              /* gathered (deformable) A operand                                              */
+    int out_f32;             /* fp32 output (head predictions, split-K partial sums)                         */
+    int stem;                /* 0 none, 1 direct conv1, 2 space-to-depth conv1                               */
+    int relu;                /* epilogue activation: 0 none, 1 ReLU, 2 exact GELU                            */
+    int bias;                /* a bias is added in the kernel's epilogue                                     */
+    int residual;            /* 0 none, 1 16-bit residual (bf16 / split), 2 fp32 residual                    */
+    int tma_epi, ncat, dcat, res_mma, b_resident, epi_merge, epi_bufs, gn_fused;   /* see csrc/dense_tc.cu      */
+    int BW[5], BH[5], BI[5]; /* per problem: the 128-pixel tile box (width, height, images)                  */
+} orp_tc_plan;
+int orp_tc_last_plan(orp_tc_plan *out);
 
 /* ------------------------------------------------------------------------------------------
  * Pairwise rotated IoU

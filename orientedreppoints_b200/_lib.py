@@ -34,6 +34,19 @@ class TcProblem(ctypes.Structure):
                 ("residual_f32", _vp), ("offset", _vp), ("gn_stats", _vp), ("mask", _vp)]
 
 
+class TcPlan(ctypes.Structure):
+    _fields_ = [(k, _i) for k in ("BN", "stages", "grid", "num_tiles", "n_tiles_n", "ksplit", "nprob", "Cout", "Cout_padded",
+                                  "split", "deform", "out_f32", "stem", "relu", "bias", "residual", "tma_epi", "ncat", "dcat",
+                                  "res_mma", "b_resident", "epi_merge", "epi_bufs", "gn_fused")] + \
+              [(k, _i * 5) for k in ("BW", "BH", "BI")]
+
+    def as_dict(self):
+        d = {k: getattr(self, k) for k, _ in self._fields_}
+        for k in ("BW", "BH", "BI"):
+            d[k] = list(d[k])[:self.nprob]
+        return d
+
+
 class GnProblem(ctypes.Structure):
     _fields_ = [("x", _vp), ("N", _i), ("H", _i), ("W", _i), ("stats", _vp), ("up_src", _vp), ("y", _vp)]
 
@@ -51,6 +64,7 @@ SIGNATURES = {
     "orp_set_timing": (None, [_i]),
     "orp_rnms_last_sweep_ms": (_i, [ctypes.POINTER(ctypes.c_float)]),
     "orp_tc_timing_collect": (_i, [ctypes.POINTER(ctypes.c_float), ctypes.POINTER(_i), ctypes.POINTER(_d)]),
+    "orp_tc_last_plan": (_i, [ctypes.POINTER(TcPlan)]),
     "orp_poly_overlaps_host": (_i, [_vp, _vp, _vp, _i, _i, _i]),
     "orp_poly_overlaps": (_i, [_vp, _i, _vp, _i, _vp, _vp]),
     "orp_quad_iou_matrix": (_i, [_vp, _i, _vp, _i, _i, _i, _vp, _vp]),
@@ -161,6 +175,13 @@ def tc_timing_collect():
     ms, n, fl = ctypes.c_float(0), ctypes.c_int(0), ctypes.c_double(0)
     check(lib().orp_tc_timing_collect(ctypes.byref(ms), ctypes.byref(n), ctypes.byref(fl)), "orp_tc_timing_collect")
     return float(ms.value), int(n.value), float(fl.value)
+
+
+def tc_last_plan():
+    """launch plan of this thread's most recent tensor-core convolution (dict of the orp_tc_plan fields)"""
+    p = TcPlan()
+    check(lib().orp_tc_last_plan(ctypes.byref(p)), "orp_tc_last_plan")
+    return p.as_dict()
 
 
 def current_stream_ptr():

@@ -1134,6 +1134,9 @@ thread_local int g_tc_ev_created = 0, g_tc_ev_used = 0;
 thread_local double g_tc_flops = 0.0;
 struct TcTrace { int nprob, N, H, W, Cin, Cout, K, stride, deform, BN, tiles, grid; double flops; };
 thread_local TcTrace g_tc_trace[kEvPool];
+// plan of this thread's most recent launch (orp_tc_last_plan)
+thread_local orp_tc_plan g_tc_plan;
+thread_local bool g_tc_plan_set = false;
 
 template <int BN, bool OUT_F32, bool DEFORM>
 int launch_tc(const TcParams &P, int stages, int grid, cudaStream_t st, int staging_bytes)
@@ -1209,6 +1212,15 @@ extern "C" int orp_tc_timing_collect(float *total_ms, int *launches, double *flo
     }
     *total_ms = sum; *launches = g_tc_ev_used; *flops = g_tc_flops;
     g_tc_ev_used = 0; g_tc_flops = 0.0;
+    return ORP_OK;
+}
+
+/* see include/orp_b200.h */
+extern "C" int orp_tc_last_plan(orp_tc_plan *out)
+{
+    if (!out) return fail(ORP_EINVAL, "orp_tc_last_plan: null");
+    if (!g_tc_plan_set) return fail(ORP_EINVAL, "orp_tc_last_plan: no tensor-core convolution launched on this thread");
+    *out = g_tc_plan;
     return ORP_OK;
 }
 
@@ -1577,6 +1589,23 @@ static int conv2d_bf16_impl(int nprob, const orp_tc_problem *probs, const void *
     if (stages > kStagesMax) stages = kStagesMax;
     if (const char *e = getenv("ORP_TC_STAGES")) { const int v = atoi(e); if (v >= 2 && v < stages) stages = v; }   // experiments
     if (deform && stages > 3) stages = 3;     // leave L1 capacity for the bilinear gather (corner reuse between neighbouring pixels)
+    {
+        // the plan as launched, for orp_tc_last_plan
+        orp_tc_plan &pl = g_tc_plan;
+        memset(&pl, 0, sizeof(pl));
+        pl.BN = BN; pl.stages = stages; pl.grid = grid; pl.num_tiles = P.num_tiles; pl.n_tiles_n = P.n_tiles_n;
+        pl.ksplit = ksplit; pl.nprob = nprob; pl.Cout = Cout; pl.Cout_padded = Cout_padded;
+        pl.split = P.split; pl.deform = deform ? 1 : 0; pl.out_f32 = out_f32 ? 1 : 0; pl.stem = stem; pl.relu = relu;
+        pl.bias = bias ? 1 : 0;
+        for (int i = 0; i < nprob; ++i) {
+            if (probs[i].residual_bf16) pl.residual = 1;
+            else if (probs[i].residual_f32) pl.residual = 2;
+            pl.BW[i] = P.prob[i].BW; pl.BH[i] = P.prob[i].BH; pl.BI[i] = P.prob[i].BI;
+        }
+        pl.tma_epi = P.tma_epi; pl.ncat = P.ncat; pl.dcat = P.dcat; pl.res_mma = P.res_mma; pl.b_resident = P.b_resident;
+        pl.epi_merge = P.epi_merge; pl.epi_bufs = P.epi_bufs; pl.gn_fused = P.gn_fused;
+        g_tc_plan_set = true;
+    }
     int lrc = ORP_EINVAL;
     bool launched = false;
 #define ORP_TC_DISPATCH(BNV)                                                                     \
