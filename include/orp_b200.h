@@ -58,11 +58,20 @@ void orp_reset_launch_count(void);
 /* degenerate-union convention:
  *   ORP_UNION_NAN_KEEPS      rnms  (rnms_kernel.cu:131-147: 0/0 = NaN, `NaN > thr` false)
  *   ORP_UNION_GUARD          poly_gpu_nms (poly_nms_kernel.cu:205-210: (inter+1)/(union+1))
- *   ORP_UNION_NAN_SUPPRESSES py_cpu_nms_poly (ResultMerge.py:39 keeps only `iou <= thr`)
+ *   ORP_UNION_NAN_SUPPRESSES py_cpu_nms_poly_fast (ResultMerge_multi_process.py:60-121: `iou <= thr` keeps, a pair
+ *                            is only compared when the axis-aligned hulls overlap with positive area)
+ *   ORP_UNION_NAN_SUPPRESSES_ALL py_cpu_nms_poly (ResultMerge.py:18-41: `iou <= thr` keeps, every pair compared)
+ * ORP_UNION_GUARD and ORP_UNION_NAN_SUPPRESSES_ALL compare two zero-area boxes (fp64 signed area exactly 0: points,
+ * segments, collinear quads) wherever they are, as the reference does: the pair suppresses when the fp64 fan
+ * intersection is exactly 0 (union 0: guard IoU 1, NaN), and keeps when a rounding residue leaves union = -inter != 0
+ * (IoU -1).  Boxes whose fp64 signed area is within 2^-36 S^2 of 0 (S: the set's largest |coordinate|; collinear rings
+ * whose shoelace sum rounds to a residue) are compared the same way.  Every pair is decided by the fp64 algorithm with
+ * the better-ranked box first.
  */
 #define ORP_UNION_NAN_KEEPS 0
 #define ORP_UNION_GUARD 1
 #define ORP_UNION_NAN_SUPPRESSES 2
+#define ORP_UNION_NAN_SUPPRESSES_ALL 3
 
 /* output ordering of the kept indices:
  *   ORP_ORDER_INDEX_ASC  rnms_cuda (rnms_kernel.cu:261-264)
@@ -112,6 +121,23 @@ typedef struct {
     int32_t n;
 } orp_nms_stats;
 int orp_rnms_last_stats(orp_nms_stats *out);
+
+/* The plan of this thread's most recent rotated NMS (orp_rnms, orp_poly_nms_host and the NMS inside
+ * orp_head_postprocess), recorded by the host code before it launches; an observation point for tests and traces
+ * that changes no decision.  ORP_EINVAL before the first call on the thread. */
+typedef struct {
+    int32_t lazy;            /* 1: ORP_NMS_EXACT64 (sweep + lazy resolve), 0: ORP_NMS_COMPAT32 (every pair)        */
+    int32_t R;               /* registrations per box: 4 = y strips, 1 = none                                     */
+    int32_t seg_limit;       /* segment bound the caller passed (0: unknown)                                      */
+    int32_t sweep_bits;      /* key bits of the sweep-order radix sort                                            */
+    int32_t no_sync;         /* 1: a candidate-list overflow is reported on the device instead of retried          */
+    int32_t flags_out;       /* 1: survivor flags by index instead of a compacted keep list                       */
+    int32_t union_mode, order, n;
+    int64_t cap_first;       /* candidate-pair capacity of the first attempt                                      */
+    int64_t cap_final;       /* capacity of the attempt whose candidates were resolved                            */
+    int32_t attempts;        /* sweeps run: 2 or more means the candidate list overflowed and was re-swept         */
+} orp_rnms_plan;
+int orp_rnms_last_plan(orp_rnms_plan *out);
 
 /* Measurement hooks: with timing on, orp_rnms brackets its dominant kernel (the sweep+clip
  * kernel) with CUDA events ON THE LAUNCHING STREAM; orp_rnms_last_sweep_ms waits for them and

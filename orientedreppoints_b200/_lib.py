@@ -10,7 +10,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "liborp_b200.so")
 
 ORP_NMS_EXACT64, ORP_NMS_COMPAT32 = 0, 1
-ORP_UNION_NAN_KEEPS, ORP_UNION_GUARD, ORP_UNION_NAN_SUPPRESSES = 0, 1, 2
+ORP_UNION_NAN_KEEPS, ORP_UNION_GUARD, ORP_UNION_NAN_SUPPRESSES, ORP_UNION_NAN_SUPPRESSES_ALL = 0, 1, 2, 3
 ORP_ORDER_INDEX_ASC, ORP_ORDER_SCORE_DESC = 0, 1
 
 _vp = ctypes.c_void_p
@@ -24,6 +24,15 @@ class NmsStats(ctypes.Structure):
                 ("pairs_clipped", ctypes.c_int64), ("pairs_fp64", ctypes.c_int64),
                 ("edges", ctypes.c_int64), ("suppressing", ctypes.c_int64), ("overflow", ctypes.c_int32),
                 ("rounds", ctypes.c_int32), ("n", ctypes.c_int32)]
+
+    def as_dict(self):
+        return {k: int(getattr(self, k)) for k, _ in self._fields_}
+
+
+class RnmsPlan(ctypes.Structure):
+    _fields_ = [(k, ctypes.c_int32) for k in ("lazy", "R", "seg_limit", "sweep_bits", "no_sync", "flags_out", "union_mode",
+                                              "order", "n")] + \
+              [("cap_first", ctypes.c_int64), ("cap_final", ctypes.c_int64), ("attempts", ctypes.c_int32)]
 
     def as_dict(self):
         return {k: int(getattr(self, k)) for k, _ in self._fields_}
@@ -61,6 +70,7 @@ SIGNATURES = {
     "orp_rnms": (_i, [_vp, _vp, _i, _d, _i, _i, _i, _vp, _vp, _vp]),
     "orp_poly_nms_host": (_i, [_vp, _vp, _vp, _i, _i, _f, _i]),
     "orp_rnms_last_stats": (_i, [ctypes.POINTER(NmsStats)]),
+    "orp_rnms_last_plan": (_i, [ctypes.POINTER(RnmsPlan)]),
     "orp_set_timing": (None, [_i]),
     "orp_rnms_last_sweep_ms": (_i, [ctypes.POINTER(ctypes.c_float)]),
     "orp_tc_timing_collect": (_i, [ctypes.POINTER(ctypes.c_float), ctypes.POINTER(_i), ctypes.POINTER(_d)]),
@@ -159,6 +169,13 @@ def last_nms_stats():
     s = NmsStats()
     check(lib().orp_rnms_last_stats(ctypes.byref(s)), "orp_rnms_last_stats")
     return s.as_dict()
+
+
+def rnms_last_plan():
+    """plan of this thread's most recent rotated NMS (dict of the orp_rnms_plan fields)"""
+    p = RnmsPlan()
+    check(lib().orp_rnms_last_plan(ctypes.byref(p)), "orp_rnms_last_plan")
+    return p.as_dict()
 
 
 def set_timing(on):

@@ -173,7 +173,7 @@ __device__ __forceinline__ T iou_from(const PairRes<T> &r, int union_mode)
 template <typename T>
 __device__ __forceinline__ bool suppresses(T iou, T thr, int union_mode)
 {
-    if (union_mode == ORP_UNION_NAN_SUPPRESSES) return !(iou <= thr);
+    if (union_mode == ORP_UNION_NAN_SUPPRESSES || union_mode == ORP_UNION_NAN_SUPPRESSES_ALL) return !(iou <= thr);
     return iou > thr;
 }
 

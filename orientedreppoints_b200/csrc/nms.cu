@@ -42,6 +42,12 @@ static thread_local orp_nms_stats g_last_stats;
 static thread_local cudaEvent_t g_ev[2] = {nullptr, nullptr};
 static thread_local NmsCounters *g_stats_dev = nullptr;   // device copy of the last call
 static thread_local NmsCounters *g_stats_pinned = nullptr;
+static thread_local orp_rnms_plan g_last_plan;
+static thread_local bool g_have_plan = false;
+
+// per-box `area` value of a quadrilateral whose fp64 signed area (ring_area<double>, the area of the fp64 decision) is
+// exactly zero; like every negative value it keeps the box out of the fp32 bounds and the fast path
+constexpr float kZeroArea = -2.0f;
 
 __device__ __forceinline__ uint32_t orderable(float f)
 {
@@ -68,7 +74,9 @@ nms_prep_kernel(const float *__restrict__ dets, const int32_t *__restrict__ segm
         finite = finite && isfinite(x[k]) && isfinite(y[k]);
     }
     float xmin = fminf(fminf(x[0], x[1]), fminf(x[2], x[3]));
-    score_key[i] = ~orderable(d[8]);                       // ascending key == descending score
+    // -0.0 and +0.0 are equal scores: one key, so that the tie rule (lower index first) holds between them
+    const float sc = (__float_as_uint(d[8]) << 1) == 0u ? 0.0f : d[8];
+    score_key[i] = ~orderable(sc);                         // ascending key == descending score
     uint32_t seg = segments ? (uint32_t)segments[i] : 0u;
     // non-finite boxes go to the very end of the sweep order and never take part in it
     uint64_t key = finite ? (((uint64_t)(seg & 0x7FFFFFFFu) << 32) | orderable(xmin)) : ~0ull;
@@ -90,6 +98,7 @@ nms_rank_kernel(const int32_t *__restrict__ order, int n, int32_t *__restrict__ 
 struct NmsGlobal {
     unsigned int ymin_key;        // orderable(min AABB ymin) over finite boxes
     unsigned int maxh_bits;       // float bits of the largest AABB height (non-negative: bit order == value order)
+    unsigned int maxabs_bits;     // float bits of the largest |coordinate|
     double sumh;                  // sum of AABB heights
     unsigned int count;           // finite boxes
 };
@@ -104,9 +113,9 @@ __global__ void __launch_bounds__(256)
 nms_boxes_kernel(const float *__restrict__ dets, int n, float4 *__restrict__ baabb, float4 *__restrict__ v01,
                  float4 *__restrict__ v23, float *__restrict__ area, NmsGlobal *__restrict__ G)
 {
-    __shared__ unsigned int s_ymin, s_maxh, s_cnt;
+    __shared__ unsigned int s_ymin, s_maxh, s_cnt, s_maxabs;
     __shared__ float s_sum;
-    if (threadIdx.x == 0) { s_ymin = 0xFFFFFFFFu; s_maxh = 0u; s_cnt = 0u; s_sum = 0.f; }
+    if (threadIdx.x == 0) { s_ymin = 0xFFFFFFFFu; s_maxh = 0u; s_cnt = 0u; s_sum = 0.f; s_maxabs = 0u; }
     __syncthreads();
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) {
@@ -126,8 +135,15 @@ nms_boxes_kernel(const float *__restrict__ dets, int n, float4 *__restrict__ baa
         const float ux = c[2] - c[0], uy = c[3] - c[1], vx = c[4] - c[0], vy = c[5] - c[1], wx = c[6] - c[0], wy = c[7] - c[1];
         area[i] = quad_is_convex(c) ? 0.5f * fabsf((ux * vy - uy * vx) + (vx * wy - vy * wx)) : -1.0f;
         if (finite) {
+            Pt<double> P[5];
+#pragma unroll
+            for (int k = 0; k < 4; ++k) { P[k].x = (double)c[2 * k]; P[k].y = (double)c[2 * k + 1]; }
+            if (ring_area(P, 4) == 0.0) area[i] = kZeroArea;
+        }
+        if (finite) {
             atomicMin(&s_ymin, orderable(ymin));
             atomicMax(&s_maxh, __float_as_uint(ymax - ymin));
+            atomicMax(&s_maxabs, __float_as_uint(fmaxf(fmaxf(fabsf(xmin), fabsf(xmax)), fmaxf(fabsf(ymin), fabsf(ymax)))));
             atomicAdd(&s_sum, ymax - ymin);
             atomicAdd(&s_cnt, 1u);
         }
@@ -136,6 +152,7 @@ nms_boxes_kernel(const float *__restrict__ dets, int n, float4 *__restrict__ baa
     if (threadIdx.x == 0 && s_cnt) {
         atomicMin(&G->ymin_key, s_ymin);
         atomicMax(&G->maxh_bits, s_maxh);
+        atomicMax(&G->maxabs_bits, s_maxabs);
         atomicAdd(&G->sumh, (double)s_sum);
         atomicAdd(&G->count, s_cnt);
     }
@@ -203,6 +220,58 @@ nms_slots_kernel(const uint64_t *__restrict__ keys, const int32_t *__restrict__ 
     const bool prev_valid = (s == 0) ? true : (keys[s - 1] != ~0ull);
     if (!valid && prev_valid) *nvalid = s;                   // first padding slot = number of registrations
     if (valid && s == m - 1) *nvalid = m;
+}
+
+// Zero-area lists (ORP_UNION_GUARD / ORP_UNION_NAN_SUPPRESSES_ALL): these conventions compare every pair, and for two
+// (near-)degenerate boxes the fp64 IoU is a ratio of rounding residues (NaN, -1 or anything), whatever their distance.
+// Such boxes are compared with each other explicitly: every one gets the segment's worse-ranked ones as implicit
+// candidates.  Degenerate = |fp64 signed area| <= 2^-36 S^2, S = the largest |coordinate| of the set: the shoelace sum of
+// a collinear ring rounds to at most a few 2^-53 S^2, and a fan residue (<= ~2^-47 S^2) over a box above the bound stays
+// far below any threshold, so pairs with one box above it need no explicit comparison.  Sort key per rank: the segment of
+// a finite degenerate box, `none` for every other box; a stable sort keeps rank order inside a segment.
+__global__ void __launch_bounds__(256)
+nms_zero_keys_kernel(const int32_t *__restrict__ order, const int32_t *__restrict__ segments, const float4 *__restrict__ v01,
+                     const float4 *__restrict__ v23, const NmsGlobal *__restrict__ G, int n, uint32_t none, float *__restrict__ area,
+                     uint32_t *__restrict__ keys)
+{
+    const int r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= n) return;
+    const int i = order[r];
+    const float4 a = v01[i], b = v23[i];
+    Pt<double> P[5];
+    P[0].x = a.x; P[0].y = a.y; P[1].x = a.z; P[1].y = a.w; P[2].x = b.x; P[2].y = b.y; P[3].x = b.z; P[3].y = b.w;
+    const double S = fmax(1.0, (double)__uint_as_float(G->maxabs_bits));
+    const bool deg = fabs(ring_area(P, 4)) <= ldexp(S * S, -36);      // NaN (non-finite box): false
+    if (deg) area[i] = kZeroArea;
+    keys[r] = deg ? (segments ? ((uint32_t)segments[i] & 0x7FFFFFFFu) : 0u) : none;
+}
+
+// sorted zero-area list -> per zero-area box: its list position, the end of its segment's run and how many better-ranked
+// zero-area boxes of its segment precede it (its extra pending count)
+__global__ void __launch_bounds__(256)
+nms_zero_list_kernel(const uint32_t *__restrict__ keys, const int32_t *__restrict__ zlist, int n, uint32_t none,
+                     int32_t *__restrict__ zpos, int32_t *__restrict__ zhi, int32_t *__restrict__ zbetter)
+{
+    const int p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= n) return;
+    const uint32_t k = keys[p];
+    if (k == none) return;
+    int a = 0, b = p;
+    while (a < b) { const int mid = (a + b) >> 1; if (keys[mid] < k) a = mid + 1; else b = mid; }
+    int c = p + 1, d = n;
+    while (c < d) { const int mid = (c + d) >> 1; if (keys[mid] <= k) c = mid + 1; else d = mid; }
+    const int box = zlist[p];
+    zpos[box] = p;
+    zhi[box] = c;
+    zbetter[box] = p - a;
+}
+
+// after the sweep (every attempt resets `pending`): a zero-area box also waits for the better zero-area boxes of its segment
+__global__ void __launch_bounds__(256)
+nms_zero_pending_kernel(const int32_t *__restrict__ zpos, const int32_t *__restrict__ zbetter, int n, int32_t *__restrict__ pending)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n && zpos[i] >= 0) pending[i] += zbetter[i];
 }
 
 // gather boxes into structure-of-arrays in `perm` order
@@ -395,7 +464,9 @@ nms_sweep_kernel(SweepParams P)
                     cont = (mj.x == grp_i) && (bb.x <= ba.z);
                     if (cont) {
                         ++c_swept;
-                        hit = (bb.x < ba.z) && (bb.y < ba.w) && (bb.w > ba.y);
+                        // the AABB intersection has positive area (py_cpu_nms_poly_fast's `hbb_ovr > 0`): a box with a
+                        // zero-width or zero-height AABB has zero area and pairs with nothing here (bb.x >= ba.x: sweep order)
+                        hit = (bb.x < ba.z) && (bb.z > bb.x) && (bb.y < ba.w) && (bb.w > ba.y) && (ba.w > ba.y) && (bb.w > bb.y);
                         // the pair belongs to the strip holding the top of the AABB intersection
                         if (hit && P.R > 1) hit = ((S.of(fmaxf(ba.y, bb.y)) & 0xFFFF) == strip_i);
                         if (hit) {
@@ -631,6 +702,8 @@ struct LazyParams {
     const float *area;
     double thr;
     int union_mode;
+    const int32_t *zlist, *zpos, *zhi;         // zero-area lists (NULL: none): a zero-area box j also has the worse zero-area
+                                               // boxes zlist[zpos[j] + 1 .. zhi[j]) of its segment as candidates
     int trace;                                 // ORP_NMS_TRACE=1: block 0 prints per-round frontier sizes and phase times
 };
 
@@ -679,36 +752,42 @@ nms_resolve_lazy_kernel(LazyParams P)
         for (unsigned int w = gwarp; w < nk + ns; w += nwarps) {
             const bool kept = w < nk;
             const int j = kept ? fk[w] : fs[w - nk];
-            const int b = P.offs[j], e = b + P.deg[j];
-            // four chunks of the list in flight per warp: the walk is a chain of dependent loads (entry -> status -> atomic)
-            for (int k0 = b; k0 < e; k0 += 128) {
-                int r[4];
-                bool act[4];
-#pragma unroll
-                for (int u = 0; u < 4; ++u) {
-                    const int k = k0 + 32 * u + lane;
-                    r[u] = k < e ? P.adj[k] : -1;
-                }
-#pragma unroll
-                for (int u = 0; u < 4; ++u) act[u] = r[u] >= 0 && *(volatile int32_t *)&P.status[r[u]] == 0;
-                if (kept) {
-#pragma unroll
+            // the out list, then (zero-area box) the rest of its segment's zero-area list
+            for (int pass = 0; pass < 2; ++pass) {
+                const int32_t *list = pass == 0 ? P.adj : P.zlist;
+                int b = 0, e = 0;
+                if (pass == 0) { b = P.offs[j]; e = b + P.deg[j]; }
+                else if (P.zpos && P.zpos[j] >= 0) { b = P.zpos[j] + 1; e = P.zhi[j]; }
+                // four chunks of the list in flight per warp: the walk is a chain of dependent loads (entry -> status -> atomic)
+                for (int k0 = b; k0 < e; k0 += 128) {
+                    int r[4];
+                    bool act[4];
+    #pragma unroll
                     for (int u = 0; u < 4; ++u) {
-                        const unsigned m = __ballot_sync(0xffffffffu, act[u]);
-                        if (m) {
-                            unsigned int base = 0;
-                            if (lane == 0) base = atomicAdd(qc, (unsigned int)__popc(m));
-                            base = __shfl_sync(0xffffffffu, base, 0);
-                            if (act[u]) P.queue[base + __popc(m & lt)] = make_int2(r[u], j);
-                        }
+                        const int k = k0 + 32 * u + lane;
+                        r[u] = k < e ? list[k] : -1;
                     }
-                } else {
-#pragma unroll
-                    for (int u = 0; u < 4; ++u)
-                        if (act[u] && atomicSub(&P.pending[r[u]], 1) == 1) {
-                            P.status[r[u]] = 1;
-                            fk_next[atomicAdd(&P.counts[nxt], 1u)] = r[u];
+    #pragma unroll
+                    for (int u = 0; u < 4; ++u) act[u] = r[u] >= 0 && *(volatile int32_t *)&P.status[r[u]] == 0;
+                    if (kept) {
+    #pragma unroll
+                        for (int u = 0; u < 4; ++u) {
+                            const unsigned m = __ballot_sync(0xffffffffu, act[u]);
+                            if (m) {
+                                unsigned int base = 0;
+                                if (lane == 0) base = atomicAdd(qc, (unsigned int)__popc(m));
+                                base = __shfl_sync(0xffffffffu, base, 0);
+                                if (act[u]) P.queue[base + __popc(m & lt)] = make_int2(r[u], j);
+                            }
                         }
+                    } else {
+    #pragma unroll
+                        for (int u = 0; u < 4; ++u)
+                            if (act[u] && atomicSub(&P.pending[r[u]], 1) == 1) {
+                                P.status[r[u]] = 1;
+                                fk_next[atomicAdd(&P.counts[nxt], 1u)] = r[u];
+                            }
+                    }
                 }
             }
         }
@@ -746,7 +825,9 @@ nms_resolve_lazy_kernel(LazyParams P)
                     HA.c[k] = __shfl_sync(0xffffffffu, A.c[k], src);
                     HB.c[k] = __shfl_sync(0xffffffffu, B.c[k], src);
                 }
-                const bool s = decide_fp64_warp(HA, HB, P.thr, P.union_mode, lane);
+                // better-ranked box first, as the reference's loops call it: for degenerate pairs the fan sum's rounding
+                // residue, and with it the IoU, depends on the order
+                const bool s = decide_fp64_warp(HB, HA, P.thr, P.union_mode, lane);
                 if (lane == src) { res = s ? 1 : 0; ++c_64; }
             }
             if (!valid) continue;
@@ -813,14 +894,21 @@ int run_nms(const float *dets, const int32_t *segments, int n, double thr, int i
     if (n < 0 || (!flags_out && !num_out) || (n > 0 && (!dets || (!flags_out && !keep_out))))
         return fail(ORP_EINVAL, "orp_rnms: null pointer or negative n");
     if (iou_mode != ORP_NMS_EXACT64 && iou_mode != ORP_NMS_COMPAT32) return fail(ORP_EINVAL, "orp_rnms: bad iou_mode");
-    if (union_mode < 0 || union_mode > 2) return fail(ORP_EINVAL, "orp_rnms: bad union_mode");
+    if (union_mode < 0 || union_mode > 3) return fail(ORP_EINVAL, "orp_rnms: bad union_mode");
     int rc = ensure_device();
     if (rc) return rc;
+    const bool lazy = (iou_mode == ORP_NMS_EXACT64);
+    memset(&g_last_plan, 0, sizeof(g_last_plan));
+    g_last_plan.lazy = lazy; g_last_plan.seg_limit = seg_limit; g_last_plan.no_sync = no_sync; g_last_plan.flags_out = flags_out != nullptr;
+    g_last_plan.union_mode = union_mode; g_last_plan.order = order; g_last_plan.n = n;
+    g_have_plan = true;
     if (n == 0) {
         if (num_out) ORP_CUDA(cudaMemsetAsync(num_out, 0, sizeof(int32_t), st));
         return ORP_OK;
     }
-    const bool lazy = (iou_mode == ORP_NMS_EXACT64);
+    // conventions that compare every pair: two zero-area boxes may suppress each other wherever they are (orp_b200.h), so
+    // they are candidates of each other although the sweep never pairs them
+    const bool zero_rule = lazy && (union_mode == ORP_UNION_GUARD || union_mode == ORP_UNION_NAN_SUPPRESSES_ALL);
     // Registration slots per box.  Large single sets (the poly_nms sweep: 10^5 boxes in one segment) are cut into y strips
     // so that a box only meets the boxes of its own strips while walking its x interval; many small segments (a tile:
     // 5 344 boxes per (image, class)) do not need them.  Segment ids must fit 15 bits next to the 16-bit strip index.
@@ -837,6 +925,14 @@ int run_nms(const float *dets, const int32_t *segments, int n, double thr, int i
         sweep_bits = (R == 1 ? 32 : 48) + sb;
         if (sweep_bits > 64) sweep_bits = 64;
     }
+    // candidate-pair buffer: grows on overflow (one retry costs a host sync; sized to make that rare).  Callers that
+    // forbid the host round trip (no_sync) get the overflow reported on the device through overflow_out instead.
+    unsigned long long cap = (unsigned long long)n * 256ull;
+    if (cap < (1ull << 20)) cap = 1ull << 20;
+    const unsigned long long all_pairs = (unsigned long long)n * (unsigned long long)(n - 1) / 2ull;
+    if (cap > all_pairs) cap = all_pairs ? all_pairs : 1;
+    g_last_plan.R = R; g_last_plan.sweep_bits = sweep_bits;
+    g_last_plan.cap_first = g_last_plan.cap_final = (int64_t)cap;
     Scratch S(st);
     const int T = 256, G = ceil_div(n, T), GM = ceil_div(m, T);
     uint32_t *score_key = S.get<uint32_t>(n), *score_key2 = S.get<uint32_t>(n);
@@ -854,18 +950,30 @@ int run_nms(const float *dets, const int32_t *segments, int n, double thr, int i
     unsigned int *qcount = S.get<unsigned int>(6);                // frontier / queue fills of the lazy resolve
     int32_t *worklist = lazy ? S.get<int32_t>(4 * (size_t)n) : nullptr;   // kept and suppressed frontiers, [2][n] each
     int32_t *status32 = lazy ? S.get<int32_t>(n) : nullptr, *pending = lazy ? S.get<int32_t>(n) : nullptr;
+    int32_t *zlist = zero_rule ? S.get<int32_t>(n) : nullptr, *zpos = zero_rule ? S.get<int32_t>(n) : nullptr;
+    int32_t *zhi = zero_rule ? S.get<int32_t>(n) : nullptr, *zbetter = zero_rule ? S.get<int32_t>(n) : nullptr;
     NmsGlobal *glob = S.get<NmsGlobal>(1);
     NmsCounters *ctr = S.get<NmsCounters>(1);
-    if (!ctr || !vals || !changed || !qcount || !glob || (lazy && (!worklist || !status32 || !pending || !meta_s))) return fail(ORP_ECUDA, "orp_rnms: scratch allocation failed");
+    if (!ctr || !vals || !changed || !qcount || !glob || (lazy && (!worklist || !status32 || !pending || !meta_s)) || (zero_rule && (!zlist || !zpos || !zhi || !zbetter))) return fail(ORP_ECUDA, "orp_rnms: scratch allocation failed");
 
-    size_t tb1 = 0, tb2 = 0, tb3 = 0, tb4 = 0;
+    // zero-area list sort: as many key bits as the segment ids need, plus the all-ones `none` key of every other box
+    int zbits = 32;
+    if (seg_limit > 0) {
+        zbits = 1;
+        while ((1ll << zbits) <= (long long)seg_limit) ++zbits;
+        if (zbits > 32) zbits = 32;
+    }
+    const uint32_t znone = zbits == 32 ? 0xFFFFFFFFu : (uint32_t)((1ull << zbits) - 1);
+    size_t tb1 = 0, tb2 = 0, tb3 = 0, tb4 = 0, tb5 = 0;
     cub::DeviceRadixSort::SortPairs(nullptr, tb1, score_key, score_key2, iota, order_r, n, 0, 32, st);
+    if (zero_rule) cub::DeviceRadixSort::SortPairs(nullptr, tb5, score_key, score_key2, order_r, zlist, n, 0, zbits, st);
     cub::DeviceRadixSort::SortPairs(nullptr, tb2, sweep_key, sweep_key2, iota, perm, m, 0, sweep_bits, st);
     cub::DeviceScan::ExclusiveSum(nullptr, tb3, indeg, offs, n + 1, st);
     if (keep_out && num_out) cub::DeviceSelect::Flagged(nullptr, tb4, vals, flags, keep_out, num_out, n, st);
     size_t tb = tb1 > tb2 ? tb1 : tb2;
     tb = tb > tb3 ? tb : tb3;
     tb = tb > tb4 ? tb : tb4;
+    tb = tb > tb5 ? tb : tb5;
     uint8_t *tmp = S.get<uint8_t>(tb);
     if (!tmp) return fail(ORP_ECUDA, "orp_rnms: scratch allocation failed");
 
@@ -879,9 +987,10 @@ int run_nms(const float *dets, const int32_t *segments, int n, double thr, int i
         ORP_CUDA(cudaMemsetAsync(status32, 0, sizeof(int32_t) * (size_t)n, st));
         ORP_CUDA(cudaMemsetAsync(pending, 0, sizeof(int32_t) * (size_t)n, st));
     }
+    if (zero_rule) ORP_CUDA(cudaMemsetAsync(zpos, 0xFF, sizeof(int32_t) * (size_t)n, st));   // -1: not a zero-area box
     {
         NmsGlobal g0;
-        g0.ymin_key = 0xFFFFFFFFu; g0.maxh_bits = 0u; g0.sumh = 0.0; g0.count = 0u;
+        g0.ymin_key = 0xFFFFFFFFu; g0.maxh_bits = 0u; g0.maxabs_bits = 0u; g0.sumh = 0.0; g0.count = 0u;
         static thread_local NmsGlobal g0_host;                    // source of an async copy must outlive the call
         g0_host = g0;
         ORP_CUDA(cudaMemcpyAsync(glob, &g0_host, sizeof(NmsGlobal), cudaMemcpyHostToDevice, st));
@@ -894,15 +1003,11 @@ int run_nms(const float *dets, const int32_t *segments, int n, double thr, int i
     nms_rank_kernel<<<G, T, 0, st>>>(order_r, n, rank);
     ORP_LAUNCHED();
 
-    // candidate-pair buffer: grows on overflow (one retry costs a host sync; sized to make that rare).  Callers that
-    // forbid the host round trip (no_sync) get the overflow reported on the device through overflow_out instead.
-    unsigned long long cap = (unsigned long long)n * 256ull;
-    if (cap < (1ull << 20)) cap = 1ull << 20;
-    const unsigned long long all_pairs = (unsigned long long)n * (unsigned long long)(n - 1) / 2ull;
-    if (cap > all_pairs) cap = all_pairs ? all_pairs : 1;
-
     for (int attempt = 0; attempt < 6; ++attempt) {
-        int2 *edges = S.get<int2>(cap);
+        g_last_plan.attempts = attempt + 1;
+        g_last_plan.cap_final = (int64_t)cap;
+        // the buffer turns into the resolve's work queue; the zero-area lists can add one pair per box and round to it
+        int2 *edges = S.get<int2>(cap + (zero_rule ? (unsigned long long)n : 0ull));
         if (!edges) return fail(ORP_ECUDA, "orp_rnms: edge buffer allocation failed");
         if (lazy) {
             if (attempt == 0) {
@@ -914,6 +1019,15 @@ int run_nms(const float *dets, const int32_t *segments, int n, double thr, int i
                 count_launches((sweep_bits + 7) / 8);
                 nms_slots_kernel<<<GM, T, 0, st>>>(sweep_key2, perm, baabb, area, rank, m, aabb, meta_s, nvalid);
                 ORP_LAUNCHED();
+                if (zero_rule) {
+                    // score keys are free after the rank sort: they carry the zero-area list keys
+                    nms_zero_keys_kernel<<<G, T, 0, st>>>(order_r, segments, v01, v23, glob, n, znone, area, score_key);
+                    ORP_LAUNCHED();
+                    ORP_CUDA(cub::DeviceRadixSort::SortPairs(tmp, tb5, score_key, score_key2, order_r, zlist, n, 0, zbits, st));
+                    count_launches((zbits + 7) / 8);
+                    nms_zero_list_kernel<<<G, T, 0, st>>>(score_key2, zlist, n, znone, zpos, zhi, zbetter);
+                    ORP_LAUNCHED();
+                }
             }
             SweepParams P{aabb, meta_s, v01, v23, nvalid, glob, R, edges, indeg, pending, cap, ctr, thr, union_mode};
             int grid = ceil_div(m, kSweepWarps);
@@ -958,6 +1072,10 @@ int run_nms(const float *dets, const int32_t *segments, int n, double thr, int i
     }
     // the loop above leaves `edges` as the last buffer obtained from S
     int2 *edges = static_cast<int2 *>(S.ptrs[S.n - 1]);
+    if (zero_rule) {
+        nms_zero_pending_kernel<<<G, T, 0, st>>>(zpos, zbetter, n, pending);
+        ORP_LAUNCHED();
+    }
 
     ORP_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tb3, indeg, offs, n + 1, st));
     count_launches(2);
@@ -981,7 +1099,8 @@ int run_nms(const float *dets, const int32_t *segments, int n, double thr, int i
             // the candidate buffer is free once scattered into the CSR: it becomes the work queue; after the scatter
             // `cursor` holds every list's length
             LazyParams LP{offs, adj, cursor, n, status32, pending, ctr, qcount, worklist, worklist + 2 * (size_t)n, edges,
-                          baabb, v01, v23, area, thr, union_mode, getenv("ORP_NMS_TRACE") ? 1 : 0};
+                          baabb, v01, v23, area, thr, union_mode, zlist, zero_rule ? zpos : nullptr, zhi,
+                          getenv("ORP_NMS_TRACE") ? 1 : 0};
             void *args[] = {&LP};
             ORP_CUDA(cudaLaunchCooperativeKernel((void *)nms_resolve_lazy_kernel, dim3(grid), dim3(256), args, 0, st));
             ORP_LAUNCHED();
@@ -1054,6 +1173,14 @@ extern "C" int orp_rnms_last_stats(orp_nms_stats *out)
     out->overflow = c.overflow;
     out->rounds = c.rounds;
     out->n = orp::g_last_stats.n;
+    return ORP_OK;
+}
+
+extern "C" int orp_rnms_last_plan(orp_rnms_plan *out)
+{
+    if (!out) return orp::fail(ORP_EINVAL, "orp_rnms_last_plan: null");
+    if (!orp::g_have_plan) return orp::fail(ORP_EINVAL, "orp_rnms_last_plan: no previous call");
+    *out = orp::g_last_plan;
     return ORP_OK;
 }
 

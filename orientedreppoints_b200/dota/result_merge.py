@@ -25,7 +25,7 @@ _PAT_XY = re.compile(r'__\d+___\d+')
 _PAT_RATE = re.compile(r'__([\d+\.]+)__\d+___')
 
 
-def _nms_segmented(dets, thresh, segments=None, device=None):
+def _nms_segmented(dets, thresh, segments=None, device=None, union_mode=_lib.ORP_UNION_NAN_SUPPRESSES):
     dev = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
     dets = np.asarray(dets)
     if dets.dtype == np.float64 and dets.shape[0]:
@@ -43,20 +43,26 @@ def _nms_segmented(dets, thresh, segments=None, device=None):
         dets[:, 1:8:2] -= np.floor(oy[seg_ids])[:, None]
     d = torch.from_numpy(np.ascontiguousarray(dets, dtype=np.float32)).to(dev)
     seg = None if segments is None else torch.from_numpy(np.ascontiguousarray(segments, dtype=np.int32)).to(dev)
-    keep = rnms_indices(d, float(thresh), segments=seg, mode="exact64", union_mode=_lib.ORP_UNION_NAN_SUPPRESSES,
-                        order=_lib.ORP_ORDER_SCORE_DESC)
+    keep = rnms_indices(d, float(thresh), segments=seg, mode="exact64", union_mode=union_mode, order=_lib.ORP_ORDER_SCORE_DESC)
     return keep.cpu().numpy()
 
 
 def py_cpu_nms_poly(dets, thresh):
-    """dets: ndarray [N,9] (x1..y4, score) -> list of kept indices in score-descending selection order."""
+    """ResultMerge.py:18-41.  dets: ndarray [N,9] (x1..y4, score) -> list of kept indices in score-descending selection
+    order.  Every pair is compared, so two zero-area boxes (union 0, NaN IoU) suppress each other wherever they are."""
+    dets = np.asarray(dets)
+    if dets.shape[0] == 0:
+        return []
+    return [int(i) for i in _nms_segmented(dets, thresh, union_mode=_lib.ORP_UNION_NAN_SUPPRESSES_ALL)]
+
+
+def py_cpu_nms_poly_fast(dets, thresh):
+    """ResultMerge_multi_process.py:60-121: as py_cpu_nms_poly, but a pair is only compared when the axis-aligned hulls
+    overlap with positive area (the kernel's sweep prefilter), so zero-area boxes apart from each other are all kept."""
     dets = np.asarray(dets)
     if dets.shape[0] == 0:
         return []
     return [int(i) for i in _nms_segmented(dets, thresh)]
-
-
-py_cpu_nms_poly_fast = py_cpu_nms_poly      # the AABB prefilter of the reference's _fast variant is built into the kernel
 
 
 def poly2origpoly(poly, x, y, rate):

@@ -35,3 +35,21 @@ def test_sass_is_sm90a_only():
     out = subprocess.run(["cuobjdump", "--list-elf", _lib.LIB_PATH], capture_output=True, text=True).stdout
     archs = set(re.findall(r"sm_(\d+a?)", out))
     assert archs == {"90a"}, archs
+
+
+def test_rnms_plan_record_matches_header():
+    """orp_rnms_last_plan is declared, exported and bound, and RnmsPlan has the header's fields in the header's order"""
+    import ctypes
+    assert "orp_rnms_last_plan" in _declared()
+    assert hasattr(_lib.lib(), "orp_rnms_last_plan")
+    src = open(os.path.join(ROOT, "include", "orp_b200.h")).read()
+    body = re.search(r"typedef struct \{([^}]*)\} orp_rnms_plan;", src).group(1)
+    body = re.sub(r"/\*.*?\*/", "", body, flags=re.S)
+    fields = []
+    for decl in body.split(";"):
+        m = re.match(r"\s*(int32_t|int64_t)\s+(.*)", decl, flags=re.S)
+        if m:
+            fields += [(n.strip(), m.group(1)) for n in m.group(2).split(",")]
+    want = {"int32_t": ctypes.c_int32, "int64_t": ctypes.c_int64}
+    assert [(n, want[t]) for n, t in fields] == list(_lib.RnmsPlan._fields_)
+    assert ctypes.sizeof(_lib.RnmsPlan) == 64

@@ -1,6 +1,8 @@
 """GPU: rotated NMS at the sizes the hot path and BASELINE.json configs[2] name - 80 160 candidates in 15 class segments
 (one 1024x1024 tile), 100 000 and 200 000 proposals - keep lists bit-exact against the CPU oracle's restatement of the
-reference's py_cpu_nms_poly_fast (ResultMerge_multi_process.py:60-121; pinned to the reference's compiled polyiou)."""
+reference's py_cpu_nms_poly_fast (ResultMerge_multi_process.py:60-121; pinned to the reference's compiled polyiou).
+These run `orp_rnms` through rnms_indices, not poly_gpu_nms: the unsegmented 100k / 200k sets are cut into y strips, the
+tile-load case (segments without a known bound) is not.  tests/test_nms_plans_gpu.py covers poly_gpu_nms and the other plans."""
 import numpy as np
 import pytest
 import torch
