@@ -18,3 +18,21 @@ model = dict(
                    norm_cfg=norm_cfg, top_ratio=0.4, **_losses))
 test_cfg = dict(nms_pre=2000, min_bbox_size=0, score_thr=0.05, nms=dict(type='rnms', iou_thr=0.4), max_per_img=2000)
 img_norm_cfg = dict(mean=[123.675, 116.28, 103.53], std=[58.395, 57.12, 57.375], to_rgb=True)
+# test-time pipeline of the reference config (test_pipeline / data.test.pipeline): run on the device by
+# orientedreppoints_b200.datasets.pipelines (Normalize and Pad are fused into the stem / patch-embed input transform)
+test_pipeline = [
+    dict(type='LoadImageFromFile'),
+    dict(
+        type='MultiScaleFlipAug',
+        img_scale=(1333, 1024),
+        flip=False,
+        transforms=[
+            dict(type='RotateResize', keep_ratio=True),
+            dict(type='RotateRandomFlip'),
+            dict(type='Normalize', **img_norm_cfg),
+            dict(type='Pad', size_divisor=32),
+            dict(type='ImageToTensor', keys=['img']),
+            dict(type='Collect', keys=['img']),
+        ])
+]
+data = dict(test=dict(pipeline=test_pipeline))

@@ -350,6 +350,10 @@ int orp_f16x3_overflow_count(unsigned int *count, int reset);
  * tiles (Normalize fused) or the NCHW fp32 image, conv1 as a 4x4 stride-1 convolution over them */
 int orp_stem_s2d_u8_f16x3(const uint8_t *img_hwc, int N, int H, int W, const float *mean, const float *std, int to_rgb,
                           void *out, void *stream);
+/* the same with a per-image valid extent: valid_hw device int32 [N,2] = (h, w); pixels at y >= h or x >= w are the
+ * pipeline's Pad after Normalize and enter the stem as exactly 0.0 (h, w may be odd) */
+int orp_stem_s2d_u8_padded_f16x3(const uint8_t *img_hwc, int N, int H, int W, const float *mean, const float *std, int to_rgb,
+                                 const int32_t *valid_hw, void *out, void *stream);
 int orp_stem_s2d_f16x3(const float *img_nchw, int N, int H, int W, void *out, void *stream);
 int orp_stem_conv_s2d_f16x3(const void *x_s2d, int N, int H, int W, const void *w_split, const float *bias,
                             int wscale_log2, int relu, void *out, void *stream);
@@ -384,6 +388,9 @@ int orp_stem_conv_s2d_bf16(const void *x_s2d, int N, int H, int W, const void *w
  * to_rgb swaps the image's channel order) fused in: a step uploads 3 bytes per pixel instead of 12 */
 int orp_stem_s2d_u8_bf16(const uint8_t *img_hwc, int N, int H, int W, const float *mean, const float *std, int to_rgb,
                          void *out, void *stream);
+/* the same with a per-image valid extent (device int32 [N,2] = (h, w)); outside it the input is exactly 0.0 */
+int orp_stem_s2d_u8_padded_bf16(const uint8_t *img_hwc, int N, int H, int W, const float *mean, const float *std, int to_rgb,
+                                const int32_t *valid_hw, void *out, void *stream);
 int orp_maxpool3x3s2_bf16(const void *x, int N, int H, int W, int C, void *y, void *stream);
 /* GroupNorm over bf16 NHWC with C = 256, 32 groups: statistics (double [N,32,2], zeroed by caller) + apply */
 int orp_gn_stats_bf16(const void *x, int N, int HW, int C, int groups, double *stats, void *stream);
@@ -416,6 +423,18 @@ int orp_split_tiles_u8(const uint8_t *img_hwc, int H, int W, int C, const int32_
                        uint8_t *out, void *stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Test-pipeline Resize -> RandomFlip -> Pad (mmdet/datasets/pipelines/transforms.py RotateResize(keep_ratio) /
+ * RotateRandomFlip / Pad): batched uint8 HWC bilinear resize [N,H,W,C] -> [N,Hd,Wd,C], bit-identical to
+ * cv2.resize(INTER_LINEAR) (what mmcv.imrescale calls), optionally mirrored horizontally AFTER the resize, written into
+ * dst [N,Hp,Wp,C] with zeros outside [Hd,Wd].  The coefficients are cv2's, computed on the host in float32
+ * (orientedreppoints_b200/datasets/pipelines.py resize_tables); the kernel is integer-only.
+ * xtab: device int32 [Wd][4] = (x0, x1, a0, a1); ytab: device int32 [Hd][4] = (y0, y1, b0, b1), indices already clamped,
+ * weights scaled by 2048; both 16-byte aligned.  1 <= C <= 4, Hd <= Hp <= 65535, Wd <= Wp.
+ * ---------------------------------------------------------------------------------------- */
+int orp_resize_u8(const uint8_t *src, int N, int H, int W, int C, uint8_t *dst, int Hd, int Wd, int Hp, int Wp, int flip,
+                  const int32_t *xtab, const int32_t *ytab, void *stream);
+
+/* ------------------------------------------------------------------------------------------
  * Swin-T backbone pieces (mmdet/models/backbones/swin_transformer.py); the Linear layers are
  * orp_conv2d_bf16 1x1 convolutions (relu = 2 selects the exact GELU epilogue)
  * ---------------------------------------------------------------------------------------- */
@@ -437,6 +456,9 @@ int orp_patch_embed_rows_bf16(const float *img_nchw, int B, int H, int W, void *
  * HOST arrays of 3 floats) and ImageToTensor fused in (mmdet/datasets/pipelines/transforms.py Normalize, formating.py ImageToTensor) */
 int orp_patch_embed_rows_u8_bf16(const uint8_t *img_hwc, int B, int H, int W, const float *mean, const float *stdinv, int to_rgb,
                                  void *out, void *stream);
+/* the same with a per-image valid extent (device int32 [B,2] = (h, w)); outside it the input is exactly 0.0 (Pad after Normalize) */
+int orp_patch_embed_rows_u8_padded_bf16(const uint8_t *img_hwc, int B, int H, int W, const float *mean, const float *stdinv,
+                                        int to_rgb, const int32_t *valid_hw, void *out, void *stream);
 /* PatchMerging gather (:288-293): [B,H,W,C] -> [B,ceil(H/2),ceil(W/2),4C] */
 int orp_patch_merge_gather_bf16(const void *x, int B, int H, int W, int C, void *y, void *stream);
 /* F.max_pool2d(x, 1, stride=2) (necks/fpn.py:163-165): [B,H,W,C] -> [B,ceil(H/2),ceil(W/2),C] */
@@ -449,6 +471,8 @@ int orp_window_attention_f16x3(const void *qkv, int B, int H, int W, int Hp, int
 int orp_patch_embed_rows_f16x3(const float *img_nchw, int B, int H, int W, void *out, void *stream);
 int orp_patch_embed_rows_u8_f16x3(const uint8_t *img_hwc, int B, int H, int W, const float *mean, const float *stdinv, int to_rgb,
                                   void *out, void *stream);
+int orp_patch_embed_rows_u8_padded_f16x3(const uint8_t *img_hwc, int B, int H, int W, const float *mean, const float *stdinv,
+                                         int to_rgb, const int32_t *valid_hw, void *out, void *stream);
 int orp_patch_merge_gather_f16x3(const void *x, int B, int H, int W, int C, void *y, void *stream);
 int orp_subsample2_f16x3(const void *x, int B, int H, int W, int C, void *y, void *stream);
 

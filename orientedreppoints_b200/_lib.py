@@ -119,6 +119,11 @@ SIGNATURES = {
     "orp_stem_s2d_bf16": (_i, [_vp, _i, _i, _i, _vp, _vp]),
     "orp_convex_iou": (_i, [_vp, _i, _vp, _i, _vp, _vp]),
     "orp_split_tiles_u8": (_i, [_vp, _i, _i, _i, _vp, _i, _i, _vp, _vp]),
+    "orp_resize_u8": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
+    "orp_stem_s2d_u8_padded_bf16": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, _vp, _vp, _vp]),
+    "orp_stem_s2d_u8_padded_f16x3": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, _vp, _vp, _vp]),
+    "orp_patch_embed_rows_u8_padded_bf16": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, _vp, _vp, _vp]),
+    "orp_patch_embed_rows_u8_padded_f16x3": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, _vp, _vp, _vp]),
     "orp_stem_s2d_u8_bf16": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, _vp, _vp]),
     "orp_stem_conv_s2d_bf16": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, _vp, _vp]),
     "orp_maxpool3x3s2_bf16": (_i, [_vp, _i, _i, _i, _i, _vp, _vp]),

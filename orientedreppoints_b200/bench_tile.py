@@ -217,6 +217,80 @@ def run_config(backbone, precision, batch, args, rank, world, local, benchmod, f
     return out, det, img
 
 
+def _config_test_pipeline(backbone):
+    """test_pipeline of configs/dota/orientedrepoints_<backbone>_demo.py"""
+    import importlib.util
+    import os
+    path = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "configs", "dota",
+                        "orientedrepoints_%s_demo.py" % backbone)
+    spec = importlib.util.spec_from_file_location("_orp_bench_cfg_" + backbone, path)
+    mod = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(mod)
+    return mod.test_pipeline
+
+
+def run_test_scale(backbone, precision, batch, args, rank, world, local, benchmod, flush, steps=None):
+    """one configuration at its config's test scale: decoded 1024x1024 uint8 tiles resident on the device -> the config's
+    test pipeline on the device (cv2-exact resize to 960^2 + pad, one orp_resize_u8 launch) -> the detector (dense graph
+    replayed as a CUDA graph with the valid extents, fused post-processing, rescale=True back to tile coordinates).  Every
+    step is timed with CUDA events, L2 flushed between steps; the resize kernel is also timed on its own."""
+    from .datasets.pipelines import resize_u8, run_test_pipeline
+    dev = torch.device("cuda", local)
+    depth, det = build_detector(backbone, precision, dev)
+    pipe = _config_test_pipeline(backbone)
+    g = torch.Generator().manual_seed(2000 + rank)
+    tiles = torch.randint(0, 256, (batch, 1024, 1024, 3), generator=g, dtype=torch.uint8).to(dev)
+    steps = steps or max(3, min(args.steps, 10))
+
+    def step():
+        data = run_test_pipeline(pipe, tiles, device=dev)
+        (view,), (metas,), (valid,) = data["img"], data["img_meta"], data["valid_hw"]
+        return det.simple_test(view, metas, rescale=True, return_tensors="padded", valid_hw=valid), view, metas
+
+    _, view, metas = step()
+    if not getattr(args, "no_graph", False):
+        det.capture(view.shape, view.dtype, padded=True)
+    for _ in range(3):
+        out, _, _ = step()
+    benchmod.barrier(world)
+    ev = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(steps)]
+    for s in range(steps):
+        flush.fill_(s & 0xFF)
+        ev[s][0].record()
+        out, _, _ = step()
+        ev[s][1].record()
+    benchmod.barrier(world)
+    ms = benchmod.max_over_ranks(sum(a.elapsed_time(b) for a, b in ev) / steps, world)
+    counts = out[2].tolist()
+    hd, wd = metas[0]["img_shape"][:2]
+    hp, wp = metas[0]["pad_shape"][:2]
+    # the resize kernel alone, same shapes, into a preallocated buffer
+    dst = torch.empty((batch, hp, wp, 3), dtype=torch.uint8, device=dev)
+    resize_u8(tiles, (hd, wd), (hp, wp), False, out=dst)
+    rev = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(steps)]
+    for s in range(steps):
+        flush.fill_(s & 0xFF)
+        rev[s][0].record()
+        resize_u8(tiles, (hd, wd), (hp, wp), False, out=dst)
+        rev[s][1].record()
+    torch.cuda.synchronize()
+    r_ms = sum(a.elapsed_time(b) for a, b in rev) / steps
+    r_bytes = batch * 3 * (1024 * 1024 + hp * wp)
+    pk = benchmod.peaks()
+    del det
+    torch.cuda.empty_cache()
+    return {"workload": "%s FPN OrientedRepPoints, %d synthetic 1024x1024 uint8 tiles per GPU per step through the config's test "
+                        "pipeline on the device (resize to %dx%d, pad to %dx%d) and simple_test(rescale=True), %s arithmetic"
+                        % ("Swin-T" if depth == "swin_tiny" else "R-%d" % depth, batch, hd, wd, hp, wp, precision),
+            "value": world * batch / (ms * 1e-3), "unit": "tiles/s", "n_gpus": world, "steps": steps, "ms_per_step": ms,
+            "tiles_per_gpu_per_step": batch, "img_shape": [hd, wd], "pad_shape": [hp, wp],
+            "scale_factor": metas[0]["scale_factor"], "detections_per_tile": counts[:4],
+            "resize_kernel": {"ms_per_step": r_ms, "bytes_per_step": r_bytes, "GBps": r_bytes / (r_ms * 1e-3) / 1e9,
+                              "hbm_peak_GBps": pk["hbm_gbs"], "frac_of_hbm_peak": r_bytes / (r_ms * 1e-3) / 1e9 / pk["hbm_gbs"],
+                              "peak_source": pk["source"],
+                              "bytes": "uint8 source tiles read once + padded destination written once"}}
+
+
 def run(args, rank, world, local, benchmod):
     dev = torch.device("cuda", local)
     batch = args.batch or 16     # tiles per GPU per step: 8 -> 16 amortises the fixed cost of the small late-backbone launches (+11 %)
@@ -392,4 +466,12 @@ def run(args, rank, world, local, benchmod):
         except Exception as ex:                                   # never lose the headline line to an extra
             cfgs["error"] = repr(ex)
         line["configs"] = cfgs
+        # the same two configurations at their configs' test scale (1024^2 tiles -> 960^2) through the device test pipeline
+        ts = {}
+        try:
+            ts["r101_b4_per_gpu"] = run_test_scale("r101", precision, 4, args, rank, world, local, benchmod, flush)
+            ts["swin_tiny_b8_per_gpu"] = run_test_scale("swin_tiny", precision, 8, args, rank, world, local, benchmod, flush)
+        except Exception as ex:                                   # never lose the headline line to an extra
+            ts["error"] = repr(ex)
+        line["test_scale"] = ts
     return line

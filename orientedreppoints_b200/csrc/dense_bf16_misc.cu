@@ -272,9 +272,11 @@ stem_s2d_kernel(const float *__restrict__ img, int N, int H, int W, __nv_bfloat1
 // Normalize step of the test pipeline (mmdet/datasets/pipelines/transforms.py Normalize -> mmcv.imnormalize:
 // optional BGR->RGB, (x - mean) * (1/std) in fp32) is applied on the fly, so a step uploads 3 bytes per pixel
 // instead of 12.  mean / stdinv are indexed by MODEL channel c; model channel c is image channel (to_rgb ? 2-c : c).
+// valid (int32 [N,2] = (h, w) per image, or null for the full extent): pixels at y >= h or x >= w are the Pad step
+// that follows Normalize in the pipeline and contribute exactly 0.0.
 __global__ void __launch_bounds__(256)
 stem_s2d_u8_kernel(const uint8_t *__restrict__ img, int N, int H, int W, float3 mean, float3 stdinv, int to_rgb,
-                   __nv_bfloat16 *__restrict__ out)
+                   const int32_t *__restrict__ valid, __nv_bfloat16 *__restrict__ out)
 {
     const int Hp = H / 2 + 3, Wp = W / 2 + 3;
     const size_t total = (size_t)N * Hp * Wp;
@@ -287,24 +289,27 @@ stem_s2d_u8_kernel(const uint8_t *__restrict__ img, int N, int H, int W, float3 
         float v[16];
 #pragma unroll
         for (int k = 0; k < 16; ++k) v[k] = 0.f;
-        if (x0 >= 0 && x0 + 1 < W) {
+        const int vh = valid ? min(valid[2 * n], H) : H, vw = valid ? min(valid[2 * n + 1], W) : W;
+        if (x0 >= 0 && x0 < vw) {
 #pragma unroll
             for (int dy = 0; dy < 2; ++dy) {
                 const int y = y0 + dy;
-                if (y < 0 || y >= H) continue;
-                const uint8_t *p = img + (((size_t)n * H + y) * W + x0) * 3;     // 6 bytes: two pixels
+                if (y < 0 || y >= vh) continue;
+                const uint8_t *p = img + (((size_t)n * H + y) * W + x0) * 3;     // 6 bytes: two pixels (W is even)
                 // x0 even -> the 6 bytes start at an even address
                 const uint16_t a = *reinterpret_cast<const uint16_t *>(p), b = *reinterpret_cast<const uint16_t *>(p + 2),
                                c2 = *reinterpret_cast<const uint16_t *>(p + 4);
                 const uint8_t px[6] = {(uint8_t)(a & 0xff), (uint8_t)(a >> 8), (uint8_t)(b & 0xff), (uint8_t)(b >> 8),
                                        (uint8_t)(c2 & 0xff), (uint8_t)(c2 >> 8)};
 #pragma unroll
-                for (int dx = 0; dx < 2; ++dx)
+                for (int dx = 0; dx < 2; ++dx) {
+                    if (x0 + dx >= vw) continue;                              // odd valid width: the pair's second pixel is padding
 #pragma unroll
                     for (int c = 0; c < 3; ++c) {
                         const int sc = to_rgb ? 2 - c : c;
                         v[(dy * 2 + dx) * 3 + c] = ((float)px[dx * 3 + sc] - mu[c]) * si[c];
                     }
+                }
             }
         }
         uint4 o0 = make_uint4(pack2(v[0], v[1]), pack2(v[2], v[3]), pack2(v[4], v[5]), pack2(v[6], v[7]));
@@ -317,8 +322,8 @@ stem_s2d_u8_kernel(const uint8_t *__restrict__ img, int N, int H, int W, float3 
 }  // namespace
 }  // namespace orp
 
-extern "C" int orp_stem_s2d_u8_bf16(const uint8_t *img_hwc, int N, int H, int W, const float *mean, const float *std,
-                                    int to_rgb, void *out, void *stream)
+static int stem_s2d_u8_bf16_impl(const uint8_t *img_hwc, int N, int H, int W, const float *mean, const float *std, int to_rgb,
+                                 const int32_t *valid, void *out, void *stream)
 {
     using namespace orp;
     if (!img_hwc || !out || !mean || !std || N < 1 || H < 2 || W < 2 || (H & 1) || (W & 1))
@@ -329,10 +334,23 @@ extern "C" int orp_stem_s2d_u8_bf16(const uint8_t *img_hwc, int N, int H, int W,
     // mmcv.imnormalize: stdinv = 1 / np.float64(std), applied to the float32 image
     const float3 si = make_float3((float)(1.0 / (double)std[0]), (float)(1.0 / (double)std[1]), (float)(1.0 / (double)std[2]));
     const size_t total = (size_t)N * (H / 2 + 3) * (W / 2 + 3);
-    stem_s2d_u8_kernel<<<grid_for(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(img_hwc, N, H, W, mu, si, to_rgb,
+    stem_s2d_u8_kernel<<<grid_for(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(img_hwc, N, H, W, mu, si, to_rgb, valid,
                                                                                            static_cast<__nv_bfloat16 *>(out));
     ORP_LAUNCHED();
     return ORP_OK;
+}
+
+extern "C" int orp_stem_s2d_u8_bf16(const uint8_t *img_hwc, int N, int H, int W, const float *mean, const float *std,
+                                    int to_rgb, void *out, void *stream)
+{
+    return stem_s2d_u8_bf16_impl(img_hwc, N, H, W, mean, std, to_rgb, nullptr, out, stream);
+}
+
+extern "C" int orp_stem_s2d_u8_padded_bf16(const uint8_t *img_hwc, int N, int H, int W, const float *mean, const float *std,
+                                           int to_rgb, const int32_t *valid_hw, void *out, void *stream)
+{
+    if (!valid_hw) return orp::fail(ORP_EINVAL, "stem_s2d_u8_padded_bf16: valid_hw is required");
+    return stem_s2d_u8_bf16_impl(img_hwc, N, H, W, mean, std, to_rgb, valid_hw, out, stream);
 }
 
 extern "C" int orp_stem_s2d_bf16(const float *img_nchw, int N, int H, int W, void *out, void *stream)

@@ -226,11 +226,12 @@ gn_apply_split_kernel(const __grid_constant__ GnApplyParams P)
 // Space-to-depth form of the stem input as two fp16 planes [2][N,Hp,Wp,16]:
 // v[n][Y][X][(dy*2+dx)*3 + c] = img[n][c][2(Y-2)+dy][2(X-2)+dx] (zero outside the image, channels 12-15 zero).
 // SRC_U8: decoded uint8 HWC tiles with the test pipeline's Normalize fused (mmcv.imnormalize: optional BGR->RGB,
-// (x - mean) * (1/std) in fp32; mean / stdinv indexed by MODEL channel).
+// (x - mean) * (1/std) in fp32; mean / stdinv indexed by MODEL channel).  valid (SRC_U8 only; int32 [N,2] = (h, w) per
+// image, or null for the full extent): pixels at y >= h or x >= w are the pipeline's Pad after Normalize, exactly 0.0.
 template <bool SRC_U8>
 __global__ void __launch_bounds__(256)
 stem_s2d_split_kernel(const void *__restrict__ img_v, int N, int H, int W, float3 mean, float3 stdinv, int to_rgb,
-                      __half *__restrict__ out)
+                      const int32_t *__restrict__ valid, __half *__restrict__ out)
 {
     const int Hp = H / 2 + 3, Wp = W / 2 + 3;
     const size_t total = (size_t)N * Hp * Wp;
@@ -243,11 +244,12 @@ stem_s2d_split_kernel(const void *__restrict__ img_v, int N, int H, int W, float
         float v[16];
 #pragma unroll
         for (int k = 0; k < 16; ++k) v[k] = 0.f;
-        if (x0 >= 0 && x0 + 1 < W) {
+        const int vh = valid ? min(valid[2 * n], H) : H, vw = valid ? min(valid[2 * n + 1], W) : W;
+        if (x0 >= 0 && x0 < vw) {                                             // W is even: x0 + 1 < W
 #pragma unroll
             for (int dy = 0; dy < 2; ++dy) {
                 const int y = y0 + dy;
-                if (y < 0 || y >= H) continue;
+                if (y < 0 || y >= vh) continue;
                 if (SRC_U8) {
                     const uint8_t *p = static_cast<const uint8_t *>(img_v) + (((size_t)n * H + y) * W + x0) * 3;   // 6 bytes, even address
                     const uint16_t a = *reinterpret_cast<const uint16_t *>(p), b = *reinterpret_cast<const uint16_t *>(p + 2),
@@ -255,12 +257,14 @@ stem_s2d_split_kernel(const void *__restrict__ img_v, int N, int H, int W, float
                     const uint8_t px[6] = {(uint8_t)(a & 0xff), (uint8_t)(a >> 8), (uint8_t)(b & 0xff), (uint8_t)(b >> 8),
                                            (uint8_t)(c2 & 0xff), (uint8_t)(c2 >> 8)};
 #pragma unroll
-                    for (int dx = 0; dx < 2; ++dx)
+                    for (int dx = 0; dx < 2; ++dx) {
+                        if (x0 + dx >= vw) continue;                          // odd valid width: the second pixel is padding
 #pragma unroll
                         for (int c = 0; c < 3; ++c) {
                             const int sc = to_rgb ? 2 - c : c;
                             v[(dy * 2 + dx) * 3 + c] = ((float)px[dx * 3 + sc] - mu[c]) * si[c];
                         }
+                    }
                 } else {
                     const float *img = static_cast<const float *>(img_v);
 #pragma unroll
@@ -349,8 +353,8 @@ extern "C" int orp_split_to_f32(const void *x_split, long long pixels, int C, fl
     return ORP_OK;
 }
 
-extern "C" int orp_stem_s2d_u8_f16x3(const uint8_t *img_hwc, int N, int H, int W, const float *mean, const float *std,
-                                     int to_rgb, void *out, void *stream)
+static int stem_s2d_u8_f16x3_impl(const uint8_t *img_hwc, int N, int H, int W, const float *mean, const float *std, int to_rgb,
+                                  const int32_t *valid, void *out, void *stream)
 {
     if (!img_hwc || !out || !mean || !std || N < 1 || H < 2 || W < 2 || (H & 1) || (W & 1))
         return fail(ORP_EINVAL, "stem_s2d_u8_f16x3: needs even H, W");
@@ -361,9 +365,22 @@ extern "C" int orp_stem_s2d_u8_f16x3(const uint8_t *img_hwc, int N, int H, int W
     const float3 si = make_float3((float)(1.0 / (double)std[0]), (float)(1.0 / (double)std[1]), (float)(1.0 / (double)std[2]));
     const size_t total = (size_t)N * (H / 2 + 3) * (W / 2 + 3);
     stem_s2d_split_kernel<true><<<grid_for(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-        img_hwc, N, H, W, mu, si, to_rgb, static_cast<__half *>(out));
+        img_hwc, N, H, W, mu, si, to_rgb, valid, static_cast<__half *>(out));
     ORP_LAUNCHED();
     return ORP_OK;
+}
+
+extern "C" int orp_stem_s2d_u8_f16x3(const uint8_t *img_hwc, int N, int H, int W, const float *mean, const float *std,
+                                     int to_rgb, void *out, void *stream)
+{
+    return stem_s2d_u8_f16x3_impl(img_hwc, N, H, W, mean, std, to_rgb, nullptr, out, stream);
+}
+
+extern "C" int orp_stem_s2d_u8_padded_f16x3(const uint8_t *img_hwc, int N, int H, int W, const float *mean, const float *std,
+                                            int to_rgb, const int32_t *valid_hw, void *out, void *stream)
+{
+    if (!valid_hw) return fail(ORP_EINVAL, "stem_s2d_u8_padded_f16x3: valid_hw is required");
+    return stem_s2d_u8_f16x3_impl(img_hwc, N, H, W, mean, std, to_rgb, valid_hw, out, stream);
 }
 
 extern "C" int orp_stem_s2d_f16x3(const float *img_nchw, int N, int H, int W, void *out, void *stream)
@@ -374,7 +391,7 @@ extern "C" int orp_stem_s2d_f16x3(const float *img_nchw, int N, int H, int W, vo
     const size_t total = (size_t)N * (H / 2 + 3) * (W / 2 + 3);
     const float3 z = make_float3(0.f, 0.f, 0.f);
     stem_s2d_split_kernel<false><<<grid_for(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-        img_nchw, N, H, W, z, z, 0, static_cast<__half *>(out));
+        img_nchw, N, H, W, z, z, 0, nullptr, static_cast<__half *>(out));
     ORP_LAUNCHED();
     return ORP_OK;
 }

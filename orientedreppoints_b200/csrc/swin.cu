@@ -488,11 +488,13 @@ patch_embed_rows_kernel(const float *__restrict__ img, int B, int H, int W, int 
 
 // the same rows straight from decoded uint8 HWC tiles: Normalize (mmdet/datasets/pipelines/transforms.py: to_rgb, (x - mean) / std as
 // (x - mean) * (1 / std), two roundings like the eager expression) + ImageToTensor fused into the gather
+// valid (int32 [B,2] = (h, w) per image, or null for the full extent): pixels at y >= h or x >= w are the Pad step after
+// Normalize and contribute exactly 0.0
 struct NormCfg { float mean[3], stdinv[3]; int to_rgb; };
 template <bool SPLIT>
 __global__ void __launch_bounds__(256)
 patch_embed_rows_u8_kernel(const uint8_t *__restrict__ img, int B, int H, int W, int Ho, int Wo, NormCfg nc,
-                           typename Act<SPLIT>::T *__restrict__ out)
+                           const int32_t *__restrict__ valid, typename Act<SPLIT>::T *__restrict__ out)
 {
     const long long total = (long long)B * Ho * Wo * 64;
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
@@ -503,7 +505,8 @@ patch_embed_rows_u8_kernel(const uint8_t *__restrict__ img, int B, int H, int W,
         if (k < 48) {
             const int c = k >> 4, kh = (k >> 2) & 3, kw = k & 3;
             const int y = oh * 4 + kh, x = ow * 4 + kw;
-            if (y < H && x < W) {
+            const int vh = valid ? min(valid[2 * b], H) : H, vw = valid ? min(valid[2 * b + 1], W) : W;
+            if (y < vh && x < vw) {
                 const float raw = (float)img[(((long long)b * H + y) * W + x) * 3 + (nc.to_rgb ? 2 - c : c)];
                 v = __fmul_rn(__fsub_rn(raw, nc.mean[c]), nc.stdinv[c]);
             }
@@ -650,7 +653,7 @@ extern "C" int orp_patch_embed_rows_f16x3(const float *img_nchw, int B, int H, i
 
 template <bool SPLIT>
 static int patch_embed_rows_u8_impl(const uint8_t *img_hwc, int B, int H, int W, const float *mean, const float *stdinv, int to_rgb,
-                                    void *out, void *stream)
+                                    const int32_t *valid, void *out, void *stream)
 {
     if (!img_hwc || !out || !mean || !stdinv) return fail(ORP_EINVAL, "patch_embed_rows_u8: bad arguments");
     int rc = ensure_device();
@@ -660,19 +663,31 @@ static int patch_embed_rows_u8_impl(const uint8_t *img_hwc, int B, int H, int W,
     nc.to_rgb = to_rgb ? 1 : 0;
     const int Ho = (H + 3) / 4, Wo = (W + 3) / 4;
     patch_embed_rows_u8_kernel<SPLIT><<<grid_for((long long)B * Ho * Wo * 64, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-        img_hwc, B, H, W, Ho, Wo, nc, static_cast<typename Act<SPLIT>::T *>(out));
+        img_hwc, B, H, W, Ho, Wo, nc, valid, static_cast<typename Act<SPLIT>::T *>(out));
     ORP_LAUNCHED();
     return ORP_OK;
 }
 extern "C" int orp_patch_embed_rows_u8_bf16(const uint8_t *img_hwc, int B, int H, int W, const float *mean, const float *stdinv,
                                             int to_rgb, void *out, void *stream)
 {
-    return patch_embed_rows_u8_impl<false>(img_hwc, B, H, W, mean, stdinv, to_rgb, out, stream);
+    return patch_embed_rows_u8_impl<false>(img_hwc, B, H, W, mean, stdinv, to_rgb, nullptr, out, stream);
 }
 extern "C" int orp_patch_embed_rows_u8_f16x3(const uint8_t *img_hwc, int B, int H, int W, const float *mean, const float *stdinv,
                                              int to_rgb, void *out, void *stream)
 {
-    return patch_embed_rows_u8_impl<true>(img_hwc, B, H, W, mean, stdinv, to_rgb, out, stream);
+    return patch_embed_rows_u8_impl<true>(img_hwc, B, H, W, mean, stdinv, to_rgb, nullptr, out, stream);
+}
+extern "C" int orp_patch_embed_rows_u8_padded_bf16(const uint8_t *img_hwc, int B, int H, int W, const float *mean,
+                                                   const float *stdinv, int to_rgb, const int32_t *valid_hw, void *out, void *stream)
+{
+    if (!valid_hw) return fail(ORP_EINVAL, "patch_embed_rows_u8_padded_bf16: valid_hw is required");
+    return patch_embed_rows_u8_impl<false>(img_hwc, B, H, W, mean, stdinv, to_rgb, valid_hw, out, stream);
+}
+extern "C" int orp_patch_embed_rows_u8_padded_f16x3(const uint8_t *img_hwc, int B, int H, int W, const float *mean,
+                                                    const float *stdinv, int to_rgb, const int32_t *valid_hw, void *out, void *stream)
+{
+    if (!valid_hw) return fail(ORP_EINVAL, "patch_embed_rows_u8_padded_f16x3: valid_hw is required");
+    return patch_embed_rows_u8_impl<true>(img_hwc, B, H, W, mean, stdinv, to_rgb, valid_hw, out, stream);
 }
 
 static int patch_merge_gather_impl(const void *x, int B, int H, int W, int C, int P, void *y, void *stream)

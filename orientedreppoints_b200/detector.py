@@ -204,9 +204,11 @@ class OrientedRepPointsDetector:
         self._load_head(sd)
 
     # ------------------------------------------------------------------ dense graph
-    def normalize(self, img):
+    def normalize(self, img, valid_hw=None):
         """decoded uint8 HWC tiles [N,H,W,3] -> the pipeline's Normalize + ImageToTensor on the device
-        (mmdet/datasets/pipelines/transforms.py:Normalize, formating.py:ImageToTensor); float NCHW input passes through"""
+        (mmdet/datasets/pipelines/transforms.py:Normalize, formating.py:ImageToTensor); float NCHW input passes through.
+        valid_hw (device int32 [N,2]): per-image extent of the image inside the padded batch; outside it the result is
+        exactly 0.0 (Pad after Normalize)"""
         if img.dtype != torch.uint8:
             return img
         c = self.img_norm_cfg
@@ -218,13 +220,21 @@ class OrientedRepPointsDetector:
             self._norm_mean = torch.tensor(c["mean"], dtype=torch.float32).to(self.device)
             self._norm_stdinv = torch.tensor([1.0 / v for v in c["std"]], dtype=torch.float64).float().to(self.device)
             self._norm_key = key
-        return ((x - self._norm_mean) * self._norm_stdinv).permute(0, 3, 1, 2).contiguous()
+        x = (x - self._norm_mean) * self._norm_stdinv
+        if valid_hw is not None:
+            n, h, w = x.shape[:3]
+            vh = valid_hw.to(self.device)
+            inside = (torch.arange(h, device=self.device).view(1, h, 1) < vh[:, 0].view(n, 1, 1)) & \
+                     (torch.arange(w, device=self.device).view(1, 1, w) < vh[:, 1].view(n, 1, 1))
+            x = torch.where(inside.unsqueeze(-1), x, torch.zeros((), dtype=x.dtype, device=self.device))
+        return x.permute(0, 3, 1, 2).contiguous()
 
-    def extract_feat(self, img):
+    def extract_feat(self, img, valid_hw=None):
+        """valid_hw: optional device int32 [N,2] extents of uint8 images padded by the test pipeline"""
         e = self.eng
         if self.depth == "swin_tiny":
-            # decoded uint8 tiles: Normalize + ImageToTensor are fused into the patch gather
-            c3, c4, c5 = self.swin.forward(img, self.img_norm_cfg)
+            # decoded uint8 tiles: Normalize + ImageToTensor (+ the zero padding outside valid_hw) are fused into the patch gather
+            c3, c4, c5 = self.swin.forward(img, self.img_norm_cfg, valid_hw)
             l2 = e.conv_gn(c5, *self.lat[2])
             l1 = e.conv_gn(c4, *self.lat[1], up=l2)
             l0 = e.conv_gn(c3, *self.lat[0], up=l1)
@@ -233,9 +243,9 @@ class OrientedRepPointsDetector:
             outs.append(self.swin.subsample2(outs[-1]))
             return outs
         if img.dtype == torch.uint8 and hasattr(e, "stem_u8") and img.shape[1] % 2 == 0 and img.shape[2] % 2 == 0:
-            x = e.maxpool(e.stem_u8(img, self.stem, self.img_norm_cfg))     # Normalize fused into the stem input transform
+            x = e.maxpool(e.stem_u8(img, self.stem, self.img_norm_cfg, valid_hw))   # Normalize (+ Pad) fused into the stem input
         else:
-            x = e.prepare_input(self.normalize(img))
+            x = e.prepare_input(self.normalize(img, valid_hw))
             x = e.maxpool(e.stem(x, self.stem))
         feats = []
         for stage in self.blocks:
@@ -277,52 +287,68 @@ class OrientedRepPointsDetector:
                            residual_f32=init)
         return [(c.float(), i, r.float()) for c, i, r in zip(cls, init, ref)]
 
-    def forward_dense(self, img):
+    def forward_dense(self, img, valid_hw=None):
         # every launch goes to the current stream of the current device: make that this detector's device
         with torch.cuda.device(self.device):
             if img.device != self.device:
                 img = img.to(self.device)
-            feats = self.extract_feat(img)
+            feats = self.extract_feat(img, valid_hw)
             return self.head(feats), feats
 
     # ------------------------------------------------------------------ CUDA graph of the dense graph
-    def capture(self, img_shape, dtype=torch.float32):
+    def capture(self, img_shape, dtype=torch.float32, padded=False):
         """Capture backbone + FPN + head for a fixed input shape into ONE CUDA graph (static buffers): the
         ~180 kernel launches of a step become a single graph launch, which removes the host-side launch
-        cost that otherwise dominates a one-tile step.  simple_test() replays it when the shape matches."""
+        cost that otherwise dominates a one-tile step.  simple_test() replays it when the shape matches.
+        padded=True captures the test-pipeline form (uint8 input with per-image valid extents): the extents are a static
+        device buffer of the graph like the image, so one capture serves every extent of that input shape."""
         shape = tuple(img_shape)
         torch.cuda.set_device(self.device)
         self._g_img = torch.zeros(shape, dtype=dtype, device=self.device)
+        self._g_valid = None
+        if padded:
+            self._g_valid = torch.tensor([list(shape[1:3])] * shape[0], dtype=torch.int32).to(self.device)
         side = torch.cuda.Stream(device=self.device)
         side.wait_stream(torch.cuda.current_stream(self.device))
         with torch.cuda.stream(side):
             for _ in range(2):                                      # warm-up: lazy weight prep, func attributes
-                self.forward_dense(self._g_img)
+                self._forward_dense_opt(self._g_img, self._g_valid)
         torch.cuda.current_stream(self.device).wait_stream(side)
         torch.cuda.synchronize(self.device)
         self._graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(self._graph):
-            self._g_out = self.forward_dense(self._g_img)
-        self._g_shape = (shape, dtype)
+            self._g_out = self._forward_dense_opt(self._g_img, self._g_valid)
+        self._g_shape = (shape, dtype) if not padded else (shape, dtype, "valid_hw")
         return self
 
-    def forward_dense_graph(self, img):
+    def _forward_dense_opt(self, img, valid_hw):
+        return self.forward_dense(img) if valid_hw is None else self.forward_dense(img, valid_hw)
+
+    def _graph_key(self, img, valid_hw):
+        key = (tuple(img.shape), img.dtype)
+        return key if valid_hw is None else key + ("valid_hw",)
+
+    def forward_dense_graph(self, img, valid_hw=None):
         with torch.cuda.device(self.device):
             self._g_img.copy_(img, non_blocking=True)
+            if valid_hw is not None:
+                self._g_valid.copy_(valid_hw, non_blocking=True)
             self._graph.replay()
         return self._g_out
 
     # ------------------------------------------------------------------ simple_test
-    def simple_test(self, img, img_metas=None, rescale=False, return_tensors=False):
+    def simple_test(self, img, img_metas=None, rescale=False, return_tensors=False, valid_hw=None):
+        """valid_hw: device int32 [N,2] extents of a uint8 batch padded by the test pipeline (datasets/pipelines.py);
+        pixels outside them enter the network as 0.0"""
         with torch.cuda.device(self.device):
-            return self._simple_test(img, img_metas, rescale, return_tensors)
+            return self._simple_test(img, img_metas, rescale, return_tensors, valid_hw)
 
-    def _simple_test(self, img, img_metas, rescale, return_tensors):
+    def _simple_test(self, img, img_metas, rescale, return_tensors, valid_hw=None):
         from .core.get_bboxes import get_bboxes
-        if getattr(self, "_g_shape", None) == (tuple(img.shape), img.dtype):
-            outs, _ = self.forward_dense_graph(img)
+        if getattr(self, "_g_shape", None) == self._graph_key(img, valid_hw):
+            outs, _ = self.forward_dense_graph(img, valid_hw)
         else:
-            outs, _ = self.forward_dense(img)
+            outs, _ = self._forward_dense_opt(img, valid_hw)
         n = img.shape[0]
         if img_metas is None:
             img_metas = [dict(scale_factor=1.0) for _ in range(n)]
@@ -370,17 +396,18 @@ class OrientedRepPointsDetector:
             return bboxes
         return bboxes, torch.cat(aug_scores, dim=0)
 
-    def aug_test(self, imgs, img_metas, rescale=False):
+    def aug_test(self, imgs, img_metas, rescale=False, valid_hws=None):
         """orientedreppoints_detector.py:112-144.  imgs: list of views, each ONE image (float NCHW [1,3,H,W] or uint8
-        HWC [1,H,W,3]); img_metas: list of [dict(img_shape, scale_factor, flip)].  Raw candidates of all views
+        HWC [1,H,W,3]); img_metas: list of [dict(img_shape, scale_factor, flip)]; valid_hws: optional list of per-view
+        device int32 [1,2] extents (views padded by the test pipeline).  Raw candidates of all views
         (get_bboxes(nms=False), head :778-779) are concatenated and go through ONE multiclass_rnms."""
         from .core.bbox_nms import multiclass_rnms
         from .core.get_bboxes import get_bboxes
         from .core.transforms import rbbox2result
         aug_bboxes, aug_scores = [], []
-        for img, meta in zip(imgs, img_metas):
+        for k, (img, meta) in enumerate(zip(imgs, img_metas)):
             assert img.shape[0] == 1, "aug_test: one image per view"
-            outs, _ = self.forward_dense(img)
+            outs, _ = self._forward_dense_opt(img, None if valid_hws is None else valid_hws[k])
             b, sc = get_bboxes([o[0] for o in outs], [o[2] for o in outs], STRIDES, meta, self.test_cfg, False, nms=False)[0]
             aug_bboxes.append(b)
             aug_scores.append(sc)

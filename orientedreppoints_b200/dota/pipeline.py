@@ -29,12 +29,25 @@ def task1_lines(results, tile_names):
     return per_class
 
 
-def detect_image(det, img_u8, name="P0000", rate=1, subsize=1024, gap=200, batch=16, merge_thresh=None):
+def detect_image(det, img_u8, name="P0000", rate=1, subsize=1024, gap=200, batch=16, merge_thresh=None, test_pipeline=None):
     """det: OrientedRepPointsDetector; img_u8: decoded uint8 HWC image (numpy or tensor).  Returns
-    {class name: [`imgname score x1 y1 x2 y2 x3 y3 x4 y4`, ...]} in the Task1 format after ResultMerge."""
+    {class name: [`imgname score x1 y1 x2 y2 x3 y3 x4 y4`, ...]} in the Task1 format after ResultMerge.
+    test_pipeline: a config's test_pipeline (list of dicts).  When given, every batch of tiles goes through it on the
+    device (resize / flip / pad, datasets/pipelines.py) and the detections are mapped back to tile coordinates
+    (rescale=True) before ResultMerge, as tools/test.py does.  None (the default) feeds the tiles unchanged."""
     tiles, names, _ = split_image(img_u8, name, rate, subsize, gap, device=det.device)
     results = []
     for i in range(0, tiles.shape[0], batch):
-        results.extend(det.simple_test(tiles[i:i + batch]))
+        if test_pipeline is None:
+            results.extend(det.simple_test(tiles[i:i + batch]))
+            continue
+        from ..datasets.pipelines import run_test_pipeline
+        data = run_test_pipeline(test_pipeline, tiles[i:i + batch], device=det.device)
+        views, metas, valids = data['img'], data['img_meta'], data['valid_hw']
+        if len(views) == 1:
+            results.extend(det.simple_test(views[0], metas[0], rescale=True, valid_hw=valids[0]))
+        else:
+            results.extend(det.aug_test([v[k:k + 1] for v in views], [[m[k]] for m in metas], rescale=True,
+                                        valid_hws=[v[k:k + 1] for v in valids]) for k in range(views[0].shape[0]))
     per_class = task1_lines(results, names)
     return {cname: merge_lines(lines, merge_thresh) for cname, lines in zip(DOTA_CLASSES, per_class)}

@@ -8,6 +8,13 @@ import torch
 from . import _lib
 
 
+def _valid(valid_hw, n, device):
+    """per-image valid extents as the kernels read them: device int32 [n, 2] = (h, w), contiguous"""
+    assert tuple(valid_hw.shape) == (n, 2) and valid_hw.dtype == torch.int32 and valid_hw.device == device, \
+        "valid_hw must be an int32 [N,2] tensor on the detector's device"
+    return valid_hw.contiguous()
+
+
 class EngineTC:
     name = "bf16"
     act_dtype = torch.bfloat16
@@ -93,9 +100,10 @@ class EngineTC:
                                                st), "orp_stem_conv_bf16")
         return y
 
-    def stem_u8(self, img_u8, L, norm_cfg):
+    def stem_u8(self, img_u8, L, norm_cfg, valid_hw=None):
         """conv1 + folded BN + ReLU from decoded uint8 HWC tiles [N,H,W,3]; Normalize (mean/std/to_rgb of the test
-        pipeline) is applied inside the space-to-depth transform kernel"""
+        pipeline) is applied inside the space-to-depth transform kernel, and so is the Pad that follows it when valid_hw
+        (device int32 [N,2] per-image extents) is given: pixels outside enter as 0.0"""
         import ctypes
         n, h, w, c = img_u8.shape
         assert c == 3 and img_u8.dtype == torch.uint8 and img_u8.is_contiguous() and h % 2 == 0 and w % 2 == 0
@@ -104,8 +112,13 @@ class EngineTC:
         xs = torch.empty((n, h // 2 + 3, w // 2 + 3, 16), dtype=torch.bfloat16, device=self.device)
         mean = (ctypes.c_float * 3)(*norm_cfg["mean"])
         std = (ctypes.c_float * 3)(*norm_cfg["std"])
-        _lib.check(self.lib.orp_stem_s2d_u8_bf16(_lib.ptr(img_u8), n, h, w, mean, std, int(bool(norm_cfg["to_rgb"])),
-                                                 _lib.ptr(xs), st), "orp_stem_s2d_u8_bf16")
+        if valid_hw is None:
+            _lib.check(self.lib.orp_stem_s2d_u8_bf16(_lib.ptr(img_u8), n, h, w, mean, std, int(bool(norm_cfg["to_rgb"])),
+                                                     _lib.ptr(xs), st), "orp_stem_s2d_u8_bf16")
+        else:
+            _lib.check(self.lib.orp_stem_s2d_u8_padded_bf16(_lib.ptr(img_u8), n, h, w, mean, std, int(bool(norm_cfg["to_rgb"])),
+                                                            _lib.ptr(_valid(valid_hw, n, self.device)), _lib.ptr(xs), st),
+                       "orp_stem_s2d_u8_padded_bf16")
         y = torch.empty((n, h // 2, w // 2, 64), dtype=torch.bfloat16, device=self.device)
         _lib.check(self.lib.orp_stem_conv_s2d_bf16(_lib.ptr(xs), n, h, w, _lib.ptr(ws), _lib.ptr(L.bias), 1, _lib.ptr(y), st),
                    "orp_stem_conv_s2d_bf16")
@@ -362,7 +375,7 @@ class EngineTCSplit(EngineTC):
                                                     _lib.ptr(y), st), "orp_stem_conv_s2d_f16x3")
         return y
 
-    def stem_u8(self, img_u8, L, norm_cfg):
+    def stem_u8(self, img_u8, L, norm_cfg, valid_hw=None):
         n, h, w, c = img_u8.shape
         assert c == 3 and img_u8.dtype == torch.uint8 and img_u8.is_contiguous() and h % 2 == 0 and w % 2 == 0
         st = _lib.current_stream_ptr()
@@ -370,8 +383,13 @@ class EngineTCSplit(EngineTC):
         xs = torch.empty((2, n, h // 2 + 3, w // 2 + 3, 16), dtype=torch.float16, device=self.device)
         mean = (ctypes.c_float * 3)(*norm_cfg["mean"])
         std = (ctypes.c_float * 3)(*norm_cfg["std"])
-        _lib.check(self.lib.orp_stem_s2d_u8_f16x3(_lib.ptr(img_u8), n, h, w, mean, std, int(bool(norm_cfg["to_rgb"])),
-                                                  _lib.ptr(xs), st), "orp_stem_s2d_u8_f16x3")
+        if valid_hw is None:
+            _lib.check(self.lib.orp_stem_s2d_u8_f16x3(_lib.ptr(img_u8), n, h, w, mean, std, int(bool(norm_cfg["to_rgb"])),
+                                                      _lib.ptr(xs), st), "orp_stem_s2d_u8_f16x3")
+        else:
+            _lib.check(self.lib.orp_stem_s2d_u8_padded_f16x3(_lib.ptr(img_u8), n, h, w, mean, std, int(bool(norm_cfg["to_rgb"])),
+                                                             _lib.ptr(_valid(valid_hw, n, self.device)), _lib.ptr(xs), st),
+                       "orp_stem_s2d_u8_padded_f16x3")
         y = torch.empty((n, h // 2, w // 2, 2, 64), dtype=torch.float16, device=self.device)
         _lib.check(self.lib.orp_stem_conv_s2d_f16x3(_lib.ptr(xs), n, h, w, _lib.ptr(ws["w"]), _lib.ptr(L.bias), ws["s"], 1,
                                                     _lib.ptr(y), st), "orp_stem_conv_s2d_f16x3")

@@ -152,9 +152,10 @@ class SwinTiny:
                    "orp_patch_merge_gather")
         return self.e.conv(self._ln(g, m["norm"]), m["red"])
 
-    def forward(self, img, img_norm_cfg=None):
+    def forward(self, img, img_norm_cfg=None, valid_hw=None):
         """img: normalised float NCHW, or decoded uint8 HWC tiles [B,H,W,3] together with the pipeline's img_norm_cfg (Normalize +
-        ImageToTensor are then fused into the patch gather)"""
+        ImageToTensor are then fused into the patch gather; with valid_hw, device int32 [B,2] per-image extents, so is the Pad
+        after Normalize: pixels outside enter as 0.0)"""
         if img.dtype == torch.uint8:
             import ctypes
             img = img.to(self.dev).contiguous()
@@ -163,9 +164,17 @@ class SwinTiny:
             stdinv = (ctypes.c_float * 3)(*[1.0 / float(v) for v in img_norm_cfg["std"]])      # rounded to fp32 as detector.normalize does
             ho, wo = (h + 3) // 4, (w + 3) // 4
             rows = self.e.alloc(b, ho, wo, 64)
-            _lib.check(self._fn("patch_embed_rows_u8")(_lib.ptr(img), b, h, w, mean, stdinv, 1 if img_norm_cfg.get("to_rgb", True) else 0,
-                                                      _lib.ptr(rows), _lib.current_stream_ptr()), "orp_patch_embed_rows_u8")
+            to_rgb = 1 if img_norm_cfg.get("to_rgb", True) else 0
+            if valid_hw is None:
+                _lib.check(self._fn("patch_embed_rows_u8")(_lib.ptr(img), b, h, w, mean, stdinv, to_rgb, _lib.ptr(rows),
+                                                          _lib.current_stream_ptr()), "orp_patch_embed_rows_u8")
+            else:
+                from .engine_tc import _valid
+                _lib.check(self._fn("patch_embed_rows_u8_padded")(_lib.ptr(img), b, h, w, mean, stdinv, to_rgb,
+                                                                 _lib.ptr(_valid(valid_hw, b, img.device)), _lib.ptr(rows),
+                                                                 _lib.current_stream_ptr()), "orp_patch_embed_rows_u8_padded")
         else:
+            assert valid_hw is None, "valid_hw applies to uint8 images (float input is already normalised and padded)"
             img = img.to(self.dev, torch.float32).contiguous()
             b, _, h, w = img.shape
             ho, wo = (h + 3) // 4, (w + 3) // 4
