@@ -274,7 +274,8 @@ int orp_conv2d_f32(const float *x, int N, int H, int W, int Cin, const float *w,
  * (mmdet/ops/dcn/src/deform_conv_cuda.cpp:152-260, 490-569) without the im2col `columns` scratch:
  * sampling per deformable_im2col_bilinear (deform_conv_cuda_kernel.cu:84-115), validity test of :229.
  *   offset  device float32 [N, Ho, Wo, 2*KH*KW], channel 2t = dy, 2t+1 = dx of tap t (:222-225)
- *   mask    device float32 [N, Ho, Wo, KH*KW] or NULL */
+ *   mask    device float32 [N, Ho, Wo, KH*KW] or NULL
+ * Cin must be a multiple of 4 (float4 channel loads); callers zero-pad x and w to it. */
 int orp_deform_conv2d_f32(const float *x, int N, int H, int W, int Cin, const float *offset, const float *mask,
                           const float *w, int Cout, int KH, int KW, int stride, int pad, int dilation,
                           const float *bias, int relu, float *y, void *stream);
@@ -313,7 +314,10 @@ typedef struct {
 
 /* y = relu?(conv(x, w) + bias + residual) for up to 5 problems sharing the weights.  deform != 0:
  * the A operand is the bilinear sample of deform_conv_cuda_kernel.cu:84-115 (DCNv1, groups =
- * deformable_groups = 1) produced on the fly in shared memory - no `columns` buffer. */
+ * deformable_groups = 1) produced on the fly in shared memory - no `columns` buffer.  Its producers address the input
+ * with 32-bit element offsets: a deformable problem with N*H*W*Cin*planes >= 2^31 16-bit elements (planes = 2 in
+ * orp_conv2d_f16x3) is ORP_EINVAL; orp_deform_conv2d_f32 has no such bound.  stride must be in 1..256 (a tile spans
+ * BW * stride <= 256 input columns); ORP_EINVAL otherwise. */
 int orp_conv2d_bf16(int nprob, const orp_tc_problem *probs, const void *w, int Cout, int Cout_padded,
                     int KH, int KW, int Cin, int stride, int pad, const float *bias, int relu, int out_f32,
                     int deform, void *stream);

@@ -1389,6 +1389,13 @@ static int conv2d_bf16_impl(int nprob, const orp_tc_problem *probs, const void *
     if (deform && !stem && (Cin % kBK)) return fail(ORP_EINVAL, "conv2d_tc: deformable conv needs Cin % 64 == 0");
     if (Cout_padded % 32 || Cout_padded < Cout) return fail(ORP_EINVAL, "conv2d_tc: padded Cout must be a multiple of 32");
     if (split && stem == 1) return fail(ORP_EINVAL, "conv2d_tc: the direct stem has no f16x3 form (use the space-to-depth stem)");
+    // a tile spans BW * stride <= 256 input columns (the TMA box limit) with BW >= 1
+    if (stride < 1 || stride > 256) return fail(ORP_EINVAL, "conv2d_tc: stride must be in 1..256");
+    // the deformable producers address the input with 32-bit element offsets (img0, s_o): N*H*W*Cin*planes must stay below 2^31
+    if (deform && !stem)
+        for (int i = 0; i < nprob; ++i)
+            if ((long long)probs[i].N * probs[i].H * probs[i].W * Cin * (split ? 2 : 1) >= (1LL << 31))
+                return fail(ORP_EINVAL, "conv2d_tc: deformable input has 2^31 or more 16-bit elements (32-bit sample offsets)");
     if (ksplit < 1) ksplit = 1;
     if (ksplit > 1 && (nprob != 1 || deform || stem || !out_f32 || (KH * KW) % ksplit || probs[0].residual_bf16 || probs[0].residual_f32 || bias || relu))
         return fail(ORP_EINVAL, "conv2d_tc: split-K serves one plain problem with an fp32 partial-sum output and taps % ksplit == 0");
@@ -1439,7 +1446,8 @@ static int conv2d_bf16_impl(int nprob, const orp_tc_problem *probs, const void *
         if (stem == 1) { pr.Ho = (q.H + 6 - 7) / 2 + 1; pr.Wo = (q.W + 6 - 7) / 2 + 1; }
         if (pr.Ho <= 0 || pr.Wo <= 0 || !q.x || !q.out) return fail(ORP_EINVAL, "conv2d_tc: bad problem");
         pr.BW = pow2_floor(pr.Wo < 128 ? pr.Wo : 128);
-        if (stride * pr.BW > 256) pr.BW = 256 / stride;
+        // the TMA box spans BW * stride columns (<= 256); BW stays a power of two, as the row decode (& (BW - 1), lbw) needs
+        if (stride * pr.BW > 256) pr.BW = pow2_floor(256 / stride);
         // (measured: 16 x 8 pixel tiles for the deformable variant change nothing - 1361 vs 1334 us per f16x3 launch, and neither
         // does the spread of the offsets: the gather runs at the ~47 GB/s per SM L2 -> SM ceiling whatever its locality)
         if (deform && !stem && pr.BW > 16 && getenv("ORP_TC_DCN_2DTILES")) pr.BW = 16;

@@ -7,16 +7,24 @@ fp32 tensors in and out, and the same error behaviour (`assert not bias`, ValueE
 NotImplementedError, `RuntimeError` for an offset of the wrong shape as deform_conv_cuda.cpp:130-136 raises).
 
 What runs underneath is NOT the reference's im2col + SGEMM (deform_conv_cuda.cpp:152-260: a 151 MB `columns` buffer per
-level): the sampling happens inside the wgmma implicit-GEMM kernel's A-operand producers (csrc/dense_tc.cu), in f16x3
-arithmetic by default (fp32-faithful: |err| ~1e-5 of max, see include/orp_b200.h) or single-pass bf16
-(`set_precision('bf16')`).  Shapes the tensor-core kernel does not cover (Cin % 64, dilation > 1, bias-free fp32 path)
-run on the fp32 CUDA-core kernel `orp_deform_conv2d_f32`.  groups / deformable_groups > 1 are not built (the reference's
-configs use 1, orientedreppoints_head.py:117-131).  Forward only: this repository is the inference path.
+level): the sampling happens inside a convolution kernel's A-operand loads.  `_route` picks the kernel from the shapes:
+
+- the wgmma implicit-GEMM kernel (csrc/dense_tc.cu), in f16x3 arithmetic by default (fp32-faithful: |err| ~1e-5 of max,
+  see include/orp_b200.h) or single-pass bf16 (`set_precision('bf16')`), when Cin % 64 == 0, dilation == 1, stride <= 256
+  and the input holds fewer than 2^31 16-bit elements (N*H*W*Cin, twice that in f16x3: its producers use 32-bit offsets);
+- the fp32 CUDA-core kernel `orp_deform_conv2d_f32` (csrc/dense_f32.cu) for every other shape and for
+  `set_precision('fp32')`.  It reads float4 channel groups, so Cin is zero-padded to a multiple of 4 (input and weights;
+  the padded channels add exactly 0).
+
+Any kernel size (KH x KW), square stride / padding / dilation, bias and DCNv2 mask are accepted on both.  groups /
+deformable_groups > 1 and non-square stride / padding / dilation are not built (the reference's configs use neither,
+orientedreppoints_head.py:117-131).  Forward only: this repository is the inference path.
 """
 import math
 
 import torch
 import torch.nn as nn
+import torch.nn.functional as F
 from torch.autograd import Function
 from torch.nn.modules.utils import _pair, _single
 
@@ -33,6 +41,24 @@ def set_precision(p):
     _PRECISION = p
 
 
+_TC_MAX_ELEMENTS = 1 << 31           # 16-bit input elements the tensor-core producers can address (32-bit offsets)
+_TC_MAX_STRIDE = 256                 # a tensor-core tile spans at least one output column: BW * stride <= 256
+
+
+def _route(precision, n, h, w, cin, stride, dilation):
+    """the kernel a deformable convolution of this shape runs on: 'tc' (wgmma, csrc/dense_tc.cu) or 'f32'
+    (orp_deform_conv2d_f32, csrc/dense_f32.cu)"""
+    if precision == "fp32" or cin % 64 or dilation != 1 or stride > _TC_MAX_STRIDE:
+        return "f32"
+    planes = 2 if precision == "f16x3" else 1                # f16x3 holds every value as an fp16 (hi, lo) pair
+    return "tc" if n * h * w * cin * planes < _TC_MAX_ELEMENTS else "f32"
+
+
+def _cin4(cin):
+    """the fp32 kernel reads float4 channel groups: Cin is zero-padded to a multiple of 4"""
+    return (cin + 3) // 4 * 4
+
+
 class _W:
     """weight holder in the layout the engines expect (same fields as detector.ConvLayer)"""
 
@@ -40,7 +66,7 @@ class _W:
         w = weight.detach().permute(0, 2, 3, 1).contiguous()
         self.w_raw = w.float().cpu()
         self.cout, self.kh, self.kw, self.cin = w.shape
-        self.w = w.float().contiguous()
+        self.w = F.pad(w.float(), (0, _cin4(self.cin) - self.cin)).contiguous()     # fp32 kernel: [Cout, KH, KW, Cin4]
         self.bias = None if bias is None else bias.detach().float().contiguous()
         self.stride, self.pad = stride, pad
         self.tc = None
@@ -50,13 +76,19 @@ _cache = {}
 
 
 def _layer(weight, bias, stride, pad):
-    key = (weight.data_ptr(), weight._version, None if bias is None else (bias.data_ptr(), bias._version), stride, pad,
-           tuple(weight.shape))
-    L = _cache.get(key)
-    if L is None:
-        if len(_cache) > 64:
-            _cache.clear()
-        L = _cache[key] = _W(weight, bias, stride, pad)
+    # keyed by address, layout and version counter; every view of a tensor shares its counter, so a caller passing
+    # `m.weight.detach()` on each call hits too.  An entry holds the weight's and the bias's storage: while it is cached no
+    # other tensor can be allocated at that address, so a key match is the same memory, not written since (writes through
+    # a `.data` alias bump a counter of its own and are not seen).  At most 65 entries, i.e. their weights, are kept.
+    key = (weight.data_ptr(), weight._version, tuple(weight.shape), weight.stride(), stride, pad,
+           None if bias is None else (bias.data_ptr(), bias._version, tuple(bias.shape), bias.stride()))
+    hit = _cache.get(key)
+    if hit is not None:
+        return hit[1]
+    if len(_cache) > 64:
+        _cache.clear()
+    L = _W(weight, bias, stride, pad)
+    _cache[key] = ((weight.untyped_storage(), None if bias is None else bias.untyped_storage()), L)
     return L
 
 
@@ -108,8 +140,7 @@ def _forward(input, offset, mask, weight, bias, stride, padding, dilation, group
         msk = None if mask is None else _to_nhwc(mask.detach().float().contiguous())
         L = _layer(weight, bias, stride[0], padding[0])
         L.w, L.bias = L.w.to(dev), None if L.bias is None else L.bias.to(dev)
-        tc_ok = (_PRECISION != "fp32" and cin % 64 == 0 and dilation[0] == 1)
-        if tc_ok:
+        if _route(_PRECISION, n, h, w, cin, stride[0], dilation[0]) == "tc":
             from ..engine_tc import EngineTC, EngineTCSplit
             if _PRECISION == "f16x3":
                 eng = EngineTCSplit(dev)
@@ -125,7 +156,9 @@ def _forward(input, offset, mask, weight, bias, stride, padding, dilation, group
                         offsets=[off], masks=None if msk is None else [msk])
         else:
             y = torch.empty((n, ho, wo, cout), dtype=torch.float32, device=dev)
-            rc = _lib.lib().orp_deform_conv2d_f32(_lib.ptr(_to_nhwc(x)), n, h, w, cin, _lib.ptr(off), _lib.ptr(msk), _lib.ptr(L.w),
+            c4 = _cin4(cin)
+            xp = x if c4 == cin else F.pad(x, (0, 0, 0, 0, 0, c4 - cin))
+            rc = _lib.lib().orp_deform_conv2d_f32(_lib.ptr(_to_nhwc(xp)), n, h, w, c4, _lib.ptr(off), _lib.ptr(msk), _lib.ptr(L.w),
                                                   cout, kh, kw, stride[0], padding[0], dilation[0], _lib.ptr(L.bias), 0,
                                                   _lib.ptr(y), _lib.current_stream_ptr())
             _lib.check(rc, "orp_deform_conv2d_f32")
