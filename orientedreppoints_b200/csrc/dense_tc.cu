@@ -30,16 +30,18 @@
 // relative) - fp32-faithful arithmetic at 1/3 of the tensor-pipe rate; this is the parity mode.  The K loop
 // simply runs three "terms" per (tap, channel block); weights are stored [Cout][tap][channel block][2][64] = (hi, lo).
 // For layers with BN <= 128 output channels per tile the terms are concatenated along N instead of K ("ncat"): per K
-// step  x_hi * [w_hi | w_lo]  is ONE MMA of width 2 BN (main product into accumulator columns [0, BN), cross term into
-// [BN, 2 BN)) and  x_lo * w_hi  a second one into [BN, 2 BN) - two instructions instead of three, the x_hi / x_lo tiles
-// of a (tap, channel block) are loaded once, and the small cross terms own an accumulator (their sum never meets the
-// large main sum before the epilogue adds the two in fp32).
+// step  x_hi * w_hi  goes to accumulator columns [0, BN), and  x_hi * w_lo  then  x_lo * w_hi  to [BN, 2 BN) - the
+// x_hi / x_lo tiles of a (tap, channel block) are loaded once, and the small cross terms own an accumulator (their sum
+// never meets the large main sum before the epilogue adds the two in fp32).
+// Operand type and walk are template parameters (SPLIT, WALK): every K block is one straight-line MMA sequence, which
+// ptxas needs to keep the MMAs in flight.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
 #include <cstdlib>
 #include <mutex>
+#include <type_traits>
 #include <unordered_map>
 
 #include "common.cuh"
@@ -302,7 +304,6 @@ __device__ IdentBlocks16 g_ident16 = make_ident16();
 __device__ unsigned int g_f16_overflow = 0;
 
 // ----------------------------------------------------------------------------------------------- kernel
-// BN: accumulator width (32..256).  OUT_F32: fp32 output (head predictions) instead of bf16.
 constexpr int kStemPatchBytes = 24576;             // conv1's input patch in dynamic shared memory (5632 floats used)
 constexpr int kConsumers = 256;                    // two consumer warpgroups: MMA, then epilogue (warps 0-7)
 constexpr int kDP = 256;                           // deformable A-operand producer threads (warps 8 .. 8 + kDP/32 - 1)
@@ -337,29 +338,50 @@ __device__ __forceinline__ void stage_acc(const float (&acc)[R], int pass, bool 
     }
 }
 
-// accumulator columns [64 g, 64 g + 64) += A * B (the residual K blocks: residual tile x identity)
-template <int BN, int R>
-__device__ __forceinline__ void wgmma_cols64(float (&acc)[R], int g, uint64_t da, uint64_t db, bool bf16)
+// Main-loop walk of an instantiation (the MMA sequence of a K block is fixed at compile time: ptxas serialises wgmma
+// instructions that sit behind run-time branches).
+constexpr int kWalkK = 0;        // one stage per K block and term: bf16, or f16x3 with a stage per term (KIter mode 1)
+constexpr int kWalkNcat = 1;     // f16x3, terms concatenated along N: BN <= 128, TMA epilogue, no residual
+constexpr int kWalkDcat = 2;     // deformable f16x3: one stage carries x_hi | x_lo | w_hi | w_lo of a K block
+constexpr int kWalkKRes = 3;     // kWalkK, then the residual K blocks (res_mma: residual tile x identity into the accumulator)
+
+// accumulator columns [64 G, 64 G + 64) += A * B[rows 64 G ..]^T for G = 0 .. NG - 1: one width-64 MMA per column group
+// (the B rows of group G start 64 rows = 8 KiB further, 512 in the descriptor's address field)
+template <int NG, bool BF16, int R, int G = 0>
+__device__ __forceinline__ void wgmma_cols64(float (&acc)[R], uint64_t da, uint64_t db, uint32_t accumulate)
 {
-    if (g == 0) wgmma_n<64>(acc_view<0, 32>(acc), da, db, 1u, bf16);
-    if constexpr (BN >= 128) { if (g == 1) wgmma_n<64>(acc_view<32, 32>(acc), da, db, 1u, bf16); }
-    if constexpr (BN >= 256) {
-        if (g == 2) wgmma_n<64>(acc_view<64, 32>(acc), da, db, 1u, bf16);
-        if (g == 3) wgmma_n<64>(acc_view<96, 32>(acc), da, db, 1u, bf16);
-    }
+    wgmma_n<64, BF16>(acc_view<32 * G, 32>(acc), da, db + (uint64_t)(G * 512), accumulate);
+    if constexpr (G + 1 < NG) wgmma_cols64<NG, BF16, R, G + 1>(acc, da, db, accumulate);
 }
 
-// DEFORM: A operand produced by the warps from 8 on (bilinear gather) instead of TMA.
-template <int BN, bool OUT_F32, bool DEFORM>
+// Register budgets of the plain variant (384 threads launched with 168 registers each = 64 512 of the SM's 65 536): the
+// TMA producer's warpgroup gives registers back, the two consumer warpgroups take them for the accumulator and the
+// epilogue.  2 * 128 * 232 + 128 * 40 = 64 512.
+constexpr int kProducerRegs = 40;
+constexpr int kConsumerRegs = 232;
+
+// BN: accumulator width (32..256).  OUT_F32: fp32 output (head predictions) instead of bf16.  DEFORM: A operand produced
+// by the warps from 8 on (bilinear gather) instead of TMA.  SPLIT: f16x3 (fp16 operand pairs) instead of bf16.  WALK:
+// kWalkK / kWalkKRes / kWalkNcat / kWalkDcat.
+template <int BN, bool OUT_F32, bool DEFORM, bool SPLIT, int WALK>
 __global__ void __launch_bounds__(DEFORM ? kConsumers + kDP : kConsumers + 128, 1)
 conv_tc_kernel(const __grid_constant__ TcParams P, int stages)
 {
+    static_assert(WALK != kWalkNcat || (SPLIT && !DEFORM && !OUT_F32 && BN >= 64 && BN <= 128), "ncat: f16x3 TMA-epilogue layers, BN 64..128");
+    static_assert(!DEFORM || (WALK == kWalkDcat) == SPLIT, "deformable: dcat exactly in f16x3");
+    static_assert(DEFORM || WALK != kWalkDcat, "dcat is the deformable walk");
+    static_assert(WALK != kWalkKRes || (!DEFORM && !OUT_F32 && BN >= 64), "residual K blocks: TMA-epilogue layers");
+    constexpr bool kBF16 = !SPLIT;                     // operand type of every MMA
+    constexpr int kWTerms = SPLIT ? 2 : 1;             // weight K blocks per (tap, channel block): hi, lo
+    constexpr bool kCat = WALK == kWalkNcat || WALK == kWalkDcat;             // a stage holds both halves of both operands
+    constexpr int kKMode = (SPLIT && !kCat) ? 1 : 0;   // KIter mode: a stage per term
+    static_assert(kConsumers + 128 == 384 && 2 * 128 * kConsumerRegs + 128 * kProducerRegs <= 65536, "register split");
     // warp roles.  0-7: consumer warpgroups (wgmma main loop, then epilogue).  plain: 8 TMA producer (9-11 idle).
     // deformable / stem: 8-15 A-operand producers, their thread 0 also loads the B tiles.
     constexpr int kEpiThreads = kConsumers;
     constexpr int kWG = 2;                             // epilogue warps per 32-row quarter (one per 32-column half)
     // accumulator columns per thread group: the ncat layout (BN <= 128) keeps main | cross columns side by side
-    constexpr int kAccN = (!DEFORM && BN <= 128) ? 2 * BN : BN;
+    constexpr int kAccN = (WALK == kWalkNcat) ? 2 * BN : BN;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     // dynamic: [staged accumulator pass][identity][stem patch][resident B][stages: A 16K | B BN*128] then the output staging tile
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -367,9 +389,9 @@ conv_tc_kernel(const __grid_constant__ TcParams P, int stages)
     smem += kAccBytes;
     constexpr int kBBytes = BN * kBK * 2;
     // b_resident: [B slab: kblocks x kBBytes] then A-only stages; otherwise every stage carries A | B
-    const int kStageBytes = (P.ncat || P.dcat) ? (P.b_resident ? 2 * kABytes : 2 * kABytes + 2 * kBBytes)
-                                   : (P.b_resident ? kABytes : kABytes + kBBytes);
-    const int kblocks_all = P.KH * P.KW * P.cin_blocks * (P.split ? 2 : 1);   // weight K blocks (hi and lo halves in split mode)
+    const int kStageBytes = kCat ? (P.b_resident ? 2 * kABytes : 2 * kABytes + 2 * kBBytes)
+                                 : (P.b_resident ? kABytes : kABytes + kBBytes);
+    const int kblocks_all = P.KH * P.KW * P.cin_blocks * kWTerms;   // weight K blocks (hi and lo halves in split mode)
     uint8_t *ident = smem;                             // [8 KiB] identity block when res_mma
     if (P.res_mma) smem += 8192;
     float *s_patch = reinterpret_cast<float *>(smem);  // [24 KiB] conv1's input patch (stem transform only)
@@ -408,7 +430,7 @@ conv_tc_kernel(const __grid_constant__ TcParams P, int stages)
     }
     __syncthreads();
     const int taps_per = (P.KH * P.KW) / (P.ksplit > 1 ? P.ksplit : 1);              // taps of one K split
-    const int kblocks = taps_per * P.cin_blocks * ((P.split && !P.ncat && !P.dcat) ? 3 : 1);     // main-loop K blocks (stages) per tile
+    const int kblocks = taps_per * P.cin_blocks * (kKMode ? 3 : 1);     // main-loop K blocks (stages) per tile
     // Programmatic dependent launch: the next kernel in the stream may start its CTAs (barrier init, descriptor
     // prefetch - the code above) on SMs this grid has already left; nothing above touches global memory,
     // and everything below (loads AND stores) comes after the wait for the preceding grid to complete and flush.
@@ -417,11 +439,10 @@ conv_tc_kernel(const __grid_constant__ TcParams P, int stages)
 
     if (warp < kConsumers / 32) {
         // ===================================================== consumers: main loop
+        if constexpr (!DEFORM) setmaxnreg_inc<kConsumerRegs>();
         const int cw = warp >> 2;                          // consumer warpgroup: accumulator rows [64 cw, 64 cw + 64)
         const uint32_t a_off = (uint32_t)cw * 8192u;       // its 64 rows of a 128-row A tile (64 x 128 B)
         const bool leader = (threadIdx.x & 127) == 0;
-        const bool bf16 = !P.split;
-        const int wterms = P.split ? 2 : 1, rterms = P.split ? 2 : 1;
         float acc[kAccN / 2];
         Ring r(stages);
         // epilogue geometry: thread -> staged row rrow = q * 32 + lane, 32-column half wg of every 64-column pass
@@ -437,12 +458,12 @@ conv_tc_kernel(const __grid_constant__ TcParams P, int stages)
         if ((P.b_resident || P.res_mma) && (int)blockIdx.x < P.num_tiles) mbar_wait(&bres_bar, 0);
         for (int tile = blockIdx.x; tile < P.num_tiles; tile += gridDim.x) {
             int res_groups = 0;
-            if (!DEFORM && P.res_mma) {
+            if constexpr (WALK == kWalkKRes) {
                 const int nt = tile - (int)P.fd_ntn.div((uint32_t)tile) * P.n_tiles_n;
                 for (int g = 0; g < BN / 64 && nt * BN + g * 64 < P.Cout; ++g) ++res_groups;
             }
             const int tap_lo = ksplit_of(P, tile) * taps_per;
-            KIter it(tap_lo + taps_per, P.cin_blocks, (P.split && !P.ncat && !P.dcat) ? 1 : 0, tap_lo);   // same walk as the producer
+            KIter it(tap_lo + taps_per, P.cin_blocks, kKMode, tap_lo);   // same walk as the producer
             // A stage is released once the MMAs reading it have retired: with one commit group in flight, the stage
             // before the current one.
             int held = -1;
@@ -454,53 +475,77 @@ conv_tc_kernel(const __grid_constant__ TcParams P, int stages)
                 mbar_wait(&full[r.stage], r.phase);
                 const uint32_t sa = smem_u32(smem + (size_t)r.stage * kStageBytes);
                 const uint64_t da = make_desc_sw128(sa + a_off);
-                const int slab = (it.tap * P.cin_blocks + it.cb) * wterms + (it.term == 2 ? 1 : 0);
+                const int slab = (it.tap * P.cin_blocks + it.cb) * kWTerms + (it.term == 2 ? 1 : 0);
                 wgmma_fence();
-                if (P.ncat) {
-                    if constexpr (kAccN == 2 * BN) {
-                        // [w_hi | w_lo] are adjacent in the stage (and in the resident slab): one operand of 2 BN rows
-                        const uint64_t dl = make_desc_sw128(sa + kABytes + a_off);
-                        const uint64_t db = make_desc_sw128(P.b_resident ? smem_u32(bres + (size_t)slab * kBBytes) : sa + 2 * kABytes);
+                if constexpr (WALK == kWalkNcat) {
+                    // [w_hi | w_lo] are adjacent in the stage (and in the resident slab).  x_hi * w_hi goes to the main
+                    // columns, x_hi * w_lo then x_lo * w_hi to the cross columns.  All three MMAs have the width BN:
+                    // successive MMAs into the same accumulator registers are ordered without a wait only when their
+                    // shapes are equal.
+                    const uint32_t sb = P.b_resident ? smem_u32(bres + (size_t)slab * kBBytes) : sa + 2 * kABytes;
+                    const uint64_t dl = make_desc_sw128(sa + kABytes + a_off);
+                    const uint64_t dbh = make_desc_sw128(sb), dbl = make_desc_sw128(sb + kBBytes);
 #pragma unroll
-                        for (int k = 0; k < kBK / 16; ++k) {
-                            wgmma_n<2 * BN>(acc, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (kb | k) ? 1u : 0u, bf16);   // x_hi * [w_hi | w_lo]
-                            wgmma_n<BN>(acc_view<BN / 2, BN / 2>(acc), dl + (uint64_t)(k * 2), db + (uint64_t)(k * 2), 1u, bf16);  // x_lo * w_hi -> cross columns
-                        }
+                    for (int k = 0; k < kBK / 16; ++k) {
+                        const uint32_t first = (kb | k) ? 1u : 0u;
+                        wgmma_n<BN, kBF16>(acc_view<0, BN / 2>(acc), da + (uint64_t)(k * 2), dbh + (uint64_t)(k * 2), first);        // x_hi * w_hi
+                        wgmma_n<BN, kBF16>(acc_view<BN / 2, BN / 2>(acc), da + (uint64_t)(k * 2), dbl + (uint64_t)(k * 2), first);   // x_hi * w_lo
+                        wgmma_n<BN, kBF16>(acc_view<BN / 2, BN / 2>(acc), dl + (uint64_t)(k * 2), dbh + (uint64_t)(k * 2), 1u);      // x_lo * w_hi
                     }
-                } else if (P.dcat) {
+                } else if constexpr (WALK == kWalkDcat) {
                     const uint64_t dl = make_desc_sw128(sa + kABytes + a_off);
                     const uint64_t dbh = make_desc_sw128(sa + 2 * kABytes), dbl = make_desc_sw128(sa + 2 * kABytes + kBBytes);
 #pragma unroll
                     for (int k = 0; k < kBK / 16; ++k) {
-                        wgmma_n<BN>(acc_view<0, BN / 2>(acc), dl + (uint64_t)(k * 2), dbh + (uint64_t)(k * 2), (kb | k) ? 1u : 0u, bf16);   // x_lo * w_hi
-                        wgmma_n<BN>(acc_view<0, BN / 2>(acc), da + (uint64_t)(k * 2), dbl + (uint64_t)(k * 2), 1u, bf16);                   // x_hi * w_lo
-                        wgmma_n<BN>(acc_view<0, BN / 2>(acc), da + (uint64_t)(k * 2), dbh + (uint64_t)(k * 2), 1u, bf16);                   // x_hi * w_hi
+                        wgmma_n<BN, kBF16>(acc, dl + (uint64_t)(k * 2), dbh + (uint64_t)(k * 2), (kb | k) ? 1u : 0u);   // x_lo * w_hi
+                        wgmma_n<BN, kBF16>(acc, da + (uint64_t)(k * 2), dbl + (uint64_t)(k * 2), 1u);                   // x_hi * w_lo
+                        wgmma_n<BN, kBF16>(acc, da + (uint64_t)(k * 2), dbh + (uint64_t)(k * 2), 1u);                   // x_hi * w_hi
                     }
                 } else {
                     const uint64_t db = make_desc_sw128(P.b_resident ? smem_u32(bres + (size_t)slab * kBBytes) : sa + kABytes);
 #pragma unroll
-                    for (int k = 0; k < kBK / 16; ++k)
-                        wgmma_n<BN>(acc_view<0, BN / 2>(acc), da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (kb | k) ? 1u : 0u, bf16);
+                    for (int k = 0; k < kBK / 16; ++k) {
+                        if constexpr (WALK == kWalkKRes)     // the shape of the residual blocks' MMAs (see there)
+                            wgmma_cols64<BN / 64, kBF16>(acc, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (kb | k) ? 1u : 0u);
+                        else
+                            wgmma_n<BN, kBF16>(acc, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (kb | k) ? 1u : 0u);
+                    }
                 }
                 wgmma_commit();
                 wgmma_wait<1>();
                 release(r.stage);
                 r.next();
             }
-            if constexpr (!DEFORM && BN >= 64) {
-                for (int g = 0; g < res_groups * rterms; ++g) {
-                    // accumulator columns [64 g', 64 g' + 64) += residual tile * (scaled) identity, g' = g / rterms
-                    mbar_wait(&full[r.stage], r.phase);
-                    const uint64_t da = make_desc_sw128(smem_u32(smem + (size_t)r.stage * kStageBytes) + a_off);
-                    const uint64_t db = make_desc_sw128(smem_u32(ident));
-                    wgmma_fence();
+            if constexpr (WALK == kWalkKRes) {
+                // residual K blocks: accumulator columns [64 G, 64 G + 64) += residual tile * (scaled) identity, a block per
+                // group G and term, all MMAs of width 64 like the main loop's in this walk (with width-BN main-loop MMAs on
+                // the same registers ptxas serialises every MMA of the kernel, C7511).  The main loop's last group retires
+                // first, unconditionally: the epilogue would wait for it anyway.
+                wgmma_wait<0>();
+                release(-1);
+                auto res_group = [&](auto gc) {
+                    constexpr int G = decltype(gc)::value;
+                    if (G >= res_groups) return;
+#pragma unroll 1
+                    for (int t = 0; t < kWTerms; ++t) {
+                        mbar_wait(&full[r.stage], r.phase);
+                        const uint64_t da = make_desc_sw128(smem_u32(smem + (size_t)r.stage * kStageBytes) + a_off);
+                        const uint64_t db = make_desc_sw128(smem_u32(ident));
+                        wgmma_fence();
 #pragma unroll
-                    for (int k = 0; k < kBK / 16; ++k)
-                        wgmma_cols64<BN>(acc, g / rterms, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), bf16);
-                    wgmma_commit();
-                    wgmma_wait<1>();
-                    release(r.stage);
-                    r.next();
+                        for (int k = 0; k < kBK / 16; ++k)
+                            wgmma_n<64, kBF16>(acc_view<32 * G, 32>(acc), da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), 1u);
+                        wgmma_commit();
+                        wgmma_wait<1>();
+                        release(r.stage);
+                        r.next();
+                    }
+                };
+                res_group(std::integral_constant<int, 0>{});
+                if constexpr (BN >= 128) res_group(std::integral_constant<int, 1>{});
+                if constexpr (BN >= 256) {
+                    res_group(std::integral_constant<int, 2>{});
+                    res_group(std::integral_constant<int, 3>{});
                 }
             }
             wgmma_wait<0>();
@@ -785,6 +830,7 @@ conv_tc_kernel(const __grid_constant__ TcParams P, int stages)
         if (P.tma_epi && et == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // stores drained before exit
     } else if (!DEFORM) {
         // ===================================================== TMA producer
+        setmaxnreg_dec<kProducerRegs>();                   // the whole warpgroup (warps 9-11 are idle)
         if (warp == kConsumers / 32 && elect_one()) {
             Ring r(stages);
             if ((P.b_resident || P.res_mma) && (int)blockIdx.x < P.num_tiles) {
@@ -796,20 +842,19 @@ conv_tc_kernel(const __grid_constant__ TcParams P, int stages)
                     for (int kb = 0; kb < kblocks_all; ++kb)
                         tma_load_2d(bres + (size_t)kb * kBBytes, &P.tmB, &bres_bar, kb * kBK, nt0 * BN);
             }
-            const int wterms = P.split ? 2 : 1, rterms = P.split ? 2 : 1;
             for (int tile = blockIdx.x; tile < P.num_tiles; tile += gridDim.x) {
                 int pi, wb, hb, ib, nt;
                 decode_tile(P, tile, pi, wb, hb, ib, nt);
                 const Problem &pr = P.prob[pi];
                 const int w0 = wb * pr.BW * P.stride - P.pad, h0 = hb * pr.BH * P.stride - P.pad, i0 = ib * pr.BI;
                 const int tap_lo = ksplit_of(P, tile) * taps_per;
-                KIter it(tap_lo + taps_per, P.cin_blocks, (P.split && !P.ncat && !P.dcat) ? 1 : 0, tap_lo);
+                KIter it(tap_lo + taps_per, P.cin_blocks, kKMode, tap_lo);
                 for (int j = 0; j < kblocks; ++j, it.next()) {
                     const int kh = it.tap / P.KW, kw = it.tap - kh * P.KW;
                     mbar_wait(&empty[r.stage], r.phase ^ 1);
                     uint8_t *sa = smem + (size_t)r.stage * kStageBytes;
-                    const int wblk = ((it.tap * P.cin_blocks + it.cb) * wterms) * kBK;      // K offset of the (hi, lo) weight blocks
-                    if (P.ncat || P.dcat) {
+                    const int wblk = ((it.tap * P.cin_blocks + it.cb) * kWTerms) * kBK;      // K offset of the (hi, lo) weight blocks
+                    if constexpr (WALK == kWalkNcat) {
                         // one stage = x_hi tile | x_lo tile | w_hi block | w_lo block of this (tap, channel block)
                         mbar_expect_tx(&full[r.stage], 2 * kABytes + (P.b_resident ? 0 : 2 * kBBytes));
                         tma_load_5d(sa, &P.tmA[pi], &full[r.stage], it.cb * kBK, 0, w0 + kw, h0 + kh, i0);
@@ -826,11 +871,11 @@ conv_tc_kernel(const __grid_constant__ TcParams P, int stages)
                     }
                     r.next();
                 }
-                if (P.res_mma) {
+                if constexpr (WALK == kWalkKRes) {
                     // residual: one extra K block per 64 output channels (two in split mode: hi and lo), the A operand
                     // is the residual tile itself
                     for (int g = 0; g < BN / 64 && nt * BN + g * 64 < P.Cout; ++g)
-                        for (int t = 0; t < rterms; ++t) {
+                        for (int t = 0; t < kWTerms; ++t) {
                             mbar_wait(&empty[r.stage], r.phase ^ 1);
                             mbar_expect_tx(&full[r.stage], kABytes);
                             tma_load_5d(smem + (size_t)r.stage * kStageBytes, &P.tmRes[pi], &full[r.stage], nt * BN + g * 64, t,
@@ -1138,13 +1183,14 @@ thread_local TcTrace g_tc_trace[kEvPool];
 thread_local orp_tc_plan g_tc_plan;
 thread_local bool g_tc_plan_set = false;
 
-template <int BN, bool OUT_F32, bool DEFORM>
+template <int BN, bool OUT_F32, bool DEFORM, bool SPLIT, int WALK>
 int launch_tc(const TcParams &P, int stages, int grid, cudaStream_t st, int staging_bytes)
 {
-    const size_t stage_b = (P.ncat || P.dcat) ? (P.b_resident ? 2 * kABytes : 2 * kABytes + 2 * BN * kBK * 2)
-                                  : (P.b_resident ? kABytes : kABytes + BN * kBK * 2);
+    constexpr bool kCat = WALK == kWalkNcat || WALK == kWalkDcat;
+    const size_t stage_b = kCat ? (P.b_resident ? 2 * kABytes : 2 * kABytes + 2 * BN * kBK * 2)
+                                : (P.b_resident ? kABytes : kABytes + BN * kBK * 2);
     const size_t smem = 1024 + (size_t)kAccBytes + (size_t)stages * stage_b + (size_t)staging_bytes;
-    auto kern = conv_tc_kernel<BN, OUT_F32, DEFORM>;
+    auto kern = conv_tc_kernel<BN, OUT_F32, DEFORM, SPLIT, WALK>;
     static bool attr_set = false;
     if (!attr_set) {
         cudaFuncAttributes fa;
@@ -1187,6 +1233,34 @@ int launch_tc(const TcParams &P, int stages, int grid, cudaStream_t st, int stag
     ORP_LAUNCHED();
     if (slot >= 0) ORP_CUDA(cudaEventRecord(g_tc_ev[slot][1], st));
     return ORP_OK;
+}
+
+// the instantiation that runs a plan: operand type (P.split) and main-loop walk (P.ncat, P.dcat, P.res_mma) are
+// compile-time
+template <int BN, bool OUT_F32, bool DEFORM>
+int launch_plan(const TcParams &P, int stages, int grid, cudaStream_t st, int staging_bytes)
+{
+    if constexpr (DEFORM) {
+        if (P.dcat != P.split || P.ncat || P.res_mma) return fail(ORP_EINVAL, "conv2d_tc: deformable plan outside dcat == split");
+        return P.split ? launch_tc<BN, OUT_F32, true, true, kWalkDcat>(P, stages, grid, st, staging_bytes)
+                       : launch_tc<BN, OUT_F32, true, false, kWalkK>(P, stages, grid, st, staging_bytes);
+    } else {
+        if (P.ncat && P.res_mma) return fail(ORP_EINVAL, "conv2d_tc: ncat plan with a residual");
+        if (P.ncat) {
+            if constexpr (!OUT_F32 && BN >= 64 && BN <= 128) {
+                if (P.split) return launch_tc<BN, false, false, true, kWalkNcat>(P, stages, grid, st, staging_bytes);
+            }
+            return fail(ORP_EINVAL, "conv2d_tc: ncat plan outside f16x3 TMA-epilogue layers with BN 64..128");
+        }
+        if (P.res_mma) {
+            if constexpr (!OUT_F32 && BN >= 64)
+                return P.split ? launch_tc<BN, false, false, true, kWalkKRes>(P, stages, grid, st, staging_bytes)
+                               : launch_tc<BN, false, false, false, kWalkKRes>(P, stages, grid, st, staging_bytes);
+            return fail(ORP_EINVAL, "conv2d_tc: residual K blocks outside TMA-epilogue layers with BN >= 64");
+        }
+        return P.split ? launch_tc<BN, OUT_F32, false, true, kWalkK>(P, stages, grid, st, staging_bytes)
+                       : launch_tc<BN, OUT_F32, false, false, kWalkK>(P, stages, grid, st, staging_bytes);
+    }
 }
 
 }  // namespace
@@ -1621,9 +1695,9 @@ static int conv2d_bf16_impl(int nprob, const orp_tc_problem *probs, const void *
         launched = true;                                                                         \
         if (deform) {                                                                            \
             if constexpr (BNV <= 128)                                                            \
-                lrc = out_f32 ? launch_tc<BNV, true, true>(P, stages, grid, st, staging + bres_bytes) : launch_tc<BNV, false, true>(P, stages, grid, st, staging + bres_bytes); \
+                lrc = out_f32 ? launch_plan<BNV, true, true>(P, stages, grid, st, staging + bres_bytes) : launch_plan<BNV, false, true>(P, stages, grid, st, staging + bres_bytes); \
         }                                                                                        \
-        else lrc = out_f32 ? launch_tc<BNV, true, false>(P, stages, grid, st, staging + bres_bytes) : launch_tc<BNV, false, false>(P, stages, grid, st, staging + bres_bytes);       \
+        else lrc = out_f32 ? launch_plan<BNV, true, false>(P, stages, grid, st, staging + bres_bytes) : launch_plan<BNV, false, false>(P, stages, grid, st, staging + bres_bytes);       \
     }
     ORP_TC_DISPATCH(256)
     ORP_TC_DISPATCH(128)

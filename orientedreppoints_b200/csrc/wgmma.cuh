@@ -1,15 +1,17 @@
 // wgmma.cuh - warpgroup MMA (sm_90a) with fp32 register accumulators: D[64, N] (+)= A[64, 16] * B[N, 16]^T, both operands
-// K-major in shared memory behind matrix descriptors.  One wrapper per accumulator width; `bf16` selects bf16 or fp16
-// operands, `accumulate` = 0 overwrites D.  Fragment of thread t (warp w = t / 32 of the warpgroup, lane l):
+// K-major in shared memory behind matrix descriptors.  One wrapper per accumulator width; the template argument BF16
+// selects bf16 or fp16 operands at compile time (one instruction per instantiation: a run-time choice would put every
+// MMA behind a branch, and ptxas serialises wgmma there), `accumulate` = 0 overwrites D.  Fragment of thread t (warp w = t / 32 of the warpgroup, lane l):
 //   d[4 i + 2 h + j] = D[16 w + l / 4 + 8 h][8 i + 2 (l % 4) + j]
 #pragma once
 #include <stdint.h>
 
 namespace orp {
 
-__device__ __forceinline__ void wgmma_n32(float (&d)[16], uint64_t da, uint64_t db, uint32_t accumulate, bool bf16)
+template <bool BF16>
+__device__ __forceinline__ void wgmma_n32(float (&d)[16], uint64_t da, uint64_t db, uint32_t accumulate)
 {
-    if (bf16)
+    if constexpr (BF16)
         asm volatile(
             "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
             "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
@@ -23,9 +25,10 @@ __device__ __forceinline__ void wgmma_n32(float (&d)[16], uint64_t da, uint64_t 
             : "l"(da), "l"(db), "r"(accumulate));
 }
 
-__device__ __forceinline__ void wgmma_n64(float (&d)[32], uint64_t da, uint64_t db, uint32_t accumulate, bool bf16)
+template <bool BF16>
+__device__ __forceinline__ void wgmma_n64(float (&d)[32], uint64_t da, uint64_t db, uint32_t accumulate)
 {
-    if (bf16)
+    if constexpr (BF16)
         asm volatile(
             "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
             "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
@@ -39,9 +42,10 @@ __device__ __forceinline__ void wgmma_n64(float (&d)[32], uint64_t da, uint64_t 
             : "l"(da), "l"(db), "r"(accumulate));
 }
 
-__device__ __forceinline__ void wgmma_n128(float (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate, bool bf16)
+template <bool BF16>
+__device__ __forceinline__ void wgmma_n128(float (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate)
 {
-    if (bf16)
+    if constexpr (BF16)
         asm volatile(
             "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
             "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
@@ -55,9 +59,10 @@ __device__ __forceinline__ void wgmma_n128(float (&d)[64], uint64_t da, uint64_t
             : "l"(da), "l"(db), "r"(accumulate));
 }
 
-__device__ __forceinline__ void wgmma_n256(float (&d)[128], uint64_t da, uint64_t db, uint32_t accumulate, bool bf16)
+template <bool BF16>
+__device__ __forceinline__ void wgmma_n256(float (&d)[128], uint64_t da, uint64_t db, uint32_t accumulate)
 {
-    if (bf16)
+    if constexpr (BF16)
         asm volatile(
             "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
             "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1, 0, 0;\n\t}"
@@ -71,14 +76,14 @@ __device__ __forceinline__ void wgmma_n256(float (&d)[128], uint64_t da, uint64_
             : "l"(da), "l"(db), "r"(accumulate));
 }
 
-template <int N>
-__device__ __forceinline__ void wgmma_n(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t accumulate, bool bf16)
+template <int N, bool BF16>
+__device__ __forceinline__ void wgmma_n(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t accumulate)
 {
     static_assert(N == 32 || N == 64 || N == 128 || N == 256, "wgmma_n: unsupported width");
-    if constexpr (N == 32) wgmma_n32(d, da, db, accumulate, bf16);
-    else if constexpr (N == 64) wgmma_n64(d, da, db, accumulate, bf16);
-    else if constexpr (N == 128) wgmma_n128(d, da, db, accumulate, bf16);
-    else wgmma_n256(d, da, db, accumulate, bf16);
+    if constexpr (N == 32) wgmma_n32<BF16>(d, da, db, accumulate);
+    else if constexpr (N == 64) wgmma_n64<BF16>(d, da, db, accumulate);
+    else if constexpr (N == 128) wgmma_n128<BF16>(d, da, db, accumulate);
+    else wgmma_n256<BF16>(d, da, db, accumulate);
 }
 // registers [OFF, OFF + M) of a fragment: the accumulator of the columns [2 OFF, 2 OFF + 2 M)
 template <int OFF, int M, int R>
@@ -99,5 +104,13 @@ __device__ __forceinline__ void wgmma_fence_acc(float (&d)[R])
 #pragma unroll
     for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
+
+// per-thread register budget of the executing warpgroup (warpgroup-collective: all four warps execute it).  A decrease
+// returns registers to the CTA's pool; an increase waits until the pool holds them, so the warpgroups' budgets after the
+// change must not exceed what the CTA was launched with.
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 
 }  // namespace orp
