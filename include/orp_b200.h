@@ -163,7 +163,7 @@ typedef struct {
     int split;               /* f16x3 operands                                                               */
     int deform;              /* gathered (deformable) A operand                                              */
     int out_f32;             /* fp32 output (head predictions, split-K partial sums)                         */
-    int stem;                /* 0 none, 1 direct conv1, 2 space-to-depth conv1                               */
+    int stem;                /* 0 none, 2 space-to-depth conv1                                               */
     int relu;                /* epilogue activation: 0 none, 1 ReLU, 2 exact GELU                            */
     int bias;                /* a bias is added in the kernel's epilogue                                     */
     int residual;            /* 0 none, 1 16-bit residual (bf16 / split), 2 fp32 residual                    */
@@ -372,14 +372,8 @@ int orp_transpose_f32(const float *x, int N, int R, int Cc, float *y, void *stre
 /* NCHW fp32 [N, C, HW] -> split fp16 NHWC [N, HW, 2, C] in one pass (C % 8 == 0) */
 int orp_nchw_f32_to_split(const float *x, int N, int C, int HW, void *y_split, void *stream);
 
-/* conv1 of the ResNet stem (7x7, stride 2, pad 3, 3 channels; resnet.py:495) + folded BN + ReLU straight
- * from the NCHW fp32 image: the im2col rows (k = (kh*7+kw)*3 + c, K padded 147 -> 192) are built in shared
- * memory by producer warps, never in HBM.  w192: bf16 [64][192]; out: bf16 NHWC [N, H/2, W/2, 64]. */
-int orp_stem_conv_bf16(const float *img_nchw, int N, int H, int W, const void *w192, const float *bias, int relu,
-                       void *out, void *stream);
-/* the same im2col rows materialised (kept for tests / comparison):
- * conv1 of the ResNet stem as a GEMM: NCHW fp32 image -> bf16 [N,Ho,Wo,192] rows
- * (k = (kh*7+kw)*3 + c, zero above 147) */
+/* conv1 of the ResNet stem (7x7, stride 2, pad 3, 3 channels; resnet.py:495) as a GEMM (the bf16 stem for odd H or W):
+ * NCHW fp32 image -> bf16 [N,Ho,Wo,192] rows (k = (kh*7+kw)*3 + c, zero above 147) */
 int orp_stem_im2col_bf16(const float *img_nchw, int N, int H, int W, void *out, void *stream);
 /* default stem path: space-to-depth bf16 copy of the image, out[n][Y][X][(dy*2+dx)*3+c] = img[n][c][2(Y-2)+dy][2(X-2)+dx]
  * (zero outside, channels 12-15 zero; [N, H/2+3, W/2+3, 16]) - 1/12 of the im2col bytes - and conv1 as a 4x4 stride-1
@@ -398,10 +392,7 @@ int orp_stem_s2d_u8_padded_bf16(const uint8_t *img_hwc, int N, int H, int W, con
 int orp_maxpool3x3s2_bf16(const void *x, int N, int H, int W, int C, void *y, void *stream);
 /* GroupNorm over bf16 NHWC with C = 256, 32 groups: statistics (double [N,32,2], zeroed by caller) + apply */
 int orp_gn_stats_bf16(const void *x, int N, int HW, int C, int groups, double *stats, void *stream);
-int orp_gn_apply_bf16(const void *x, int N, int H, int W, int C, const double *stats, int groups,
-                      const float *gamma, const float *beta, float eps, int relu, const void *up_src, void *y,
-                      void *stream);
-/* the same for up to 8 tensors that share gamma / beta (the five pyramid levels of one head tower layer,
+/* apply to up to 8 tensors that share gamma / beta (the five pyramid levels of one head tower layer,
  * orientedreppoints_head.py:175-190) in one launch.  up_src (optional, [N,(H+1)/2,(W+1)/2,256]) is added after the
  * normalisation with nearest-neighbour upsampling (the FPN top-down path, fpn.py:171-176). */
 typedef struct orp_gn_problem {

@@ -108,7 +108,6 @@ SIGNATURES = {
     "orp_patch_embed_rows_u8_bf16": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, _vp, _vp]),
     "orp_patch_merge_gather_bf16": (_i, [_vp, _i, _i, _i, _i, _vp, _vp]),
     "orp_subsample2_bf16": (_i, [_vp, _i, _i, _i, _i, _vp, _vp]),
-    "orp_stem_conv_bf16": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, _vp, _vp]),
     "orp_layernorm_f16x3": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _f, _i, _i, _vp, _vp]),
     "orp_window_attention_f16x3": (_i, [_vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _f, _vp, _vp]),
     "orp_patch_embed_rows_f16x3": (_i, [_vp, _i, _i, _i, _vp, _vp]),
@@ -128,7 +127,6 @@ SIGNATURES = {
     "orp_stem_conv_s2d_bf16": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, _vp, _vp]),
     "orp_maxpool3x3s2_bf16": (_i, [_vp, _i, _i, _i, _i, _vp, _vp]),
     "orp_gn_stats_bf16": (_i, [_vp, _i, _i, _i, _i, _vp, _vp]),
-    "orp_gn_apply_bf16": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _vp, _vp, _f, _i, _vp, _vp, _vp]),
     "orp_gn_apply_bf16_multi": (_i, [_i, _vp, _i, _i, _vp, _vp, _f, _i, _vp]),
 }
 

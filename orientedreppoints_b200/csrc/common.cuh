@@ -67,4 +67,12 @@ static inline int ceil_div(long long a, long long b) { return (int)((a + b - 1) 
 // streaming multiprocessors of an H100 SXM: caps of grid-stride launches are multiples of it
 constexpr int kNumSMs = 132;
 
+// blocks of a grid-stride launch over `items`: enough for one item per thread, at most 16 per SM, at least one
+inline int grid_for(size_t items, int threads)
+{
+    const size_t g = (items + threads - 1) / threads;
+    const size_t cap = kNumSMs * 16;
+    return (int)(g < cap ? (g ? g : 1) : cap);
+}
+
 }  // namespace orp

@@ -103,14 +103,13 @@ struct alignas(64) TcParams {
     int res_mma;                              // residual added by the tensor core: extra K blocks  R[128x64] * I[64x64]
     int gn_fused;                             // GroupNorm statistics accumulated in the TMA epilogue (Cout == 256)
     int dcat;                                 // deformable split mode: one stage = sampled x_hi | x_lo | w_hi | w_lo of a K block
-    int stem;                                 // producers build conv1's 7x7/2 im2col rows from the NCHW fp32 image
-    int s2d_stem;                             // conv1 in space-to-depth form (host bookkeeping: 147 useful K of 256)
     int split;                                // f16x3 mode: fp16 (hi, lo) operand pairs, three MMA terms per K block
     float oscale;                             // epilogue multiplier 2^-s undoing the power-of-two weight scale (split mode)
     unsigned int *ovf;                        // split mode: count of outputs beyond the fp16 range (saturated)
     int nprob, num_m_tiles, n_tiles_n, num_tiles;
     FastDiv fd_ntn;                           // / n_tiles_n
     int KH, KW, Cin, cin_blocks, stride, pad, Cout, relu;
+    int s2d_stem;                             // conv1 in space-to-depth form (host bookkeeping: 147 useful K of 256)
     const float *bias;
 };
 
@@ -304,7 +303,6 @@ __device__ IdentBlocks16 g_ident16 = make_ident16();
 __device__ unsigned int g_f16_overflow = 0;
 
 // ----------------------------------------------------------------------------------------------- kernel
-constexpr int kStemPatchBytes = 24576;             // conv1's input patch in dynamic shared memory (5632 floats used)
 constexpr int kConsumers = 256;                    // two consumer warpgroups: MMA, then epilogue (warps 0-7)
 constexpr int kDP = 256;                           // deformable A-operand producer threads (warps 8 .. 8 + kDP/32 - 1)
 constexpr int kDItems = 1024 / kDP;                // (pixel row, 8-channel chunk) items of one 128 x 64 A block per thread
@@ -377,13 +375,13 @@ conv_tc_kernel(const __grid_constant__ TcParams P, int stages)
     constexpr int kKMode = (SPLIT && !kCat) ? 1 : 0;   // KIter mode: a stage per term
     static_assert(kConsumers + 128 == 384 && 2 * 128 * kConsumerRegs + 128 * kProducerRegs <= 65536, "register split");
     // warp roles.  0-7: consumer warpgroups (wgmma main loop, then epilogue).  plain: 8 TMA producer (9-11 idle).
-    // deformable / stem: 8-15 A-operand producers, their thread 0 also loads the B tiles.
+    // deformable: 8-15 A-operand producers, their thread 0 also loads the B tiles.
     constexpr int kEpiThreads = kConsumers;
     constexpr int kWG = 2;                             // epilogue warps per 32-row quarter (one per 32-column half)
     // accumulator columns per thread group: the ncat layout (BN <= 128) keeps main | cross columns side by side
     constexpr int kAccN = (WALK == kWalkNcat) ? 2 * BN : BN;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
-    // dynamic: [staged accumulator pass][identity][stem patch][resident B][stages: A 16K | B BN*128] then the output staging tile
+    // dynamic: [staged accumulator pass][identity][resident B][stages: A 16K | B BN*128] then the output staging tile
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     float *s_acc = reinterpret_cast<float *>(smem);
     smem += kAccBytes;
@@ -394,8 +392,6 @@ conv_tc_kernel(const __grid_constant__ TcParams P, int stages)
     const int kblocks_all = P.KH * P.KW * P.cin_blocks * kWTerms;   // weight K blocks (hi and lo halves in split mode)
     uint8_t *ident = smem;                             // [8 KiB] identity block when res_mma
     if (P.res_mma) smem += 8192;
-    float *s_patch = reinterpret_cast<float *>(smem);  // [24 KiB] conv1's input patch (stem transform only)
-    if (DEFORM && P.stem) smem += kStemPatchBytes;
     uint8_t *bres = smem;
     if (P.b_resident) smem += (size_t)kblocks_all * kBBytes;
     constexpr int HC = BN < 64 ? BN : 64;              // columns staged per epilogue pass
@@ -420,7 +416,7 @@ conv_tc_kernel(const __grid_constant__ TcParams P, int stages)
     if (warp == 0) {
         if (elect_one()) {
             for (int s = 0; s < stages; ++s) {
-                mbar_init(&full[s], DEFORM ? 1 + (P.stem ? 8 : kDP / 32) : 1);          // TMA expect_tx arrival (+ one arrival per producer warp)
+                mbar_init(&full[s], DEFORM ? 1 + kDP / 32 : 1);                          // TMA expect_tx arrival (+ one arrival per producer warp)
                 mbar_init(&empty[s], kConsumers / 128);                                 // one arrival per consumer warpgroup
             }
             mbar_init(&bres_bar, 1);
@@ -895,7 +891,7 @@ conv_tc_kernel(const __grid_constant__ TcParams P, int stages)
         __shared__ float4 s_w[2][128];
         __shared__ uint2 s_wh[2][128];                     // the same four weights as fp16 (split mode: blend of the lo halves)
         __shared__ int4 s_o[2][128];
-        const int pt = threadIdx.x - kConsumers;           // 0..kDP-1 (the stem transform uses the first 256)
+        const int pt = threadIdx.x - kConsumers;           // 0..kDP-1
         // the B tile(s) of a stage: thread 0 of the producers adds their bytes to the stage's barrier and issues the TMA loads
         auto load_b = [&](int stage, int tap, int cb, int nt) {
             uint8_t *sb = smem + (size_t)stage * kStageBytes + (P.dcat ? 2 * kABytes : kABytes);
@@ -906,85 +902,6 @@ conv_tc_kernel(const __grid_constant__ TcParams P, int stages)
         };
         Ring r(stages);
         int tb = 0;
-        if (P.stem && pt >= 256) {
-            // conv1's operand is built from a shared-memory patch: 8 warps are plenty
-        } else if (P.stem) {
-            // conv1 (resnet.py:495, 7x7 stride 2 pad 3, 3 input channels) as a GEMM with K = 192 (147 used),
-            // k = (kh*7 + kw)*3 + c.  Per tile the input patch ((2*BH+5) x (2*BW+5) pixels x 3 channels per image
-            // of the tile) is staged once in shared memory with coalesced loads of the NCHW fp32 image
-            // (pr.offset); the three 64-wide K blocks of A rows are then built from shared memory.
-            __shared__ __align__(16) int s_koff[192];                                      // k -> offset inside the patch (-1: k >= 147)
-            {
-                const Problem &p0 = P.prob[0];
-                const int pw0 = 2 * p0.BW + 5, ph0 = 2 * p0.BH + 5;
-                if (pt < 192) {
-                    const int tap = pt / 3, c = pt - tap * 3, kh = tap / 7, kw = tap - kh * 7;
-                    s_koff[pt] = pt < 147 ? (c * ph0 + kh) * pw0 + kw : -1;
-                }
-            }
-            for (int tile = blockIdx.x; tile < P.num_tiles; tile += gridDim.x) {
-                int pi, wb, hb, ib, nt;
-                decode_tile(P, tile, pi, wb, hb, ib, nt);
-                const Problem &pr = P.prob[pi];
-                const float *img = pr.offset;
-                const int pw = 2 * pr.BW + 5, ph = 2 * pr.BH + 5;            // patch extent per image
-                const int x0 = wb * pr.BW * 2 - 3, y0 = hb * pr.BH * 2 - 3;
-                const int per_img = 3 * ph * pw;
-                asm volatile("bar.sync 2, 256;" ::: "memory");               // previous tile's reads of the patch are done
-                {
-                    // one patch row (image, channel, y) per iteration: the row decode is warp-uniform, the loads of
-                    // different rows are independent (unrolled for memory-level parallelism) and coalesced along x
-                    const int nrows = pr.BI * 3 * ph;
-#pragma unroll 7
-                    for (int rowi = 0; rowi < nrows; ++rowi) {
-                        const int ii = rowi / (3 * ph), rem = rowi - ii * 3 * ph;
-                        const int c = rem / ph, py = rem - c * ph;
-                        const int n = ib * pr.BI + ii, yy = y0 + py;
-                        const bool rok = (n < pr.N) && (yy >= 0) && (yy < pr.H);
-                        const float *src = img + (((size_t)(rok ? n : 0) * 3 + c) * pr.H + (rok ? yy : 0)) * pr.W;
-                        for (int px = pt; px < pw; px += 256) {
-                            const int xx = x0 + px;
-                            s_patch[rowi * pw + px] = (rok && xx >= 0 && xx < pr.W) ? __ldg(src + xx) : 0.f;
-                        }
-                    }
-                }
-                asm volatile("bar.sync 2, 256;" ::: "memory");
-                int pbase[4];
-#pragma unroll
-                for (int it = 0; it < 4; ++it) {
-                    const int row = (pt + it * 256) >> 3;
-                    const int iw = row & (pr.BW - 1), ih = (row >> pr.lbw) & (pr.BH - 1), ii = row >> (pr.lbw + pr.lbh);
-                    pbase[it] = ii * per_img + (ih * 2) * pw + iw * 2;
-                }
-                const int c16 = pt & 7;
-                for (int kb = 0; kb < 3; ++kb) {
-                    mbar_wait(&empty[r.stage], r.phase ^ 1);
-                    if (pt == 0) load_b(r.stage, 0, kb, nt);
-                    uint8_t *sa = smem + (size_t)r.stage * kStageBytes;
-                    const int4 o0 = *reinterpret_cast<const int4 *>(&s_koff[kb * 64 + c16 * 8]);
-                    const int4 o1 = *reinterpret_cast<const int4 *>(&s_koff[kb * 64 + c16 * 8 + 4]);
-                    const int off[8] = {o0.x, o0.y, o0.z, o0.w, o1.x, o1.y, o1.z, o1.w};
-#pragma unroll
-                    for (int it = 0; it < 4; ++it) {
-                        const int row = (pt + it * 256) >> 3;
-                        float v[8];
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) v[j] = off[j] >= 0 ? s_patch[pbase[it] + off[j]] : 0.f;
-                        uint32_t pk[4];
-#pragma unroll
-                        for (int k2 = 0; k2 < 4; ++k2) {
-                            __nv_bfloat162 b2 = __floats2bfloat162_rn(v[2 * k2], v[2 * k2 + 1]);
-                            pk[k2] = *reinterpret_cast<uint32_t *>(&b2);
-                        }
-                        *reinterpret_cast<uint4 *>(sa + (size_t)row * 128 + ((c16 ^ (row & 7)) << 4)) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-                    }
-                    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                    __syncwarp();
-                    if ((pt & 31) == 0) mbar_arrive(&full[r.stage]);
-                    r.next();
-                }
-            }
-        } else
         for (int tile = blockIdx.x; tile < P.num_tiles; tile += gridDim.x) {
             int pi, wb, hb, ib, nt;
             decode_tile(P, tile, pi, wb, hb, ib, nt);
@@ -1210,7 +1127,7 @@ int launch_tc(const TcParams &P, int stages, int grid, cudaStream_t st, int stag
         double fl = 0;
         for (int i = 0; i < P.nprob; ++i)
             fl += 2.0 * P.prob[i].N * P.prob[i].Ho * P.prob[i].Wo * (double)P.Cout *
-                  (P.s2d_stem ? 147.0 : (double)P.KH * P.KW * (P.stem ? 147 : P.Cin));   // algorithmic K, not the padded one
+                  (P.s2d_stem ? 147.0 : (double)P.KH * P.KW * P.Cin);   // algorithmic K, not the padded one
         g_tc_flops += fl;
         g_tc_trace[slot] = TcTrace{P.nprob, P.prob[0].N, P.prob[0].H, P.prob[0].W, P.Cin, P.Cout, P.KH, P.stride, DEFORM ? 1 : 0,
                                    BN, P.num_tiles, grid, fl};
@@ -1298,6 +1215,7 @@ extern "C" int orp_tc_last_plan(orp_tc_plan *out)
     return ORP_OK;
 }
 
+// stem: 0, or 2 for conv1 in space-to-depth form (the value orp_tc_plan.stem reports)
 static int conv2d_bf16_impl(int nprob, const orp_tc_problem *probs, const void *w, int Cout, int Cout_padded, int KH,
                             int KW, int Cin, int stride, int pad, const float *bias, int relu, int out_f32,
                             int deform, int stem, void *stream, int split = 0, int wscale_log2 = 0, int ksplit = 1);
@@ -1342,19 +1260,6 @@ extern "C" int orp_f16x3_overflow_count(unsigned int *count, int reset)
         ORP_CUDA(cudaMemcpyToSymbol(g_f16_overflow, &z, sizeof(z)));
     }
     return ORP_OK;
-}
-
-/* see include/orp_b200.h */
-extern "C" int orp_stem_conv_bf16(const float *img_nchw, int N, int H, int W, const void *w192, const float *bias, int relu,
-                                  void *out, void *stream)
-{
-    if (!img_nchw || !w192 || !out || N < 1) return fail(ORP_EINVAL, "stem_conv_bf16: bad arguments");
-    orp_tc_problem q;
-    memset(&q, 0, sizeof(q));
-    q.x = img_nchw;                       // never dereferenced as bf16: the producers read q.offset
-    q.offset = img_nchw;
-    q.N = N; q.H = H; q.W = W; q.out = out;
-    return conv2d_bf16_impl(1, &q, w192, 64, 64, 1, 1, 192, 1, 0, bias, relu, 0, 1, 1, stream);
 }
 
 extern "C" int orp_stem_conv_s2d_bf16(const void *x_s2d, int N, int H, int W, const void *w256, const float *bias, int relu,
@@ -1440,10 +1345,7 @@ extern "C" int orp_conv2d_tc_splitk(const orp_tc_problem *prob, const void *w, i
     if (rc) return rc;
     void *ovf = nullptr;
     ORP_CUDA(cudaGetSymbolAddress(&ovf, g_f16_overflow));
-    const size_t items = pixels * (Cout / 8);
-    size_t g = (items + 255) / 256;
-    if (g > kNumSMs * 16) g = kNumSMs * 16;
-    splitk_finish_kernel<<<(unsigned)(g ? g : 1), 256, 0, st>>>(workspace, ksplit, pixels, Cout, bias, relu, f16x3 ? 1 : 0, prob->out,
+    splitk_finish_kernel<<<grid_for(pixels * (Cout / 8), 256), 256, 0, st>>>(workspace, ksplit, pixels, Cout, bias, relu, f16x3 ? 1 : 0, prob->out,
                                                                 static_cast<unsigned int *>(ovf));
     ORP_LAUNCHED();
     if (prob->gn_stats) {
@@ -1460,13 +1362,12 @@ static int conv2d_bf16_impl(int nprob, const orp_tc_problem *probs, const void *
 {
     if (nprob < 1 || nprob > kMaxProb || !probs || !w) return fail(ORP_EINVAL, "conv2d_tc: bad arguments");
     if (Cin % 8) return fail(ORP_EINVAL, "conv2d_tc: Cin must be a multiple of 8 (16-byte channel rows)");
-    if (deform && !stem && (Cin % kBK)) return fail(ORP_EINVAL, "conv2d_tc: deformable conv needs Cin % 64 == 0");
+    if (deform && (Cin % kBK)) return fail(ORP_EINVAL, "conv2d_tc: deformable conv needs Cin % 64 == 0");
     if (Cout_padded % 32 || Cout_padded < Cout) return fail(ORP_EINVAL, "conv2d_tc: padded Cout must be a multiple of 32");
-    if (split && stem == 1) return fail(ORP_EINVAL, "conv2d_tc: the direct stem has no f16x3 form (use the space-to-depth stem)");
     // a tile spans BW * stride <= 256 input columns (the TMA box limit) with BW >= 1
     if (stride < 1 || stride > 256) return fail(ORP_EINVAL, "conv2d_tc: stride must be in 1..256");
     // the deformable producers address the input with 32-bit element offsets (img0, s_o): N*H*W*Cin*planes must stay below 2^31
-    if (deform && !stem)
+    if (deform)
         for (int i = 0; i < nprob; ++i)
             if ((long long)probs[i].N * probs[i].H * probs[i].W * Cin * (split ? 2 : 1) >= (1LL << 31))
                 return fail(ORP_EINVAL, "conv2d_tc: deformable input has 2^31 or more 16-bit elements (32-bit sample offsets)");
@@ -1500,7 +1401,7 @@ static int conv2d_bf16_impl(int nprob, const orp_tc_problem *probs, const void *
     // a partial last channel block is zero-filled by TMA (A operand) and by the weight layout (B operand)
     P.nprob = nprob; P.KH = KH; P.KW = KW; P.Cin = Cin; P.cin_blocks = (Cin + kBK - 1) / kBK;
     P.stride = stride; P.pad = pad;
-    P.Cout = Cout; P.relu = relu; P.bias = bias; P.stem = (stem == 1) ? 1 : 0; P.s2d_stem = (stem == 2) ? 1 : 0;
+    P.Cout = Cout; P.relu = relu; P.bias = bias; P.s2d_stem = (stem == 2) ? 1 : 0;
     P.split = split ? 1 : 0;
     P.oscale = split ? ldexpf(1.f, -wscale_log2) : 1.f;
     {
@@ -1517,14 +1418,13 @@ static int conv2d_bf16_impl(int nprob, const orp_tc_problem *probs, const void *
         pr.N = q.N; pr.H = q.H; pr.W = q.W;
         pr.Ho = (q.H + 2 * pad - (KH - 1) - 1) / stride + 1;
         pr.Wo = (q.W + 2 * pad - (KW - 1) - 1) / stride + 1;
-        if (stem == 1) { pr.Ho = (q.H + 6 - 7) / 2 + 1; pr.Wo = (q.W + 6 - 7) / 2 + 1; }
         if (pr.Ho <= 0 || pr.Wo <= 0 || !q.x || !q.out) return fail(ORP_EINVAL, "conv2d_tc: bad problem");
         pr.BW = pow2_floor(pr.Wo < 128 ? pr.Wo : 128);
         // the TMA box spans BW * stride columns (<= 256); BW stays a power of two, as the row decode (& (BW - 1), lbw) needs
         if (stride * pr.BW > 256) pr.BW = pow2_floor(256 / stride);
         // (measured: 16 x 8 pixel tiles for the deformable variant change nothing - 1361 vs 1334 us per f16x3 launch, and neither
         // does the spread of the offsets: the gather runs at the ~47 GB/s per SM L2 -> SM ceiling whatever its locality)
-        if (deform && !stem && pr.BW > 16 && getenv("ORP_TC_DCN_2DTILES")) pr.BW = 16;
+        if (deform && pr.BW > 16 && getenv("ORP_TC_DCN_2DTILES")) pr.BW = 16;
         pr.BH = pow2_floor(pr.Ho < 128 / pr.BW ? pr.Ho : 128 / pr.BW);
         pr.BI = 128 / (pr.BW * pr.BH);
         pr.lbw = 0; while ((1 << pr.lbw) < pr.BW) ++pr.lbw;
@@ -1597,8 +1497,8 @@ static int conv2d_bf16_impl(int nprob, const orp_tc_problem *probs, const void *
     P.epi_merge = (split && P.tma_epi && (mem_bound || stem == 2) && !getenv("ORP_TC_NO_MERGE")) ? 1 : 0;
     // terms concatenated along N for narrow layers (kernel header); the residual / deformable / fp32-output variants keep
     // the K-concatenated walk
-    P.dcat = (split && deform && stem != 1) ? 1 : 0;
-    P.ncat = (split && P.tma_epi && BN <= 128 && !deform && !any_res && stem != 1 && !getenv("ORP_TC_NO_NCAT")) ? 1 : 0;
+    P.dcat = (split && deform) ? 1 : 0;
+    P.ncat = (split && P.tma_epi && BN <= 128 && !deform && !any_res && !getenv("ORP_TC_NO_NCAT")) ? 1 : 0;
     // residual through the tensor core (TMA epilogue only; the staged epilogue adds it itself)
     P.res_mma = (P.tma_epi && any_res) ? 1 : 0;
     if (P.res_mma) {
@@ -1657,11 +1557,11 @@ static int conv2d_bf16_impl(int nprob, const orp_tc_problem *probs, const void *
     for (;;) {
         stage_bytes = (P.ncat || P.dcat) ? (P.b_resident ? 2 * kABytes : 2 * kABytes + 2 * BN * kBK * 2)
                                          : (P.b_resident ? kABytes : kABytes + BN * kBK * 2);
-        bres_bytes = (P.b_resident ? KH * KW * T * P.cin_blocks * BN * kBK * 2 : 0) + (P.res_mma ? 8192 : 0) + (stem == 1 ? kStemPatchBytes : 0);
+        bres_bytes = (P.b_resident ? KH * KW * T * P.cin_blocks * BN * kBK * 2 : 0) + (P.res_mma ? 8192 : 0);
         const int hc = BN < 64 ? BN : 64;
         staging = out_f32 ? 0 : 128 * (hc * 2 + 16);
         if (P.tma_epi) staging = P.epi_bufs * (P.epi_merge ? 32768 : 16384);
-        stages = (int)((227 * 1024 - (deform || stem == 1 ? 14336 : 4096) - 1024 - kAccBytes - staging - bres_bytes) / stage_bytes);   // static shared memory of the variant
+        stages = (int)((227 * 1024 - (deform ? 14336 : 4096) - 1024 - kAccBytes - staging - bres_bytes) / stage_bytes);   // static shared memory of the variant
         if (stages >= 3) break;
         if (P.epi_bufs == 2) { P.epi_bufs = 1; continue; }
         if (P.b_resident) { P.b_resident = 0; continue; }

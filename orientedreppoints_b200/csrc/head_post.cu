@@ -217,13 +217,6 @@ dcn_offsets_kernel(const __grid_constant__ OffsetParams P)
     }
 }
 
-int grid_for(size_t items, int threads)
-{
-    size_t g = (items + threads - 1) / threads;
-    const size_t cap = kNumSMs * 16;
-    return (int)(g < cap ? (g ? g : 1) : cap);
-}
-
 }  // namespace
 }  // namespace orp
 

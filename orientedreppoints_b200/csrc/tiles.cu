@@ -38,13 +38,6 @@ split_tiles_kernel(const uint8_t *__restrict__ img, int H, int W, int C, const i
     }
 }
 
-int grid_for(size_t items, int threads)
-{
-    size_t g = (items + threads - 1) / threads;
-    const size_t cap = kNumSMs * 16;
-    return (int)(g < cap ? (g ? g : 1) : cap);
-}
-
 }  // namespace
 }  // namespace orp
 

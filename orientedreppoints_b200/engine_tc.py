@@ -1,6 +1,7 @@
 """Tensor-core engines of the dense path: wgmma implicit-GEMM convolutions (csrc/dense_tc.cu) plus their
-memory-bound companions (csrc/dense_bf16_misc.cu, csrc/dense_f16x3_misc.cu).  EngineTC: bf16 operands (fast, ~1e-2);
-EngineTCSplit: f16x3 split operands (fp32-faithful, the parity mode).  Same interface as detector.EngineF32."""
+memory-bound companions (csrc/dense_misc.cu).  EngineTC: bf16 operands (fast, ~1e-2); EngineTCSplit: f16x3 split
+operands (fp32-faithful, the parity mode).  Both run the same layer methods; a format is its activation layout (`alloc`,
+`dims`), its C entry points (`suffix`) and its weight packing.  Same interface as detector.EngineF32."""
 import ctypes
 
 import torch
@@ -18,10 +19,16 @@ def _valid(valid_hw, n, device):
 class EngineTC:
     name = "bf16"
     act_dtype = torch.bfloat16
+    suffix = "bf16"                                      # C-ABI entry points of this engine's activation format
 
     def __init__(self, device):
         self.device = device
         self.lib = _lib.lib()
+
+    def _call(self, name, *args):
+        """the C entry point name % suffix, looked up at call time (tests substitute entry points on the library)"""
+        fn = name % self.suffix
+        _lib.check(getattr(self.lib, fn)(*args), fn)
 
     # ------------------------------------------------------------------ weights
     def _tc(self, L):
@@ -44,84 +51,92 @@ class EngineTC:
             L.tc = dict(w=wp.to(self.device, torch.bfloat16).contiguous(), cout_p=64)
         return L.tc
 
+    @staticmethod
+    def _s2d_weights(L):
+        """conv1 weights for the space-to-depth form, fp32 [64][kh' 0..3][kw' 0..3][16] with ky = 2kh'+dy-1,
+        kx = 2kw'+dx-1, channel (dy*2+dx)*3+c (zero where ky/kx fall outside 0..6, channels 12-15 zero)"""
+        w = L.w_raw                                                  # [64, 7, 7, 3]
+        wp = torch.zeros((64, 4, 4, 16), dtype=torch.float32)
+        for khp in range(4):
+            for dy in range(2):
+                ky = 2 * khp + dy - 1
+                if not 0 <= ky <= 6:
+                    continue
+                for kwp in range(4):
+                    for dx in range(2):
+                        kx = 2 * kwp + dx - 1
+                        if not 0 <= kx <= 6:
+                            continue
+                        ch = (dy * 2 + dx) * 3
+                        wp[:, khp, kwp, ch:ch + 3] = w[:, ky, kx, :]
+        return wp
+
+    def _stem_s2d_tc(self, L):
+        if getattr(L, "tc_s2d", None) is None:
+            L.tc_s2d = self._s2d_weights(L).reshape(64, 256).to(self.device, torch.bfloat16).contiguous()
+        return L.tc_s2d
+
+    def _stem_s2d_operands(self, L):
+        """(weights, weight-scale arguments) of orp_stem_conv_s2d_*"""
+        return self._stem_s2d_tc(L), ()
+
+    @staticmethod
+    def _wscale(tc):
+        """the weight-scale argument of the f16x3 entry points (none in bf16)"""
+        return ()
+
     # ------------------------------------------------------------------ layers
     def prepare_input(self, img_nchw):
         img = img_nchw.to(self.device, torch.float32).contiguous()
         assert img.shape[1] == 3
         return img                                                   # the stem kernel reads the NCHW image directly
 
-    def _stem_s2d_tc(self, L):
-        """conv1 weights for the space-to-depth form: [64][kh' 0..3][kw' 0..3][16] with ky = 2kh'+dy-1,
-        kx = 2kw'+dx-1, channel (dy*2+dx)*3+c (zero where ky/kx fall outside 0..6, channels 12-15 zero)"""
-        if getattr(L, "tc_s2d", None) is None:
-            w = L.w_raw                                              # [64, 7, 7, 3]
-            wp = torch.zeros((64, 4, 4, 16), dtype=torch.float32)
-            for khp in range(4):
-                for dy in range(2):
-                    ky = 2 * khp + dy - 1
-                    if not 0 <= ky <= 6:
-                        continue
-                    for kwp in range(4):
-                        for dx in range(2):
-                            kx = 2 * kwp + dx - 1
-                            if not 0 <= kx <= 6:
-                                continue
-                            ch = (dy * 2 + dx) * 3
-                            wp[:, khp, kwp, ch:ch + 3] = w[:, ky, kx, :]
-            L.tc_s2d = wp.reshape(64, 256).to(self.device, torch.bfloat16).contiguous()
-        return L.tc_s2d
-
-    def stem(self, img, L, materialise=True, mode=None):
-        """conv1 + folded BN + ReLU.  mode "s2d" (default): space-to-depth bf16 copy of the image (1/12 of the im2col
-        bytes) + a 4x4 stride-1 tensor-core convolution reading it through TMA; "im2col": K=192 rows materialised in
-        HBM + plain GEMM; "direct": im2col rows built in shared memory by producer warps (no HBM intermediate)."""
+    def stem(self, img, L, mode="s2d"):
+        """conv1 + folded BN + ReLU.  mode "s2d" (default): space-to-depth copy of the image (1/12 of the im2col bytes)
+        + a 4x4 stride-1 tensor-core convolution reading it through TMA; "im2col" (bf16 only, also taken for odd H or W):
+        K=192 rows materialised in HBM + plain GEMM"""
+        assert mode in ("s2d", "im2col"), mode
         n, _, h, w = img.shape
-        if mode is None:
-            mode = "s2d" if materialise else "direct"
-        if mode == "s2d" and (h % 2 or w % 2):
-            mode = "im2col"
+        st = _lib.current_stream_ptr()
+        if mode == "s2d" and not (h % 2 or w % 2):
+            xs = self._s2d_input(n, h, w)
+            self._call("orp_stem_s2d_%s", _lib.ptr(img), n, h, w, _lib.ptr(xs), st)
+            return self._stem_conv_s2d(xs, L, n, h, w)
         ho, wo = (h + 6 - 7) // 2 + 1, (w + 6 - 7) // 2 + 1
         y = torch.empty((n, ho, wo, 64), dtype=torch.bfloat16, device=self.device)
-        st = _lib.current_stream_ptr()
-        if mode == "s2d":
-            ws = self._stem_s2d_tc(L)
-            xs = torch.empty((n, h // 2 + 3, w // 2 + 3, 16), dtype=torch.bfloat16, device=self.device)
-            _lib.check(self.lib.orp_stem_s2d_bf16(_lib.ptr(img), n, h, w, _lib.ptr(xs), st), "orp_stem_s2d_bf16")
-            _lib.check(self.lib.orp_stem_conv_s2d_bf16(_lib.ptr(xs), n, h, w, _lib.ptr(ws), _lib.ptr(L.bias), 1, _lib.ptr(y),
-                                                       st), "orp_stem_conv_s2d_bf16")
-            return y
-        tc = self._stem_tc(L)
-        if mode == "im2col":
-            cols = torch.empty((n, ho, wo, 192), dtype=torch.bfloat16, device=self.device)
-            _lib.check(self.lib.orp_stem_im2col_bf16(_lib.ptr(img), n, h, w, _lib.ptr(cols), st), "orp_stem_im2col_bf16")
-            self._launch([cols], [y], tc, 64, 1, 1, 192, 1, 0, L.bias, True, False, False)
-            return y
-        _lib.check(self.lib.orp_stem_conv_bf16(_lib.ptr(img), n, h, w, _lib.ptr(tc["w"]), _lib.ptr(L.bias), 1, _lib.ptr(y),
-                                               st), "orp_stem_conv_bf16")
+        cols = torch.empty((n, ho, wo, 192), dtype=torch.bfloat16, device=self.device)
+        _lib.check(self.lib.orp_stem_im2col_bf16(_lib.ptr(img), n, h, w, _lib.ptr(cols), st), "orp_stem_im2col_bf16")
+        self._launch([cols], [y], self._stem_tc(L), 64, 1, 1, 192, 1, 0, L.bias, True, False, False)
         return y
 
     def stem_u8(self, img_u8, L, norm_cfg, valid_hw=None):
         """conv1 + folded BN + ReLU from decoded uint8 HWC tiles [N,H,W,3]; Normalize (mean/std/to_rgb of the test
         pipeline) is applied inside the space-to-depth transform kernel, and so is the Pad that follows it when valid_hw
         (device int32 [N,2] per-image extents) is given: pixels outside enter as 0.0"""
-        import ctypes
         n, h, w, c = img_u8.shape
         assert c == 3 and img_u8.dtype == torch.uint8 and img_u8.is_contiguous() and h % 2 == 0 and w % 2 == 0
         st = _lib.current_stream_ptr()
-        ws = self._stem_s2d_tc(L)
-        xs = torch.empty((n, h // 2 + 3, w // 2 + 3, 16), dtype=torch.bfloat16, device=self.device)
+        xs = self._s2d_input(n, h, w)
         mean = (ctypes.c_float * 3)(*norm_cfg["mean"])
         std = (ctypes.c_float * 3)(*norm_cfg["std"])
+        to_rgb = int(bool(norm_cfg["to_rgb"]))
         if valid_hw is None:
-            _lib.check(self.lib.orp_stem_s2d_u8_bf16(_lib.ptr(img_u8), n, h, w, mean, std, int(bool(norm_cfg["to_rgb"])),
-                                                     _lib.ptr(xs), st), "orp_stem_s2d_u8_bf16")
+            self._call("orp_stem_s2d_u8_%s", _lib.ptr(img_u8), n, h, w, mean, std, to_rgb, _lib.ptr(xs), st)
         else:
-            _lib.check(self.lib.orp_stem_s2d_u8_padded_bf16(_lib.ptr(img_u8), n, h, w, mean, std, int(bool(norm_cfg["to_rgb"])),
-                                                            _lib.ptr(_valid(valid_hw, n, self.device)), _lib.ptr(xs), st),
-                       "orp_stem_s2d_u8_padded_bf16")
-        y = torch.empty((n, h // 2, w // 2, 64), dtype=torch.bfloat16, device=self.device)
-        _lib.check(self.lib.orp_stem_conv_s2d_bf16(_lib.ptr(xs), n, h, w, _lib.ptr(ws), _lib.ptr(L.bias), 1, _lib.ptr(y), st),
-                   "orp_stem_conv_s2d_bf16")
+            self._call("orp_stem_s2d_u8_padded_%s", _lib.ptr(img_u8), n, h, w, mean, std, to_rgb,
+                       _lib.ptr(_valid(valid_hw, n, self.device)), _lib.ptr(xs), st)
+        return self._stem_conv_s2d(xs, L, n, h, w)
+
+    def _s2d_input(self, n, h, w):
+        """the space-to-depth stem input: bf16 [N,H/2+3,W/2+3,16], or in split form its hi and lo planes one after the
+        other - in both formats the bytes of an activation tensor of that shape"""
+        return self.alloc(n, h // 2 + 3, w // 2 + 3, 16)
+
+    def _stem_conv_s2d(self, xs, L, n, h, w):
+        ws, scale = self._stem_s2d_operands(L)
+        y = self.alloc(n, h // 2, w // 2, 64)
+        self._call("orp_stem_conv_s2d_%s", _lib.ptr(xs), n, h, w, _lib.ptr(ws), _lib.ptr(L.bias), *scale, 1,
+                   _lib.ptr(y), _lib.current_stream_ptr())
         return y
 
     def _launch(self, xs, ys, tc, cout, kh, kw, cin, stride, pad, bias, relu, out_f32, deform, res=None, res32=None,
@@ -137,9 +152,8 @@ class EngineTC:
             arr[i].offset = offsets[i].data_ptr() if offsets is not None else None
             arr[i].gn_stats = stats[i].data_ptr() if stats is not None else None
             arr[i].mask = masks[i].data_ptr() if masks is not None else None
-        rc = self.lib.orp_conv2d_bf16(n, arr, _lib.ptr(tc["w"]), cout, tc["cout_p"], kh, kw, cin, stride, pad,
-                                      _lib.ptr(bias), int(relu), int(out_f32), int(deform), _lib.current_stream_ptr())
-        _lib.check(rc, "orp_conv2d_bf16")
+        self._call("orp_conv2d_%s", n, arr, _lib.ptr(tc["w"]), cout, tc["cout_p"], kh, kw, cin, stride, pad, _lib.ptr(bias),
+                   *self._wscale(tc), int(relu), int(out_f32), int(deform), _lib.current_stream_ptr())
 
     @staticmethod
     def _ksplit(n, ho, wo, L, nprob, relu, residual, out_f32, residual_f32):
@@ -168,15 +182,15 @@ class EngineTC:
         tc = self._tc(L)
         ys = []
         for x in xs:
-            n, h, w, cin = x.shape
-            assert cin == L.w_raw.shape[3] and x.dtype == torch.bfloat16
+            n, h, w, cin = self.dims(x)
+            assert cin == L.w_raw.shape[3] and x.dtype == self.act_dtype
             ho = (h + 2 * L.pad - L.kh) // L.stride + 1
             wo = (w + 2 * L.pad - L.kw) // L.stride + 1
-            ys.append(torch.empty((n, ho, wo, L.cout), dtype=torch.float32 if out_f32 else torch.bfloat16,
-                                  device=self.device))
+            ys.append(torch.empty((n, ho, wo, L.cout), dtype=torch.float32, device=self.device) if out_f32 else
+                      self.alloc(n, ho, wo, L.cout))
         ks = self._ksplit(ys[0].shape[0], ys[0].shape[1], ys[0].shape[2], L, len(xs), relu, residual, out_f32, residual_f32)
         if ks > 1:
-            self._conv_splitk(xs[0], ys[0], tc, L, relu, ks, None if stats is None else stats[0], False)
+            self._conv_splitk(xs[0], ys[0], tc, L, relu, ks, None if stats is None else stats[0], self.suffix == "f16x3")
             return ys
         self._launch(xs, ys, tc, L.cout, L.kh, L.kw, L.w_raw.shape[3], L.stride, L.pad, L.bias, relu, out_f32, False,
                      res=residual, res32=residual_f32, stats=stats)
@@ -193,21 +207,20 @@ class EngineTC:
         if stats is None:
             stats = []
             for x in xs:
-                n, h, w, c = x.shape
+                n, h, w, c = self.dims(x)
                 s = torch.zeros((n, 32, 2), dtype=torch.float64, device=self.device)
-                _lib.check(self.lib.orp_gn_stats_bf16(_lib.ptr(x), n, h * w, c, 32, _lib.ptr(s), st), "orp_gn_stats_bf16")
+                self._call("orp_gn_stats_%s", _lib.ptr(x), n, h * w, c, 32, _lib.ptr(s), st)
                 stats.append(s)
         ys = [torch.empty_like(x) for x in xs]
         arr = (_lib.GnProblem * k)()
         for i, x in enumerate(xs):
-            assert x.shape[3] == 256 and x.dtype == torch.bfloat16
+            assert self.dims(x)[3] == 256 and x.dtype == self.act_dtype
             arr[i].x = x.data_ptr()
             arr[i].N, arr[i].H, arr[i].W = x.shape[0], x.shape[1], x.shape[2]
             arr[i].stats = stats[i].data_ptr()
             arr[i].up_src = ups[i].data_ptr() if ups is not None and ups[i] is not None else None
             arr[i].y = ys[i].data_ptr()
-        _lib.check(self.lib.orp_gn_apply_bf16_multi(k, arr, 256, 32, _lib.ptr(norm.gamma), _lib.ptr(norm.beta), 1e-5,
-                                                    int(relu), st), "orp_gn_apply_bf16_multi")
+        self._call("orp_gn_apply_%s_multi", k, arr, 256, 32, _lib.ptr(norm.gamma), _lib.ptr(norm.beta), 1e-5, int(relu), st)
         return ys
 
     def gn(self, x, norm, relu=False, up=None, stats=None):
@@ -224,17 +237,14 @@ class EngineTC:
         return self.gn_multi(ys, norm, relu=relu, stats=[sts[i] for i in range(len(xs))])
 
     def maxpool(self, x):
-        n, h, w, c = x.shape
-        ho, wo = (h + 2 - 3) // 2 + 1, (w + 2 - 3) // 2 + 1
-        y = torch.empty((n, ho, wo, c), dtype=torch.bfloat16, device=self.device)
-        _lib.check(self.lib.orp_maxpool3x3s2_bf16(_lib.ptr(x), n, h, w, c, _lib.ptr(y), _lib.current_stream_ptr()),
-                   "orp_maxpool3x3s2_bf16")
+        n, h, w, c = self.dims(x)
+        y = self.alloc(n, (h + 2 - 3) // 2 + 1, (w + 2 - 3) // 2 + 1, c)
+        self._call("orp_maxpool3x3s2_%s", _lib.ptr(x), n, h, w, c, _lib.ptr(y), _lib.current_stream_ptr())
         return y
 
     def deform_conv_multi(self, xs, offsets, L, relu=False, masks=None):
         tc = self._tc(L)
-        ys = [torch.empty((x.shape[0], x.shape[1], x.shape[2], L.cout), dtype=torch.bfloat16, device=self.device)
-              for x in xs]
+        ys = [self.alloc(*self.dims(x)[:3], L.cout) for x in xs]
         self._launch(xs, ys, tc, L.cout, L.kh, L.kw, L.w_raw.shape[3], L.stride, L.pad, L.bias, relu, False, True,
                      offsets=offsets, masks=masks)
         return ys
@@ -250,8 +260,6 @@ class EngineTC:
 
     def from_float(self, x):
         return x.to(self.device, torch.bfloat16).contiguous()
-
-    suffix = "bf16"                                      # C-ABI entry points of this engine's activation format
 
     def alloc(self, b, h, w, c, zero=False):
         f = torch.zeros if zero else torch.empty
@@ -269,6 +277,7 @@ class EngineTCSplit(EngineTC):
     fp16 tensors [N,H,W,2,C] (hi channels, then lo channels)."""
     name = "f16x3"
     act_dtype = torch.float16
+    suffix = "f16x3"
 
     @staticmethod
     def _split_weights(wp):
@@ -316,26 +325,29 @@ class EngineTCSplit(EngineTC):
 
     def _stem_s2d_tc(self, L):
         if getattr(L, "tc3_s2d", None) is None:
-            w = L.w_raw                                              # [64, 7, 7, 3]
-            wp = torch.zeros((64, 4, 4, 16), dtype=torch.float32)
-            for khp in range(4):
-                for dy in range(2):
-                    ky = 2 * khp + dy - 1
-                    if not 0 <= ky <= 6:
-                        continue
-                    for kwp in range(4):
-                        for dx in range(2):
-                            kx = 2 * kwp + dx - 1
-                            if not 0 <= kx <= 6:
-                                continue
-                            ch = (dy * 2 + dx) * 3
-                            wp[:, khp, kwp, ch:ch + 3] = w[:, ky, kx, :]
-            hi, lo, s = self._split_weights(wp.reshape(64, 4, 64))   # taps = kh', 64 virtual channels = (kw', 16)
+            hi, lo, s = self._split_weights(self._s2d_weights(L).reshape(64, 4, 64))   # taps = kh', 64 virtual channels = (kw', 16)
             L.tc3_s2d = dict(w=torch.stack([hi, lo], dim=2).reshape(64, -1).to(self.device).contiguous(), s=s)
         return L.tc3_s2d
 
+    def _stem_s2d_operands(self, L):
+        ws = self._stem_s2d_tc(L)
+        return ws["w"], (ws["s"],)
+
+    @staticmethod
+    def _wscale(tc):
+        return (tc["s"],)
+
+    # the same launch as the class attribute of this engine: patching one engine class's _launch (as tests do to record
+    # which kernel a layer reaches) leaves the other's alone
+    _launch = EngineTC._launch
+
+    def stem(self, img, L, mode="s2d"):
+        assert img.shape[2] % 2 == 0 and img.shape[3] % 2 == 0 and mode == "s2d", \
+            "the f16x3 stem runs in space-to-depth form (even H, W)"
+        return super().stem(img, L, mode)
+
     def to_float(self, x):
-        n, h, w, _, c = x.shape
+        n, h, w, c = self.dims(x)
         y = torch.empty((n, h, w, c), dtype=torch.float32, device=self.device)
         _lib.check(self.lib.orp_split_to_f32(_lib.ptr(x), n * h * w, c, _lib.ptr(y), _lib.current_stream_ptr()), "orp_split_to_f32")
         return y
@@ -343,11 +355,9 @@ class EngineTCSplit(EngineTC):
     def from_float(self, x):
         x = x.to(self.device, torch.float32).contiguous()
         n, h, w, c = x.shape
-        y = torch.empty((n, h, w, 2, c), dtype=torch.float16, device=self.device)
+        y = self.alloc(n, h, w, c)
         _lib.check(self.lib.orp_split_from_f32(_lib.ptr(x), n * h * w, c, _lib.ptr(y), _lib.current_stream_ptr()), "orp_split_from_f32")
         return y
-
-    suffix = "f16x3"
 
     def alloc(self, b, h, w, c, zero=False):
         f = torch.zeros if zero else torch.empty
@@ -355,117 +365,11 @@ class EngineTCSplit(EngineTC):
 
     @staticmethod
     def dims(x):
-        b, h, w, _, c = x.shape
+        b, h, w, two, c = x.shape
+        assert two == 2, "split activations are [N,H,W,2,C]"
         return b, h, w, c
 
     def overflow_count(self, reset=True):
         c = ctypes.c_uint(0)
         _lib.check(self.lib.orp_f16x3_overflow_count(ctypes.byref(c), int(reset)), "orp_f16x3_overflow_count")
         return int(c.value)
-
-    def stem(self, img, L, materialise=True, mode=None):
-        n, _, h, w = img.shape
-        assert h % 2 == 0 and w % 2 == 0, "the f16x3 stem runs in space-to-depth form (even H, W)"
-        st = _lib.current_stream_ptr()
-        ws = self._stem_s2d_tc(L)
-        xs = torch.empty((2, n, h // 2 + 3, w // 2 + 3, 16), dtype=torch.float16, device=self.device)
-        _lib.check(self.lib.orp_stem_s2d_f16x3(_lib.ptr(img), n, h, w, _lib.ptr(xs), st), "orp_stem_s2d_f16x3")
-        y = torch.empty((n, h // 2, w // 2, 2, 64), dtype=torch.float16, device=self.device)
-        _lib.check(self.lib.orp_stem_conv_s2d_f16x3(_lib.ptr(xs), n, h, w, _lib.ptr(ws["w"]), _lib.ptr(L.bias), ws["s"], 1,
-                                                    _lib.ptr(y), st), "orp_stem_conv_s2d_f16x3")
-        return y
-
-    def stem_u8(self, img_u8, L, norm_cfg, valid_hw=None):
-        n, h, w, c = img_u8.shape
-        assert c == 3 and img_u8.dtype == torch.uint8 and img_u8.is_contiguous() and h % 2 == 0 and w % 2 == 0
-        st = _lib.current_stream_ptr()
-        ws = self._stem_s2d_tc(L)
-        xs = torch.empty((2, n, h // 2 + 3, w // 2 + 3, 16), dtype=torch.float16, device=self.device)
-        mean = (ctypes.c_float * 3)(*norm_cfg["mean"])
-        std = (ctypes.c_float * 3)(*norm_cfg["std"])
-        if valid_hw is None:
-            _lib.check(self.lib.orp_stem_s2d_u8_f16x3(_lib.ptr(img_u8), n, h, w, mean, std, int(bool(norm_cfg["to_rgb"])),
-                                                      _lib.ptr(xs), st), "orp_stem_s2d_u8_f16x3")
-        else:
-            _lib.check(self.lib.orp_stem_s2d_u8_padded_f16x3(_lib.ptr(img_u8), n, h, w, mean, std, int(bool(norm_cfg["to_rgb"])),
-                                                             _lib.ptr(_valid(valid_hw, n, self.device)), _lib.ptr(xs), st),
-                       "orp_stem_s2d_u8_padded_f16x3")
-        y = torch.empty((n, h // 2, w // 2, 2, 64), dtype=torch.float16, device=self.device)
-        _lib.check(self.lib.orp_stem_conv_s2d_f16x3(_lib.ptr(xs), n, h, w, _lib.ptr(ws["w"]), _lib.ptr(L.bias), ws["s"], 1,
-                                                    _lib.ptr(y), st), "orp_stem_conv_s2d_f16x3")
-        return y
-
-    def _launch(self, xs, ys, tc, cout, kh, kw, cin, stride, pad, bias, relu, out_f32, deform, res=None, res32=None,
-                offsets=None, stats=None, masks=None):
-        n = len(xs)
-        arr = (_lib.TcProblem * n)()
-        for i in range(n):
-            arr[i].x = xs[i].data_ptr()
-            arr[i].N, arr[i].H, arr[i].W = xs[i].shape[0], xs[i].shape[1], xs[i].shape[2]
-            arr[i].out = ys[i].data_ptr()
-            arr[i].residual_bf16 = res[i].data_ptr() if res is not None else None
-            arr[i].residual_f32 = res32[i].data_ptr() if res32 is not None else None
-            arr[i].offset = offsets[i].data_ptr() if offsets is not None else None
-            arr[i].gn_stats = stats[i].data_ptr() if stats is not None else None
-            arr[i].mask = masks[i].data_ptr() if masks is not None else None
-        rc = self.lib.orp_conv2d_f16x3(n, arr, _lib.ptr(tc["w"]), cout, tc["cout_p"], kh, kw, cin, stride, pad,
-                                       _lib.ptr(bias), tc["s"], int(relu), int(out_f32), int(deform),
-                                       _lib.current_stream_ptr())
-        _lib.check(rc, "orp_conv2d_f16x3")
-
-    def conv_multi(self, xs, L, relu=False, residual=None, out_f32=False, residual_f32=None, stats=None):
-        tc = self._tc(L)
-        ys = []
-        for x in xs:
-            n, h, w, two, cin = x.shape
-            assert two == 2 and cin == L.w_raw.shape[3] and x.dtype == torch.float16
-            ho = (h + 2 * L.pad - L.kh) // L.stride + 1
-            wo = (w + 2 * L.pad - L.kw) // L.stride + 1
-            ys.append(torch.empty((n, ho, wo, L.cout), dtype=torch.float32, device=self.device) if out_f32 else
-                      torch.empty((n, ho, wo, 2, L.cout), dtype=torch.float16, device=self.device))
-        ks = self._ksplit(ys[0].shape[0], ys[0].shape[1], ys[0].shape[2], L, len(xs), relu, residual, out_f32, residual_f32)
-        if ks > 1:
-            self._conv_splitk(xs[0], ys[0], tc, L, relu, ks, None if stats is None else stats[0], True)
-            return ys
-        self._launch(xs, ys, tc, L.cout, L.kh, L.kw, L.w_raw.shape[3], L.stride, L.pad, L.bias, relu, out_f32, False,
-                     res=residual, res32=residual_f32, stats=stats)
-        return ys
-
-    def gn_multi(self, xs, norm, relu=False, ups=None, stats=None):
-        st = _lib.current_stream_ptr()
-        k = len(xs)
-        if stats is None:
-            stats = []
-            for x in xs:
-                n, h, w, _, c = x.shape
-                s = torch.zeros((n, 32, 2), dtype=torch.float64, device=self.device)
-                _lib.check(self.lib.orp_gn_stats_f16x3(_lib.ptr(x), n, h * w, c, 32, _lib.ptr(s), st), "orp_gn_stats_f16x3")
-                stats.append(s)
-        ys = [torch.empty_like(x) for x in xs]
-        arr = (_lib.GnProblem * k)()
-        for i, x in enumerate(xs):
-            assert x.shape[4] == 256 and x.dtype == torch.float16
-            arr[i].x = x.data_ptr()
-            arr[i].N, arr[i].H, arr[i].W = x.shape[0], x.shape[1], x.shape[2]
-            arr[i].stats = stats[i].data_ptr()
-            arr[i].up_src = ups[i].data_ptr() if ups is not None and ups[i] is not None else None
-            arr[i].y = ys[i].data_ptr()
-        _lib.check(self.lib.orp_gn_apply_f16x3_multi(k, arr, 256, 32, _lib.ptr(norm.gamma), _lib.ptr(norm.beta), 1e-5,
-                                                     int(relu), st), "orp_gn_apply_f16x3_multi")
-        return ys
-
-    def maxpool(self, x):
-        n, h, w, _, c = x.shape
-        ho, wo = (h + 2 - 3) // 2 + 1, (w + 2 - 3) // 2 + 1
-        y = torch.empty((n, ho, wo, 2, c), dtype=torch.float16, device=self.device)
-        _lib.check(self.lib.orp_maxpool3x3s2_f16x3(_lib.ptr(x), n, h, w, c, _lib.ptr(y), _lib.current_stream_ptr()),
-                   "orp_maxpool3x3s2_f16x3")
-        return y
-
-    def deform_conv_multi(self, xs, offsets, L, relu=False, masks=None):
-        tc = self._tc(L)
-        ys = [torch.empty((x.shape[0], x.shape[1], x.shape[2], 2, L.cout), dtype=torch.float16, device=self.device)
-              for x in xs]
-        self._launch(xs, ys, tc, L.cout, L.kh, L.kw, L.w_raw.shape[3], L.stride, L.pad, L.bias, relu, False, True,
-                     offsets=offsets, masks=masks)
-        return ys

@@ -1,9 +1,9 @@
 """GPU: the memory-bound and token kernels of the benchmarked graphs against fp64 or bitwise against torch, once per
 launch signature the detector reaches.
 
-Kernels: csrc/dense_f16x3_misc.cu and csrc/dense_bf16_misc.cu (GroupNorm apply for up to 8 problems with the FPN
-top-down add and ReLU, GroupNorm statistics, the 3x3/2 max-pool, the stem's space-to-depth input from float, uint8 or
-uint8 with per-image extents) and csrc/swin.cu (LayerNorm into a plain or 7-padded grid, the mma.sync window attention,
+Kernels: csrc/dense_misc.cu (GroupNorm apply for up to 8 problems with the FPN top-down add and ReLU, GroupNorm
+statistics, the 3x3/2 max-pool, the stem's space-to-depth input from float, uint8 or uint8 with per-image extents) and
+csrc/swin.cu (LayerNorm into a plain or 7-padded grid, the mma.sync window attention,
 the patch-embed rows, the patch-merge gather, the stride-2 subsample of Swin P6 / P7).
 
 - A signature per kernel family reduces a launch to what selects code paths (`call_signature` reads it from the
