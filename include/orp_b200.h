@@ -150,7 +150,8 @@ int orp_rnms_last_sweep_ms(float *ms);
 int orp_tc_timing_collect(float *total_ms, int *launches, double *flops);
 /* The launch plan of this thread's most recent tensor-core convolution (orp_conv2d_bf16 / orp_conv2d_f16x3 /
  * orp_conv2d_tc_splitk / orp_stem_conv_*), as launched: the host code picks it from the shapes.  An observation point
- * for tests and traces (there is no way to request a plan).  ORP_EINVAL before the first launch on the thread. */
+ * for tests and traces: there is no way to request a plan (orp_tc_plan_conv only reports one).  ORP_EINVAL before the
+ * first launch on the thread. */
 typedef struct {
     int BN;                  /* accumulator width: 256, 128, 64 or 32 output channels per tile              */
     int stages;              /* main-loop pipeline stages                                                    */
@@ -348,6 +349,14 @@ int orp_conv2d_f16x3(int nprob, const orp_tc_problem *probs, const void *w_split
 int orp_conv2d_tc_splitk(const orp_tc_problem *prob, const void *w, int Cout, int Cout_padded, int KH, int KW, int Cin,
                          int stride, int pad, const float *bias, int f16x3, int wscale_log2, int relu, int ksplit,
                          float *workspace, void *stream);
+/* Dry run: the plan (as orp_tc_last_plan would report it) of the launch that these arguments make on a device with `sms`
+ * SMs, with the same argument checks and error codes.  split selects orp_conv2d_f16x3 over orp_conv2d_bf16 (wscale_log2
+ * is read in f16x3 only).  stem = 2: orp_stem_conv_s2d_* over probs[0]'s x, N, H, W (the image) and out; the geometry
+ * arguments are ignored.  ksplit > 1: the inner launch of orp_conv2d_tc_splitk over probs[0]; out_f32 and deform must be 0.
+ * Problem pointers are only tested for NULL, never read; no device is needed, and the last-plan record is untouched. */
+int orp_tc_plan_conv(int nprob, const orp_tc_problem *probs, const void *w, int Cout, int Cout_padded, int KH, int KW,
+                     int Cin, int stride, int pad, const float *bias, int wscale_log2, int relu, int out_f32, int deform,
+                     int split, int stem, int ksplit, int sms, orp_tc_plan *out);
 /* number of tile rows that saturated since the last reset (host-blocking read of a device counter) */
 int orp_f16x3_overflow_count(unsigned int *count, int reset);
 /* stem in split form: space-to-depth planes fp16 [2][N, H/2+3, W/2+3, 16] (hi plane, lo plane) from the uint8 HWC

@@ -91,6 +91,8 @@ SIGNATURES = {
     "orp_conv2d_bf16": (_i, [_i, ctypes.POINTER(TcProblem), _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _i, _i, _i, _vp]),
     "orp_conv2d_f16x3": (_i, [_i, ctypes.POINTER(TcProblem), _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _i, _i, _i, _i, _vp]),
     "orp_conv2d_tc_splitk": (_i, [ctypes.POINTER(TcProblem), _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _i, _i, _i, _i, _vp, _vp]),
+    "orp_tc_plan_conv": (_i, [_i, ctypes.POINTER(TcProblem), _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _i, _i, _i, _i, _i, _i, _i, _i,
+                              ctypes.POINTER(TcPlan)]),
     "orp_f16x3_overflow_count": (_i, [ctypes.POINTER(ctypes.c_uint), _i]),
     "orp_stem_s2d_u8_f16x3": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, _vp, _vp]),
     "orp_stem_s2d_f16x3": (_i, [_vp, _i, _i, _i, _vp, _vp]),
@@ -201,6 +203,27 @@ def tc_last_plan():
     """launch plan of this thread's most recent tensor-core convolution (dict of the orp_tc_plan fields)"""
     p = TcPlan()
     check(lib().orp_tc_last_plan(ctypes.byref(p)), "orp_tc_last_plan")
+    return p.as_dict()
+
+
+def tc_plan_for(problems, cout, cout_p, kh, kw, cin, stride, pad, *, bias=False, relu=0, out_f32=False, deform=False,
+                split=False, residual=0, gn=False, stem=0, ksplit=1, sms=132):
+    """the plan orp_tc_plan_conv reports for a launch over problems [(N, H, W), ...] (dict of the orp_tc_plan fields); the
+    pointers it passes are placeholders that the dry run only tests for NULL, so no device is needed.  residual: 0 none,
+    1 16-bit, 2 fp32; gn: GroupNorm statistics requested; stem = 2: problems hold the image; ksplit > 1: the inner launch of
+    the split-K convolution"""
+    ph = 256                                                # a non-NULL placeholder address
+    arr = (TcProblem * len(problems))()
+    for q, (n, h, w) in zip(arr, problems):
+        q.x, q.N, q.H, q.W, q.out = ph, n, h, w, ph
+        q.residual_bf16 = ph if residual == 1 else None
+        q.residual_f32 = ph if residual == 2 else None
+        q.offset = ph if deform else None
+        q.gn_stats = ph if gn else None
+    p = TcPlan()
+    check(lib().orp_tc_plan_conv(len(problems), arr, ph, cout, cout_p, kh, kw, cin, stride, pad, ph if bias else None, 0,
+                                 int(relu), int(out_f32), int(deform), int(split), stem, ksplit, sms, ctypes.byref(p)),
+          "orp_tc_plan_conv")
     return p.as_dict()
 
 

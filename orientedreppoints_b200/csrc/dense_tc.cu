@@ -42,7 +42,6 @@
 #include <cstdlib>
 #include <mutex>
 #include <type_traits>
-#include <unordered_map>
 
 #include "common.cuh"
 #include "wgmma.cuh"
@@ -310,6 +309,16 @@ constexpr int kDRound = kDItems / 2;               // items gathered together (t
 constexpr int kAccPitch = 68;                      // words per staged accumulator row: 64 columns + 4 (conflict-free 16-byte reads)
 constexpr int kAccBytes = 128 * kAccPitch * 4;     // one 64-column pass of the 128 x BN accumulator, fp32 (34 KiB)
 
+// bytes of one main-loop stage: the A tile (x_hi | x_lo when a stage carries both halves: ncat, dcat) and, unless the weight
+// slab of the CTA's N tile is resident, the B tile (w_hi | w_lo likewise)
+__host__ __device__ constexpr int stage_bytes(int BN, bool cat, bool b_resident)
+{
+    return cat ? (b_resident ? 2 * kABytes : 2 * kABytes + 2 * BN * kBK * 2) : (b_resident ? kABytes : kABytes + BN * kBK * 2);
+}
+// dynamic shared memory of a launch: 1 KiB alignment slack, the staged accumulator pass, `stages` main-loop stages and
+// `extra` bytes (identity block, resident weight slab, output staging)
+constexpr int dyn_smem_bytes(int stage_b, int stages, int extra) { return 1024 + kAccBytes + stages * stage_b + extra; }
+
 // Columns [64 pass, 64 pass + 64) of this thread's accumulator fragment -> the staged rows (ncat: main + cross columns,
 // added here in fp32 with round-to-nearest).  The pass loop is unrolled with a compile-time index so that the fragment
 // stays in registers.  row0 / col0: the fragment's first row and column (wgmma.cuh).
@@ -387,8 +396,7 @@ conv_tc_kernel(const __grid_constant__ TcParams P, int stages)
     smem += kAccBytes;
     constexpr int kBBytes = BN * kBK * 2;
     // b_resident: [B slab: kblocks x kBBytes] then A-only stages; otherwise every stage carries A | B
-    const int kStageBytes = kCat ? (P.b_resident ? 2 * kABytes : 2 * kABytes + 2 * kBBytes)
-                                 : (P.b_resident ? kABytes : kABytes + kBBytes);
+    const int kStageBytes = stage_bytes(BN, kCat, P.b_resident);
     const int kblocks_all = P.KH * P.KW * P.cin_blocks * kWTerms;   // weight K blocks (hi and lo halves in split mode)
     uint8_t *ident = smem;                             // [8 KiB] identity block when res_mma
     if (P.res_mma) smem += 8192;
@@ -1100,20 +1108,312 @@ thread_local TcTrace g_tc_trace[kEvPool];
 thread_local orp_tc_plan g_tc_plan;
 thread_local bool g_tc_plan_set = false;
 
+// shared memory one thread block of an H100 can opt into, and the static shared memory the budget sets aside for each variant
+// (barriers and bias slice; the deformable producers' sample tables too).  launch_tc checks the compiled size against the plan.
+constexpr int kSmemPerBlock = 227 * 1024;
+constexpr int kStaticSmemPlain = 4096;
+constexpr int kStaticSmemDeform = 14336;
+
+// what a launch asks for
+struct ConvDesc {
+    int nprob;
+    const orp_tc_problem *probs;
+    const void *w;
+    int Cout, Cout_padded, KH, KW, Cin, stride, pad;
+    const float *bias;
+    int relu, out_f32, deform;
+    int split;                                // f16x3 operands (0 / 1)
+    int wscale_log2;                          // f16x3: power-of-two weight scale
+    int stem;                                 // 0, or 2 for conv1 in space-to-depth form (the value orp_tc_plan.stem reports)
+    int ksplit;                               // split-K factor, >= 1
+};
+
+// how it runs: the plan orp_tc_last_plan reports, plus the tile geometry of every problem (Problem without its pointers)
+struct ConvPlan {
+    orp_tc_plan rep;
+    Problem prob[kMaxProb];
+    int num_m_tiles;
+    int extra_bytes;                          // dynamic shared memory beside the stages: identity, resident slab, output staging
+};
+
+// the checks that need no device (see orp_conv2d_bf16 / orp_conv2d_f16x3 in include/orp_b200.h)
+int check_conv(const ConvDesc &d)
+{
+    if (d.split && (d.wscale_log2 < 0 || d.wscale_log2 > 15)) return fail(ORP_EINVAL, "conv2d_f16x3: weight scale exponent must be in 0..15");
+    if (d.nprob < 1 || d.nprob > kMaxProb || !d.probs || !d.w) return fail(ORP_EINVAL, "conv2d_tc: bad arguments");
+    if (d.Cin % 8) return fail(ORP_EINVAL, "conv2d_tc: Cin must be a multiple of 8 (16-byte channel rows)");
+    if (d.deform && (d.Cin % kBK)) return fail(ORP_EINVAL, "conv2d_tc: deformable conv needs Cin % 64 == 0");
+    if (d.Cout_padded % 32 || d.Cout_padded < d.Cout) return fail(ORP_EINVAL, "conv2d_tc: padded Cout must be a multiple of 32");
+    // a tile spans BW * stride <= 256 input columns (the TMA box limit) with BW >= 1
+    if (d.stride < 1 || d.stride > 256) return fail(ORP_EINVAL, "conv2d_tc: stride must be in 1..256");
+    // the deformable producers address the input with 32-bit element offsets (img0, s_o): N*H*W*Cin*planes must stay below 2^31
+    if (d.deform)
+        for (int i = 0; i < d.nprob; ++i)
+            if ((long long)d.probs[i].N * d.probs[i].H * d.probs[i].W * d.Cin * (d.split ? 2 : 1) >= (1LL << 31))
+                return fail(ORP_EINVAL, "conv2d_tc: deformable input has 2^31 or more 16-bit elements (32-bit sample offsets)");
+    const orp_tc_problem &q0 = d.probs[0];
+    if (d.ksplit > 1 && (d.nprob != 1 || d.deform || d.stem || !d.out_f32 || (d.KH * d.KW) % d.ksplit || q0.residual_bf16 ||
+                         q0.residual_f32 || d.bias || d.relu))
+        return fail(ORP_EINVAL, "conv2d_tc: split-K serves one plain problem with an fp32 partial-sum output and taps % ksplit == 0");
+    return ORP_OK;
+}
+
+// The launch plan of a convolution on a device with `sms` SMs.  Pure: no CUDA call, no environment, no global state; the
+// problem pointers are only tested for NULL.
+int plan_conv(const ConvDesc &d, int sms, ConvPlan &pl)
+{
+    int rc = check_conv(d);
+    if (rc) return rc;
+    memset(&pl, 0, sizeof(pl));
+    const int nprob = d.nprob, ksplit = d.ksplit, T = d.split ? 2 : 1;   // T: 16-bit planes per value (hi, lo)
+    const orp_tc_problem *probs = d.probs;
+
+    int BN = 256;
+    if (d.Cout_padded % 256) BN = (d.Cout_padded % 128 == 0) ? 128 : (d.Cout_padded % 64 == 0) ? 64 : 32;
+    {
+        // narrower accumulators when the 128 x BN tiling would leave SMs idle
+        long long mtiles = 0;
+        for (int i = 0; i < nprob; ++i) {
+            const int ho = (probs[i].H + 2 * d.pad - (d.KH - 1) - 1) / d.stride + 1, wo = (probs[i].W + 2 * d.pad - (d.KW - 1) - 1) / d.stride + 1;
+            mtiles += ((long long)probs[i].N * ho * wo + 127) / 128;
+        }
+        while (BN > 64 && mtiles * (d.Cout_padded / BN) * ksplit < 120) BN /= 2;
+    }
+    // the deformable variant's 512 threads leave 128 registers each: a 64 x 128 fp32 accumulator fragment (64 per thread)
+    // fits beside the epilogue, a 64 x 256 one does not
+    if (d.deform && BN > 128) BN = 128;
+    // a partial last channel block is zero-filled by TMA (A operand) and by the weight layout (B operand)
+    const int cin_blocks = (d.Cin + kBK - 1) / kBK;
+    const int n_tiles_n = d.Cout_padded / BN;
+    int mt = 0;
+    for (int i = 0; i < nprob; ++i) {
+        const orp_tc_problem &q = probs[i];
+        Problem &pr = pl.prob[i];
+        pr.N = q.N; pr.H = q.H; pr.W = q.W;
+        pr.Ho = (q.H + 2 * d.pad - (d.KH - 1) - 1) / d.stride + 1;
+        pr.Wo = (q.W + 2 * d.pad - (d.KW - 1) - 1) / d.stride + 1;
+        if (pr.Ho <= 0 || pr.Wo <= 0 || !q.x || !q.out) return fail(ORP_EINVAL, "conv2d_tc: bad problem");
+        pr.BW = pow2_floor(pr.Wo < 128 ? pr.Wo : 128);
+        // the TMA box spans BW * stride columns (<= 256); BW stays a power of two, as the row decode (& (BW - 1), lbw) needs
+        if (d.stride * pr.BW > 256) pr.BW = pow2_floor(256 / d.stride);
+        // (measured: 16 x 8 pixel tiles for the deformable variant change nothing - 1361 vs 1334 us per f16x3 launch, and neither
+        // does the spread of the offsets: the gather runs at the ~47 GB/s per SM L2 -> SM ceiling whatever its locality)
+        pr.BH = pow2_floor(pr.Ho < 128 / pr.BW ? pr.Ho : 128 / pr.BW);
+        pr.BI = 128 / (pr.BW * pr.BH);
+        pr.lbw = 0; while ((1 << pr.lbw) < pr.BW) ++pr.lbw;
+        pr.lbh = 0; while ((1 << pr.lbh) < pr.BH) ++pr.lbh;
+        pr.tiles_w = ceil_div(pr.Wo, pr.BW); pr.tiles_h = ceil_div(pr.Ho, pr.BH); pr.tiles_i = ceil_div(pr.N, pr.BI);
+        pr.tile_start = mt;
+        pr.fd_tw.set((uint32_t)pr.tiles_w); pr.fd_th.set((uint32_t)pr.tiles_h);
+        mt += pr.tiles_w * pr.tiles_h * pr.tiles_i;
+        if (d.deform && !q.offset) return fail(ORP_EINVAL, "conv2d_tc: deformable conv needs offsets");
+    }
+    const int num_tiles = mt * n_tiles_n * ksplit;
+    // TMA epilogue: 16-bit outputs whose channel count is a multiple of 64
+    bool any_res = false;
+    for (int i = 0; i < nprob; ++i) any_res = any_res || (probs[i].residual_bf16 != nullptr);
+    // (f16x3 also takes channel counts that are only a multiple of 8 - Swin's 96 / 288: the TMA unit clips the last box)
+    const int tma_epi = (!d.out_f32 && ((d.Cout % 64 == 0) || (d.split && d.Cout % 8 == 0)) && BN >= 64) ? 1 : 0;
+    if (d.split && !d.out_f32 && !tma_epi) return fail(ORP_EINVAL, "conv2d_f16x3: 16-bit outputs need Cout % 8 == 0 and weights padded to a multiple of 64 rows");
+    if (d.split && d.out_f32 && any_res) return fail(ORP_EINVAL, "conv2d_f16x3: fp32 outputs take an fp32 residual only");
+    // GroupNorm statistics: fused into the TMA epilogue when every warp's 32 rows lie in one image
+    bool want_gn = false, gn_ok = tma_epi && d.Cout == 256 && !d.bias && !d.relu;
+    for (int i = 0; i < nprob; ++i) {
+        want_gn = want_gn || (probs[i].gn_stats != nullptr);
+        if (pl.prob[i].BW * pl.prob[i].BH < 32) gn_ok = false;
+    }
+    const int gn_fused = (want_gn && gn_ok) ? 1 : 0;
+    const bool mem_bound = any_res || (d.KH * d.KW * (d.Cin / kBK) <= 8);
+    int epi_bufs = mem_bound ? 2 : 1;          // a second staging tile costs compute-bound layers a main-loop stage
+    const int epi_merge = (d.split && tma_epi && (mem_bound || d.stem == 2)) ? 1 : 0;
+    // terms concatenated along N for narrow layers (kernel header); the residual / deformable / fp32-output variants keep
+    // the K-concatenated walk
+    const int dcat = (d.split && d.deform) ? 1 : 0;
+    const int ncat = (d.split && tma_epi && BN <= 128 && !d.deform && !any_res) ? 1 : 0;
+    // residual through the tensor core (TMA epilogue only; the staged epilogue adds it itself)
+    const int res_mma = (tma_epi && any_res) ? 1 : 0;
+    if (res_mma) {
+        if (d.deform) return fail(ORP_EINVAL, "conv2d_tc: residual is not supported on the deformable path");
+        for (int i = 0; i < nprob; ++i)
+            if (!probs[i].residual_bf16) return fail(ORP_EINVAL, "conv2d_tc: residual must be given for every problem or none");
+    }
+    // layers whose whole weight slab for one N tile is <= 72 KiB keep it resident; stages then carry only the A tile
+    const int slab_bytes = d.KH * d.KW * T * cin_blocks * BN * kBK * 2;
+    int b_resident = (!d.deform && ksplit == 1 && slab_bytes <= 72 * 1024) ? 1 : 0;
+    int grid = num_tiles < sms ? num_tiles : sms;
+    if (b_resident && grid >= n_tiles_n) grid -= grid % n_tiles_n;       // fixed N tile per CTA
+    else if (b_resident) b_resident = 0;
+    // shared-memory budget: staged accumulator pass + output staging + resident weights + main-loop stages.  When the extras
+    // leave fewer than three stages they are given up in order of least value: the second staging slot, the resident slab.
+    int stage_b = 0, extra = 0, stages = 0;
+    for (;;) {
+        stage_b = stage_bytes(BN, ncat || dcat, b_resident);
+        const int hc = BN < 64 ? BN : 64;
+        int staging = d.out_f32 ? 0 : 128 * (hc * 2 + 16);
+        if (tma_epi) staging = epi_bufs * (epi_merge ? 32768 : 16384);
+        extra = (res_mma ? 8192 : 0) + (b_resident ? slab_bytes : 0) + staging;
+        stages = (kSmemPerBlock - (d.deform ? kStaticSmemDeform : kStaticSmemPlain) - dyn_smem_bytes(stage_b, 0, extra)) / stage_b;
+        if (stages >= 3) break;
+        if (epi_bufs == 2) { epi_bufs = 1; continue; }
+        if (b_resident) { b_resident = 0; continue; }
+        if (stages >= 2) break;
+        return fail(ORP_EINVAL, "conv2d_tc: shared-memory budget cannot hold two main-loop stages");
+    }
+    if (stages > kStagesMax) stages = kStagesMax;
+    if (d.deform && stages > 3) stages = 3;     // leave L1 capacity for the bilinear gather (corner reuse between neighbouring pixels)
+
+    pl.num_m_tiles = mt;
+    pl.extra_bytes = extra;
+    orp_tc_plan &r = pl.rep;
+    r.BN = BN; r.stages = stages; r.grid = grid; r.num_tiles = num_tiles; r.n_tiles_n = n_tiles_n;
+    r.ksplit = ksplit; r.nprob = nprob; r.Cout = d.Cout; r.Cout_padded = d.Cout_padded;
+    r.split = d.split ? 1 : 0; r.deform = d.deform ? 1 : 0; r.out_f32 = d.out_f32 ? 1 : 0; r.stem = d.stem; r.relu = d.relu;
+    r.bias = d.bias ? 1 : 0;
+    for (int i = 0; i < nprob; ++i) {
+        if (probs[i].residual_bf16) r.residual = 1;
+        else if (probs[i].residual_f32) r.residual = 2;
+        r.BW[i] = pl.prob[i].BW; r.BH[i] = pl.prob[i].BH; r.BI[i] = pl.prob[i].BI;
+    }
+    r.tma_epi = tma_epi; r.ncat = ncat; r.dcat = dcat; r.res_mma = res_mma; r.b_resident = b_resident;
+    r.epi_merge = epi_merge; r.epi_bufs = epi_bufs; r.gn_fused = gn_fused;
+    return ORP_OK;
+}
+
+// the kernel's parameter block of a plan, tensor maps aside
+int make_params(const ConvDesc &d, const ConvPlan &pl, TcParams &P)
+{
+    memset(&P, 0, sizeof(P));
+    P.nprob = d.nprob; P.KH = d.KH; P.KW = d.KW; P.Cin = d.Cin; P.cin_blocks = (d.Cin + kBK - 1) / kBK;
+    P.stride = d.stride; P.pad = d.pad;
+    P.Cout = d.Cout; P.relu = d.relu; P.bias = d.bias; P.s2d_stem = (d.stem == 2) ? 1 : 0;
+    P.split = d.split ? 1 : 0;
+    P.oscale = d.split ? ldexpf(1.f, -d.wscale_log2) : 1.f;
+    {
+        void *ovf = nullptr;
+        ORP_CUDA(cudaGetSymbolAddress(&ovf, g_f16_overflow));
+        P.ovf = static_cast<unsigned int *>(ovf);
+    }
+    P.n_tiles_n = pl.rep.n_tiles_n;
+    P.fd_ntn.set((uint32_t)P.n_tiles_n);
+    for (int i = 0; i < d.nprob; ++i) {
+        const orp_tc_problem &q = d.probs[i];
+        Problem &pr = P.prob[i];
+        pr = pl.prob[i];
+        pr.out = q.out; pr.res = static_cast<const __nv_bfloat16 *>(q.residual_bf16); pr.res32 = q.residual_f32;
+        pr.x = static_cast<const __nv_bfloat16 *>(q.x); pr.offset = q.offset; pr.gn_stats = q.gn_stats; pr.mask = q.mask;
+    }
+    P.num_m_tiles = pl.num_m_tiles;
+    P.num_tiles = pl.rep.num_tiles;
+    P.ksplit = d.ksplit;
+    P.fd_ks.set((uint32_t)d.ksplit);
+    P.ks_stride = (long long)P.prob[0].N * P.prob[0].Ho * P.prob[0].Wo * d.Cout;
+    P.tma_epi = pl.rep.tma_epi; P.epi_bufs = pl.rep.epi_bufs; P.epi_merge = pl.rep.epi_merge; P.ncat = pl.rep.ncat;
+    P.b_resident = pl.rep.b_resident; P.res_mma = pl.rep.res_mma; P.gn_fused = pl.rep.gn_fused; P.dcat = pl.rep.dcat;
+    return ORP_OK;
+}
+
+// the tensor maps of a launch: A (plain variant), B, the identity (res_mma), output and residual (TMA epilogue)
+int encode_maps(const ConvDesc &d, const ConvPlan &pl, TcParams &P)
+{
+    EncodeTiledFn enc = encode_fn();
+    if (!enc) return fail(ORP_ECUDA, "conv2d_tc: cuTensorMapEncodeTiled unavailable");
+    const CUtensorMapDataType dt16 = d.split ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+    const int T = d.split ? 2 : 1, Cin = d.Cin, Cout = d.Cout, stride = d.stride;
+    if (!d.deform) {
+        for (int i = 0; i < d.nprob; ++i) {
+            const orp_tc_problem &q = d.probs[i];
+            const Problem &pr = P.prob[i];
+            // 5-D view {channel, plane (hi / lo), w, h, image}; bf16 tensors have a single plane.  Split activations are
+            // [N,H,W,2,C]: the lo plane of a pixel follows its hi plane.
+            cuuint64_t gdim[5] = {(cuuint64_t)Cin, (cuuint64_t)T, (cuuint64_t)q.W, (cuuint64_t)q.H, (cuuint64_t)q.N};
+            cuuint64_t gstr[4] = {(cuuint64_t)Cin * 2, (cuuint64_t)Cin * 2 * T, (cuuint64_t)q.W * Cin * 2 * T,
+                                  (cuuint64_t)q.H * q.W * Cin * 2 * T};
+            if (d.stem == 2) {
+                // space-to-depth stem: the tensor is [T][N, H, W + 3, 16] (planes outermost); a 64-element "pixel" row of
+                // the GEMM is the 4 horizontally adjacent 16-channel pixels starting at w, so consecutive w overlap
+                // (stride 32 bytes)
+                gstr[0] = (cuuint64_t)q.N * q.H * (q.W + 3) * 32;
+                gstr[1] = 32;
+                gstr[2] = (cuuint64_t)(q.W + 3) * 32;
+                gstr[3] = (cuuint64_t)q.H * (q.W + 3) * 32;
+            }
+            cuuint32_t box[5] = {(cuuint32_t)kBK, 1u, (cuuint32_t)(pr.BW * stride), (cuuint32_t)(pr.BH * stride), (cuuint32_t)pr.BI};
+            cuuint32_t estr[5] = {1, 1, (cuuint32_t)stride, (cuuint32_t)stride, 1};
+            CUresult r = enc(&P.tmA[i], dt16, 5, const_cast<void *>(q.x), gdim, gstr, box, estr,
+                             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+            if (r != CUDA_SUCCESS) return fail(ORP_ECUDA, "conv2d_tc: cuTensorMapEncodeTiled(A) failed");
+        }
+    }
+    {
+        // weights [Cout_padded][tap][cin_blocks][T][64] (zero padded per tap; T = 2: the hi block, then the lo block)
+        const cuuint64_t K = (cuuint64_t)d.KH * d.KW * T * P.cin_blocks * kBK;
+        cuuint64_t gdim[2] = {K, (cuuint64_t)d.Cout_padded};
+        cuuint64_t gstr[1] = {K * 2};
+        cuuint32_t box[2] = {(cuuint32_t)kBK, (cuuint32_t)pl.rep.BN};
+        cuuint32_t estr[2] = {1, 1};
+        CUresult r = enc(&P.tmB, dt16, 2, const_cast<void *>(d.w), gdim, gstr, box, estr,
+                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+        if (r != CUDA_SUCCESS) return fail(ORP_ECUDA, "conv2d_tc: cuTensorMapEncodeTiled(B) failed");
+    }
+    if (P.res_mma) {
+        void *ident_ptr = nullptr;
+        if (d.split) {
+            ORP_CUDA(cudaGetSymbolAddress(&ident_ptr, g_ident16));
+            ident_ptr = static_cast<char *>(ident_ptr) + (size_t)d.wscale_log2 * 8192;
+        } else {
+            ORP_CUDA(cudaGetSymbolAddress(&ident_ptr, g_ident));
+        }
+        cuuint64_t gdim[2] = {64, 64};
+        cuuint64_t gstr[1] = {128};
+        cuuint32_t box[2] = {64, 64};
+        cuuint32_t estr[2] = {1, 1};
+        CUresult r = enc(&P.tmI, dt16, 2, ident_ptr, gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                         CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+        if (r != CUDA_SUCCESS) return fail(ORP_ECUDA, "conv2d_tc: cuTensorMapEncodeTiled(identity) failed");
+    }
+    if (P.tma_epi) {
+        for (int i = 0; i < d.nprob; ++i) {
+            const Problem &pr = P.prob[i];
+            cuuint64_t gdim[5] = {(cuuint64_t)Cout, (cuuint64_t)T, (cuuint64_t)pr.Wo, (cuuint64_t)pr.Ho, (cuuint64_t)pr.N};
+            cuuint64_t gstr[4] = {(cuuint64_t)Cout * 2, (cuuint64_t)Cout * 2 * T, (cuuint64_t)pr.Wo * Cout * 2 * T,
+                                  (cuuint64_t)pr.Ho * pr.Wo * Cout * 2 * T};
+            cuuint32_t box[5] = {64u, 1u, (cuuint32_t)pr.BW, (cuuint32_t)pr.BH, (cuuint32_t)pr.BI};
+            cuuint32_t estr[5] = {1, 1, 1, 1, 1};
+            CUresult r = enc(&P.tmOut[i], dt16, 5, pr.out, gdim, gstr, box, estr,
+                             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
+                             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+            if (r != CUDA_SUCCESS) return fail(ORP_ECUDA, "conv2d_tc: cuTensorMapEncodeTiled(out) failed");
+            if (pr.res) {
+                r = enc(&P.tmRes[i], dt16, 5, const_cast<__nv_bfloat16 *>(pr.res), gdim, gstr, box, estr,
+                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                if (r != CUDA_SUCCESS) return fail(ORP_ECUDA, "conv2d_tc: cuTensorMapEncodeTiled(residual) failed");
+            }
+        }
+    }
+    return ORP_OK;
+}
+
 template <int BN, bool OUT_F32, bool DEFORM, bool SPLIT, int WALK>
-int launch_tc(const TcParams &P, int stages, int grid, cudaStream_t st, int staging_bytes)
+int launch_tc(const TcParams &P, int stages, int grid, cudaStream_t st, int extra_bytes)
 {
     constexpr bool kCat = WALK == kWalkNcat || WALK == kWalkDcat;
-    const size_t stage_b = kCat ? (P.b_resident ? 2 * kABytes : 2 * kABytes + 2 * BN * kBK * 2)
-                                : (P.b_resident ? kABytes : kABytes + BN * kBK * 2);
-    const size_t smem = 1024 + (size_t)kAccBytes + (size_t)stages * stage_b + (size_t)staging_bytes;
+    const int smem = dyn_smem_bytes(stage_bytes(BN, kCat, P.b_resident), stages, extra_bytes);
     auto kern = conv_tc_kernel<BN, OUT_F32, DEFORM, SPLIT, WALK>;
-    static bool attr_set = false;
-    if (!attr_set) {
+    static int smem_max = -1;                  // dynamic shared memory beside this instantiation's static shared memory
+    if (smem_max < 0) {
         cudaFuncAttributes fa;
         ORP_CUDA(cudaFuncGetAttributes(&fa, kern));
-        ORP_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - (int)fa.sharedSizeBytes));
-        attr_set = true;
+        ORP_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemPerBlock - (int)fa.sharedSizeBytes));
+        smem_max = kSmemPerBlock - (int)fa.sharedSizeBytes;
+    }
+    if (smem > smem_max) {
+        char need[32];
+        snprintf(need, sizeof(need), "%d", smem);
+        return fail(ORP_EINVAL, "conv2d_tc: the plan's %s bytes of dynamic shared memory do not fit beside the static shared memory of %s",
+                    need, __PRETTY_FUNCTION__);
     }
     int slot = -1;
     if (g_timing && g_tc_ev_used < kEvPool) {
@@ -1133,7 +1433,6 @@ int launch_tc(const TcParams &P, int stages, int grid, cudaStream_t st, int stag
                                    BN, P.num_tiles, grid, fl};
     }
     {
-        static const bool pdl = getenv("ORP_TC_NO_PDL") == nullptr;
         cudaLaunchConfig_t cfg;
         memset(&cfg, 0, sizeof(cfg));
         cfg.gridDim = dim3((unsigned)grid);
@@ -1144,7 +1443,7 @@ int launch_tc(const TcParams &P, int stages, int grid, cudaStream_t st, int stag
         at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
         at[0].val.programmaticStreamSerializationAllowed = 1;
         cfg.attrs = at;
-        cfg.numAttrs = pdl ? 1 : 0;
+        cfg.numAttrs = 1;
         ORP_CUDA(cudaLaunchKernelEx(&cfg, kern, P, stages));
     }
     ORP_LAUNCHED();
@@ -1155,127 +1454,132 @@ int launch_tc(const TcParams &P, int stages, int grid, cudaStream_t st, int stag
 // the instantiation that runs a plan: operand type (P.split) and main-loop walk (P.ncat, P.dcat, P.res_mma) are
 // compile-time
 template <int BN, bool OUT_F32, bool DEFORM>
-int launch_plan(const TcParams &P, int stages, int grid, cudaStream_t st, int staging_bytes)
+int launch_plan(const TcParams &P, int stages, int grid, cudaStream_t st, int extra_bytes)
 {
     if constexpr (DEFORM) {
         if (P.dcat != P.split || P.ncat || P.res_mma) return fail(ORP_EINVAL, "conv2d_tc: deformable plan outside dcat == split");
-        return P.split ? launch_tc<BN, OUT_F32, true, true, kWalkDcat>(P, stages, grid, st, staging_bytes)
-                       : launch_tc<BN, OUT_F32, true, false, kWalkK>(P, stages, grid, st, staging_bytes);
+        return P.split ? launch_tc<BN, OUT_F32, true, true, kWalkDcat>(P, stages, grid, st, extra_bytes)
+                       : launch_tc<BN, OUT_F32, true, false, kWalkK>(P, stages, grid, st, extra_bytes);
     } else {
         if (P.ncat && P.res_mma) return fail(ORP_EINVAL, "conv2d_tc: ncat plan with a residual");
         if (P.ncat) {
             if constexpr (!OUT_F32 && BN >= 64 && BN <= 128) {
-                if (P.split) return launch_tc<BN, false, false, true, kWalkNcat>(P, stages, grid, st, staging_bytes);
+                if (P.split) return launch_tc<BN, false, false, true, kWalkNcat>(P, stages, grid, st, extra_bytes);
             }
             return fail(ORP_EINVAL, "conv2d_tc: ncat plan outside f16x3 TMA-epilogue layers with BN 64..128");
         }
         if (P.res_mma) {
             if constexpr (!OUT_F32 && BN >= 64)
-                return P.split ? launch_tc<BN, false, false, true, kWalkKRes>(P, stages, grid, st, staging_bytes)
-                               : launch_tc<BN, false, false, false, kWalkKRes>(P, stages, grid, st, staging_bytes);
+                return P.split ? launch_tc<BN, false, false, true, kWalkKRes>(P, stages, grid, st, extra_bytes)
+                               : launch_tc<BN, false, false, false, kWalkKRes>(P, stages, grid, st, extra_bytes);
             return fail(ORP_EINVAL, "conv2d_tc: residual K blocks outside TMA-epilogue layers with BN >= 64");
         }
-        return P.split ? launch_tc<BN, OUT_F32, false, true, kWalkK>(P, stages, grid, st, staging_bytes)
-                       : launch_tc<BN, OUT_F32, false, false, kWalkK>(P, stages, grid, st, staging_bytes);
+        return P.split ? launch_tc<BN, OUT_F32, false, true, kWalkK>(P, stages, grid, st, extra_bytes)
+                       : launch_tc<BN, OUT_F32, false, false, kWalkK>(P, stages, grid, st, extra_bytes);
     }
 }
 
-}  // namespace
-}  // namespace orp
-
-using namespace orp;
-
-extern "C" int orp_tc_timing_collect(float *total_ms, int *launches, double *flops)
+// the plan's accumulator width as a template argument (the deformable variant is built up to BN = 128)
+template <bool OUT_F32, bool DEFORM>
+int launch_bn(const TcParams &P, const ConvPlan &pl, cudaStream_t st)
 {
-    if (!total_ms || !launches || !flops) return fail(ORP_EINVAL, "orp_tc_timing_collect: null");
-    float sum = 0.f;
-    for (int i = 0; i < g_tc_ev_used; ++i) {
-        float ms = 0.f;
-        ORP_CUDA(cudaEventSynchronize(g_tc_ev[i][1]));
-        ORP_CUDA(cudaEventElapsedTime(&ms, g_tc_ev[i][0], g_tc_ev[i][1]));
-        sum += ms;
-        if (getenv("ORP_TC_TRACE")) {
-            const TcTrace &t = g_tc_trace[i];
-            fprintf(stderr, "tc[%3d] np=%d N=%d %4dx%-4d Cin=%4d Cout=%4d k=%d s=%d dcn=%d BN=%3d tiles=%5d grid=%3d  %8.1f us  %7.1f TFLOP/s\n",
-                    i, t.nprob, t.N, t.H, t.W, t.Cin, t.Cout, t.K, t.stride, t.deform, t.BN, t.tiles, t.grid, ms * 1e3,
-                    t.flops / (ms * 1e-3) / 1e12);
-        }
+    const int s = pl.rep.stages, g = pl.rep.grid, e = pl.extra_bytes;
+    switch (pl.rep.BN) {
+    case 256:
+        if constexpr (!DEFORM) return launch_plan<256, OUT_F32, false>(P, s, g, st, e);
+        break;
+    case 128: return launch_plan<128, OUT_F32, DEFORM>(P, s, g, st, e);
+    case 64: return launch_plan<64, OUT_F32, DEFORM>(P, s, g, st, e);
+    case 32: return launch_plan<32, OUT_F32, DEFORM>(P, s, g, st, e);
     }
-    *total_ms = sum; *launches = g_tc_ev_used; *flops = g_tc_flops;
-    g_tc_ev_used = 0; g_tc_flops = 0.0;
+    return fail(ORP_EINVAL, "conv2d_tc: unsupported tile width");
+}
+
+// multiprocessors of the current device, looked up once per device
+int device_sms(int &sms)
+{
+    static thread_local int dev_known = -1, sms_known = 0;
+    int dev = 0;
+    ORP_CUDA(cudaGetDevice(&dev));
+    if (dev != dev_known) {
+        ORP_CUDA(cudaDeviceGetAttribute(&sms_known, cudaDevAttrMultiProcessorCount, dev));
+        dev_known = dev;
+    }
+    sms = sms_known;
     return ORP_OK;
 }
 
-/* see include/orp_b200.h */
-extern "C" int orp_tc_last_plan(orp_tc_plan *out)
+// One tensor-core convolution: plan, parameter block and tensor maps, the launch, then the GroupNorm statistics the epilogue
+// could not fuse.
+int conv2d_tc(const ConvDesc &d, void *stream)
 {
-    if (!out) return fail(ORP_EINVAL, "orp_tc_last_plan: null");
-    if (!g_tc_plan_set) return fail(ORP_EINVAL, "orp_tc_last_plan: no tensor-core convolution launched on this thread");
-    *out = g_tc_plan;
+    int rc = check_conv(d);                    // argument errors come before any device work
+    if (rc) return rc;
+    rc = ensure_device();
+    if (rc) return rc;
+    int sms = 0;
+    rc = device_sms(sms);
+    if (rc) return rc;
+    ConvPlan pl;
+    rc = plan_conv(d, sms, pl);
+    if (rc) return rc;
+    TcParams P;
+    rc = make_params(d, pl, P);
+    if (rc) return rc;
+    rc = encode_maps(d, pl, P);
+    if (rc) return rc;
+    g_tc_plan = pl.rep;
+    g_tc_plan_set = true;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    rc = d.out_f32 ? (d.deform ? launch_bn<true, true>(P, pl, st) : launch_bn<true, false>(P, pl, st))
+                   : (d.deform ? launch_bn<false, true>(P, pl, st) : launch_bn<false, false>(P, pl, st));
+    if (rc) return rc;
+    bool want_gn = false;
+    for (int i = 0; i < d.nprob; ++i) want_gn = want_gn || (d.probs[i].gn_stats != nullptr);
+    if (want_gn && !P.gn_fused) {
+        // statistics requested but not fusable for this shape: separate pass over the bf16 output
+        if (d.out_f32 || d.Cout != 256) return fail(ORP_EINVAL, "conv2d_tc: gn_stats needs a 16-bit output with 256 channels");
+        for (int i = 0; i < d.nprob; ++i)
+            if (d.probs[i].gn_stats) {
+                int r2 = d.split ? orp_gn_stats_f16x3(P.prob[i].out, P.prob[i].N, P.prob[i].Ho * P.prob[i].Wo, 256, 32, d.probs[i].gn_stats, stream)
+                                 : orp_gn_stats_bf16(P.prob[i].out, P.prob[i].N, P.prob[i].Ho * P.prob[i].Wo, 256, 32, d.probs[i].gn_stats, stream);
+                if (r2) return r2;
+            }
+    }
     return ORP_OK;
 }
 
-// stem: 0, or 2 for conv1 in space-to-depth form (the value orp_tc_plan.stem reports)
-static int conv2d_bf16_impl(int nprob, const orp_tc_problem *probs, const void *w, int Cout, int Cout_padded, int KH,
-                            int KW, int Cin, int stride, int pad, const float *bias, int relu, int out_f32,
-                            int deform, int stem, void *stream, int split = 0, int wscale_log2 = 0, int ksplit = 1);
-
-/* see include/orp_b200.h */
-extern "C" int orp_conv2d_bf16(int nprob, const orp_tc_problem *probs, const void *w, int Cout, int Cout_padded, int KH,
-                               int KW, int Cin, int stride, int pad, const float *bias, int relu, int out_f32,
-                               int deform, void *stream)
+// conv1 in space-to-depth form over N images of H x W: 4 x 1 taps over the rows of the [N, H/2+3, W/2+3, 16] input, each row
+// read as W/2 "pixels" of 64 virtual channels (4 horizontally adjacent pixels), stride 1, no padding
+int stem_desc(const void *x_s2d, int N, int H, int W, const void *w, const float *bias, int relu, void *out, int split,
+              int wscale_log2, orp_tc_problem &q, ConvDesc &d)
 {
-    return conv2d_bf16_impl(nprob, probs, w, Cout, Cout_padded, KH, KW, Cin, stride, pad, bias, relu, out_f32, deform, 0, stream);
-}
-
-/* see include/orp_b200.h */
-extern "C" int orp_conv2d_f16x3(int nprob, const orp_tc_problem *probs, const void *w_split, int Cout, int Cout_padded, int KH,
-                                int KW, int Cin, int stride, int pad, const float *bias, int wscale_log2, int relu,
-                                int out_f32, int deform, void *stream)
-{
-    if (wscale_log2 < 0 || wscale_log2 > 15) return fail(ORP_EINVAL, "conv2d_f16x3: weight scale exponent must be in 0..15");
-    return conv2d_bf16_impl(nprob, probs, w_split, Cout, Cout_padded, KH, KW, Cin, stride, pad, bias, relu, out_f32, deform, 0,
-                            stream, 1, wscale_log2);
-}
-
-extern "C" int orp_stem_conv_s2d_f16x3(const void *x_s2d, int N, int H, int W, const void *w_split, const float *bias,
-                                       int wscale_log2, int relu, void *out, void *stream)
-{
-    if (!x_s2d || !w_split || !out || N < 1 || H < 2 || W < 2 || (H & 1) || (W & 1))
-        return fail(ORP_EINVAL, "stem_conv_s2d_f16x3: needs even H, W");
-    if (wscale_log2 < 0 || wscale_log2 > 15) return fail(ORP_EINVAL, "stem_conv_s2d_f16x3: weight scale exponent must be in 0..15");
-    orp_tc_problem q;
+    if (!x_s2d || !w || !out || N < 1 || H < 2 || W < 2 || (H & 1) || (W & 1))
+        return fail(ORP_EINVAL, "stem_conv_s2d_%s: needs even H, W", split ? "f16x3" : "bf16");
+    if (split && (wscale_log2 < 0 || wscale_log2 > 15)) return fail(ORP_EINVAL, "stem_conv_s2d_f16x3: weight scale exponent must be in 0..15");
     memset(&q, 0, sizeof(q));
     q.x = x_s2d;
     q.N = N; q.H = H / 2 + 3; q.W = W / 2; q.out = out;
-    return conv2d_bf16_impl(1, &q, w_split, 64, 64, 4, 1, 64, 1, 0, bias, relu, 0, 0, 2, stream, 1, wscale_log2);
-}
-
-extern "C" int orp_f16x3_overflow_count(unsigned int *count, int reset)
-{
-    if (!count) return fail(ORP_EINVAL, "f16x3_overflow_count: null");
-    ORP_CUDA(cudaMemcpyFromSymbol(count, g_f16_overflow, sizeof(unsigned int)));
-    if (reset) {
-        const unsigned int z = 0;
-        ORP_CUDA(cudaMemcpyToSymbol(g_f16_overflow, &z, sizeof(z)));
-    }
+    d = ConvDesc{1, &q, w, 64, 64, 4, 1, 64, 1, 0, bias, relu, 0, 0, split, split ? wscale_log2 : 0, 2, 1};
     return ORP_OK;
 }
 
-extern "C" int orp_stem_conv_s2d_bf16(const void *x_s2d, int N, int H, int W, const void *w256, const float *bias, int relu,
-                                      void *out, void *stream)
+// the launch inside orp_conv2d_tc_splitk: fp32 partial sums into the workspace, no bias, no activation, no statistics
+int splitk_desc(const orp_tc_problem *prob, const void *w, int Cout, int Cout_padded, int KH, int KW, int Cin, int stride, int pad,
+                int f16x3, int wscale_log2, int ksplit, void *workspace, orp_tc_problem &q, ConvDesc &d, int &Ho, int &Wo)
 {
-    if (!x_s2d || !w256 || !out || N < 1 || H < 2 || W < 2 || (H & 1) || (W & 1))
-        return fail(ORP_EINVAL, "stem_conv_s2d_bf16: needs even H, W");
-    orp_tc_problem q;
-    memset(&q, 0, sizeof(q));
-    q.x = x_s2d;
-    q.N = N; q.H = H / 2 + 3; q.W = W / 2; q.out = out;     // 4 x 1 taps over rows, 64 virtual channels, no padding
-    return conv2d_bf16_impl(1, &q, w256, 64, 64, 4, 1, 64, 1, 0, bias, relu, 0, 0, 2, stream);
+    if (!prob || !w || !workspace || ksplit < 2 || (Cout % 8)) return fail(ORP_EINVAL, "conv2d_tc_splitk: bad arguments");
+    if (f16x3 && (wscale_log2 < 0 || wscale_log2 > 15)) return fail(ORP_EINVAL, "conv2d_tc_splitk: weight scale exponent must be in 0..15");
+    Ho = (prob->H + 2 * pad - (KH - 1) - 1) / stride + 1;
+    Wo = (prob->W + 2 * pad - (KW - 1) - 1) / stride + 1;
+    if (Ho <= 0 || Wo <= 0) return fail(ORP_EINVAL, "conv2d_tc_splitk: bad problem");
+    q = *prob;                                  // every (pixel, channel, split) element of the workspace is written
+    q.out = workspace;
+    q.gn_stats = nullptr;
+    d = ConvDesc{1, &q, w, Cout, Cout_padded, KH, KW, Cin, stride, pad, nullptr, 0, 1, 0, f16x3 ? 1 : 0, wscale_log2, 0, ksplit};
+    return ORP_OK;
 }
 
-namespace orp {
-namespace {
 // split-K finish: fp32 sums [pixels, C] -> + bias -> ReLU -> bf16 [pixels, C] or split fp16 [pixels, 2, C]
 __global__ void __launch_bounds__(256)
 splitk_finish_kernel(const float *__restrict__ ws, int ksplit, size_t pixels, int C, const float *__restrict__ bias, int relu, int split,
@@ -1326,23 +1630,129 @@ splitk_finish_kernel(const float *__restrict__ ws, int ksplit, size_t pixels, in
 }  // namespace
 }  // namespace orp
 
+using namespace orp;
+
+extern "C" int orp_tc_timing_collect(float *total_ms, int *launches, double *flops)
+{
+    if (!total_ms || !launches || !flops) return fail(ORP_EINVAL, "orp_tc_timing_collect: null");
+    float sum = 0.f;
+    for (int i = 0; i < g_tc_ev_used; ++i) {
+        float ms = 0.f;
+        ORP_CUDA(cudaEventSynchronize(g_tc_ev[i][1]));
+        ORP_CUDA(cudaEventElapsedTime(&ms, g_tc_ev[i][0], g_tc_ev[i][1]));
+        sum += ms;
+        if (getenv("ORP_TC_TRACE")) {
+            const TcTrace &t = g_tc_trace[i];
+            fprintf(stderr, "tc[%3d] np=%d N=%d %4dx%-4d Cin=%4d Cout=%4d k=%d s=%d dcn=%d BN=%3d tiles=%5d grid=%3d  %8.1f us  %7.1f TFLOP/s\n",
+                    i, t.nprob, t.N, t.H, t.W, t.Cin, t.Cout, t.K, t.stride, t.deform, t.BN, t.tiles, t.grid, ms * 1e3,
+                    t.flops / (ms * 1e-3) / 1e12);
+        }
+    }
+    *total_ms = sum; *launches = g_tc_ev_used; *flops = g_tc_flops;
+    g_tc_ev_used = 0; g_tc_flops = 0.0;
+    return ORP_OK;
+}
+
+/* see include/orp_b200.h */
+extern "C" int orp_tc_last_plan(orp_tc_plan *out)
+{
+    if (!out) return fail(ORP_EINVAL, "orp_tc_last_plan: null");
+    if (!g_tc_plan_set) return fail(ORP_EINVAL, "orp_tc_last_plan: no tensor-core convolution launched on this thread");
+    *out = g_tc_plan;
+    return ORP_OK;
+}
+
+/* see include/orp_b200.h */
+extern "C" int orp_tc_plan_conv(int nprob, const orp_tc_problem *probs, const void *w, int Cout, int Cout_padded, int KH, int KW,
+                                int Cin, int stride, int pad, const float *bias, int wscale_log2, int relu, int out_f32, int deform,
+                                int split, int stem, int ksplit, int sms, orp_tc_plan *out)
+{
+    if (!out || sms < 1 || (stem != 0 && stem != 2)) return fail(ORP_EINVAL, "orp_tc_plan_conv: bad arguments");
+    split = split ? 1 : 0;
+    orp_tc_problem q;
+    ConvDesc d;
+    int rc = ORP_OK;
+    if (stem == 2 || ksplit > 1) {
+        // one problem: the stem's carries the image's N, H, W; split-K's output stands in for the workspace
+        if (nprob != 1 || !probs || deform || out_f32 || (stem == 2 && ksplit > 1))
+            return fail(ORP_EINVAL, "orp_tc_plan_conv: the stem and split-K plan one problem with a 16-bit output");
+        int Ho, Wo;
+        rc = stem == 2 ? stem_desc(probs->x, probs->N, probs->H, probs->W, w, bias, relu, probs->out, split, wscale_log2, q, d)
+                       : splitk_desc(probs, w, Cout, Cout_padded, KH, KW, Cin, stride, pad, split, wscale_log2, ksplit, probs->out, q,
+                                     d, Ho, Wo);
+    } else {
+        d = ConvDesc{nprob, probs, w, Cout, Cout_padded, KH, KW, Cin, stride, pad, bias, relu, out_f32, deform, split, wscale_log2, 0, 1};
+    }
+    if (rc) return rc;
+    ConvPlan pl;
+    rc = plan_conv(d, sms, pl);
+    if (rc) return rc;
+    *out = pl.rep;
+    return ORP_OK;
+}
+
+/* see include/orp_b200.h */
+extern "C" int orp_conv2d_bf16(int nprob, const orp_tc_problem *probs, const void *w, int Cout, int Cout_padded, int KH,
+                               int KW, int Cin, int stride, int pad, const float *bias, int relu, int out_f32,
+                               int deform, void *stream)
+{
+    return conv2d_tc(ConvDesc{nprob, probs, w, Cout, Cout_padded, KH, KW, Cin, stride, pad, bias, relu, out_f32, deform, 0, 0, 0, 1},
+                     stream);
+}
+
+/* see include/orp_b200.h */
+extern "C" int orp_conv2d_f16x3(int nprob, const orp_tc_problem *probs, const void *w_split, int Cout, int Cout_padded, int KH,
+                                int KW, int Cin, int stride, int pad, const float *bias, int wscale_log2, int relu,
+                                int out_f32, int deform, void *stream)
+{
+    return conv2d_tc(ConvDesc{nprob, probs, w_split, Cout, Cout_padded, KH, KW, Cin, stride, pad, bias, relu, out_f32, deform, 1,
+                              wscale_log2, 0, 1},
+                     stream);
+}
+
+extern "C" int orp_stem_conv_s2d_f16x3(const void *x_s2d, int N, int H, int W, const void *w_split, const float *bias,
+                                       int wscale_log2, int relu, void *out, void *stream)
+{
+    orp_tc_problem q;
+    ConvDesc d;
+    const int rc = stem_desc(x_s2d, N, H, W, w_split, bias, relu, out, 1, wscale_log2, q, d);
+    return rc ? rc : conv2d_tc(d, stream);
+}
+
+extern "C" int orp_stem_conv_s2d_bf16(const void *x_s2d, int N, int H, int W, const void *w256, const float *bias, int relu,
+                                      void *out, void *stream)
+{
+    orp_tc_problem q;
+    ConvDesc d;
+    const int rc = stem_desc(x_s2d, N, H, W, w256, bias, relu, out, 0, 0, q, d);
+    return rc ? rc : conv2d_tc(d, stream);
+}
+
+extern "C" int orp_f16x3_overflow_count(unsigned int *count, int reset)
+{
+    if (!count) return fail(ORP_EINVAL, "f16x3_overflow_count: null");
+    ORP_CUDA(cudaMemcpyFromSymbol(count, g_f16_overflow, sizeof(unsigned int)));
+    if (reset) {
+        const unsigned int z = 0;
+        ORP_CUDA(cudaMemcpyToSymbol(g_f16_overflow, &z, sizeof(z)));
+    }
+    return ORP_OK;
+}
+
 /* see include/orp_b200.h */
 extern "C" int orp_conv2d_tc_splitk(const orp_tc_problem *prob, const void *w, int Cout, int Cout_padded, int KH, int KW, int Cin,
                                     int stride, int pad, const float *bias, int f16x3, int wscale_log2, int relu, int ksplit,
                                     float *workspace, void *stream)
 {
-    if (!prob || !w || !workspace || ksplit < 2 || (Cout % 8)) return fail(ORP_EINVAL, "conv2d_tc_splitk: bad arguments");
-    if (f16x3 && (wscale_log2 < 0 || wscale_log2 > 15)) return fail(ORP_EINVAL, "conv2d_tc_splitk: weight scale exponent must be in 0..15");
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const int Ho = (prob->H + 2 * pad - (KH - 1) - 1) / stride + 1, Wo = (prob->W + 2 * pad - (KW - 1) - 1) / stride + 1;
-    if (Ho <= 0 || Wo <= 0) return fail(ORP_EINVAL, "conv2d_tc_splitk: bad problem");
-    const size_t pixels = (size_t)prob->N * Ho * Wo;
-    orp_tc_problem q = *prob;                                  // every (pixel, channel, split) element of the workspace is written
-    q.out = workspace;
-    q.gn_stats = nullptr;
-    int rc = conv2d_bf16_impl(1, &q, w, Cout, Cout_padded, KH, KW, Cin, stride, pad, nullptr, 0, 1, 0, 0, stream, f16x3 ? 1 : 0,
-                              wscale_log2, ksplit);
+    orp_tc_problem q;
+    ConvDesc d;
+    int Ho = 0, Wo = 0;
+    int rc = splitk_desc(prob, w, Cout, Cout_padded, KH, KW, Cin, stride, pad, f16x3, wscale_log2, ksplit, workspace, q, d, Ho, Wo);
     if (rc) return rc;
+    rc = conv2d_tc(d, stream);
+    if (rc) return rc;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const size_t pixels = (size_t)prob->N * Ho * Wo;
     void *ovf = nullptr;
     ORP_CUDA(cudaGetSymbolAddress(&ovf, g_f16_overflow));
     splitk_finish_kernel<<<grid_for(pixels * (Cout / 8), 256), 256, 0, st>>>(workspace, ksplit, pixels, Cout, bias, relu, f16x3 ? 1 : 0, prob->out,
@@ -1352,269 +1762,6 @@ extern "C" int orp_conv2d_tc_splitk(const orp_tc_problem *prob, const void *w, i
         if (Cout != 256) return fail(ORP_EINVAL, "conv2d_tc_splitk: gn_stats needs 256 output channels");
         return f16x3 ? orp_gn_stats_f16x3(prob->out, prob->N, Ho * Wo, 256, 32, prob->gn_stats, stream)
                      : orp_gn_stats_bf16(prob->out, prob->N, Ho * Wo, 256, 32, prob->gn_stats, stream);
-    }
-    return ORP_OK;
-}
-
-static int conv2d_bf16_impl(int nprob, const orp_tc_problem *probs, const void *w, int Cout, int Cout_padded, int KH,
-                            int KW, int Cin, int stride, int pad, const float *bias, int relu, int out_f32,
-                            int deform, int stem, void *stream, int split, int wscale_log2, int ksplit)
-{
-    if (nprob < 1 || nprob > kMaxProb || !probs || !w) return fail(ORP_EINVAL, "conv2d_tc: bad arguments");
-    if (Cin % 8) return fail(ORP_EINVAL, "conv2d_tc: Cin must be a multiple of 8 (16-byte channel rows)");
-    if (deform && (Cin % kBK)) return fail(ORP_EINVAL, "conv2d_tc: deformable conv needs Cin % 64 == 0");
-    if (Cout_padded % 32 || Cout_padded < Cout) return fail(ORP_EINVAL, "conv2d_tc: padded Cout must be a multiple of 32");
-    // a tile spans BW * stride <= 256 input columns (the TMA box limit) with BW >= 1
-    if (stride < 1 || stride > 256) return fail(ORP_EINVAL, "conv2d_tc: stride must be in 1..256");
-    // the deformable producers address the input with 32-bit element offsets (img0, s_o): N*H*W*Cin*planes must stay below 2^31
-    if (deform)
-        for (int i = 0; i < nprob; ++i)
-            if ((long long)probs[i].N * probs[i].H * probs[i].W * Cin * (split ? 2 : 1) >= (1LL << 31))
-                return fail(ORP_EINVAL, "conv2d_tc: deformable input has 2^31 or more 16-bit elements (32-bit sample offsets)");
-    if (ksplit < 1) ksplit = 1;
-    if (ksplit > 1 && (nprob != 1 || deform || stem || !out_f32 || (KH * KW) % ksplit || probs[0].residual_bf16 || probs[0].residual_f32 || bias || relu))
-        return fail(ORP_EINVAL, "conv2d_tc: split-K serves one plain problem with an fp32 partial-sum output and taps % ksplit == 0");
-    int rc = ensure_device();
-    if (rc) return rc;
-    EncodeTiledFn enc = encode_fn();
-    if (!enc) return fail(ORP_ECUDA, "conv2d_tc: cuTensorMapEncodeTiled unavailable");
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const CUtensorMapDataType dt16 = split ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
-    const int T = split ? 2 : 1;             // 16-bit planes per value (hi, lo)
-
-    int BN = 256;
-    if (Cout_padded % 256) BN = (Cout_padded % 128 == 0) ? 128 : (Cout_padded % 64 == 0) ? 64 : 32;
-    {
-        // narrower accumulators when the 128 x BN tiling would leave SMs idle
-        long long mtiles = 0;
-        for (int i = 0; i < nprob; ++i) {
-            const int ho = (probs[i].H + 2 * pad - (KH - 1) - 1) / stride + 1, wo = (probs[i].W + 2 * pad - (KW - 1) - 1) / stride + 1;
-            mtiles += ((long long)probs[i].N * ho * wo + 127) / 128;
-        }
-        while (BN > 64 && mtiles * (Cout_padded / BN) * ksplit < 120) BN /= 2;
-    }
-    // the deformable variant's 512 threads leave 128 registers each: a 64 x 128 fp32 accumulator fragment (64 per thread)
-    // fits beside the epilogue, a 64 x 256 one does not
-    if (deform && BN > 128) BN = 128;
-    TcParams P;
-    memset(&P, 0, sizeof(P));
-    // a partial last channel block is zero-filled by TMA (A operand) and by the weight layout (B operand)
-    P.nprob = nprob; P.KH = KH; P.KW = KW; P.Cin = Cin; P.cin_blocks = (Cin + kBK - 1) / kBK;
-    P.stride = stride; P.pad = pad;
-    P.Cout = Cout; P.relu = relu; P.bias = bias; P.s2d_stem = (stem == 2) ? 1 : 0;
-    P.split = split ? 1 : 0;
-    P.oscale = split ? ldexpf(1.f, -wscale_log2) : 1.f;
-    {
-        void *ovf = nullptr;
-        ORP_CUDA(cudaGetSymbolAddress(&ovf, g_f16_overflow));
-        P.ovf = static_cast<unsigned int *>(ovf);
-    }
-    P.n_tiles_n = Cout_padded / BN;
-    P.fd_ntn.set((uint32_t)P.n_tiles_n);
-    int mt = 0;
-    for (int i = 0; i < nprob; ++i) {
-        const orp_tc_problem &q = probs[i];
-        Problem &pr = P.prob[i];
-        pr.N = q.N; pr.H = q.H; pr.W = q.W;
-        pr.Ho = (q.H + 2 * pad - (KH - 1) - 1) / stride + 1;
-        pr.Wo = (q.W + 2 * pad - (KW - 1) - 1) / stride + 1;
-        if (pr.Ho <= 0 || pr.Wo <= 0 || !q.x || !q.out) return fail(ORP_EINVAL, "conv2d_tc: bad problem");
-        pr.BW = pow2_floor(pr.Wo < 128 ? pr.Wo : 128);
-        // the TMA box spans BW * stride columns (<= 256); BW stays a power of two, as the row decode (& (BW - 1), lbw) needs
-        if (stride * pr.BW > 256) pr.BW = pow2_floor(256 / stride);
-        // (measured: 16 x 8 pixel tiles for the deformable variant change nothing - 1361 vs 1334 us per f16x3 launch, and neither
-        // does the spread of the offsets: the gather runs at the ~47 GB/s per SM L2 -> SM ceiling whatever its locality)
-        if (deform && pr.BW > 16 && getenv("ORP_TC_DCN_2DTILES")) pr.BW = 16;
-        pr.BH = pow2_floor(pr.Ho < 128 / pr.BW ? pr.Ho : 128 / pr.BW);
-        pr.BI = 128 / (pr.BW * pr.BH);
-        pr.lbw = 0; while ((1 << pr.lbw) < pr.BW) ++pr.lbw;
-        pr.lbh = 0; while ((1 << pr.lbh) < pr.BH) ++pr.lbh;
-        pr.tiles_w = ceil_div(pr.Wo, pr.BW); pr.tiles_h = ceil_div(pr.Ho, pr.BH); pr.tiles_i = ceil_div(pr.N, pr.BI);
-        pr.tile_start = mt;
-        pr.fd_tw.set((uint32_t)pr.tiles_w); pr.fd_th.set((uint32_t)pr.tiles_h);
-        mt += pr.tiles_w * pr.tiles_h * pr.tiles_i;
-        pr.out = q.out; pr.res = static_cast<const __nv_bfloat16 *>(q.residual_bf16); pr.res32 = q.residual_f32;
-        pr.x = static_cast<const __nv_bfloat16 *>(q.x); pr.offset = q.offset; pr.gn_stats = q.gn_stats; pr.mask = q.mask;
-        if (deform && !q.offset) return fail(ORP_EINVAL, "conv2d_tc: deformable conv needs offsets");
-        if (!deform) {
-            // 5-D view {channel, plane (hi / lo), w, h, image}; bf16 tensors have a single plane.  Split activations are
-            // [N,H,W,2,C]: the lo plane of a pixel follows its hi plane.
-            cuuint64_t gdim[5] = {(cuuint64_t)Cin, (cuuint64_t)T, (cuuint64_t)q.W, (cuuint64_t)q.H, (cuuint64_t)q.N};
-            cuuint64_t gstr[4] = {(cuuint64_t)Cin * 2, (cuuint64_t)Cin * 2 * T, (cuuint64_t)q.W * Cin * 2 * T,
-                                  (cuuint64_t)q.H * q.W * Cin * 2 * T};
-            if (stem == 2) {
-                // space-to-depth stem: the tensor is [T][N, H, W + 3, 16] (planes outermost); a 64-element "pixel" row of
-                // the GEMM is the 4 horizontally adjacent 16-channel pixels starting at w, so consecutive w overlap
-                // (stride 32 bytes)
-                gstr[0] = (cuuint64_t)q.N * q.H * (q.W + 3) * 32;
-                gstr[1] = 32;
-                gstr[2] = (cuuint64_t)(q.W + 3) * 32;
-                gstr[3] = (cuuint64_t)q.H * (q.W + 3) * 32;
-            }
-            cuuint32_t box[5] = {(cuuint32_t)kBK, 1u, (cuuint32_t)(pr.BW * stride), (cuuint32_t)(pr.BH * stride), (cuuint32_t)pr.BI};
-            cuuint32_t estr[5] = {1, 1, (cuuint32_t)stride, (cuuint32_t)stride, 1};
-            CUresult r = enc(&P.tmA[i], dt16, 5, const_cast<void *>(q.x), gdim, gstr, box, estr,
-                             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-            if (r != CUDA_SUCCESS) return fail(ORP_ECUDA, "conv2d_tc: cuTensorMapEncodeTiled(A) failed");
-        }
-    }
-    {
-        // weights [Cout_padded][tap][cin_blocks][T][64] (zero padded per tap; T = 2: the hi block, then the lo block)
-        const cuuint64_t K = (cuuint64_t)KH * KW * T * P.cin_blocks * kBK;
-        cuuint64_t gdim[2] = {K, (cuuint64_t)Cout_padded};
-        cuuint64_t gstr[1] = {K * 2};
-        cuuint32_t box[2] = {(cuuint32_t)kBK, (cuuint32_t)BN};
-        cuuint32_t estr[2] = {1, 1};
-        CUresult r = enc(&P.tmB, dt16, 2, const_cast<void *>(w), gdim, gstr, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) return fail(ORP_ECUDA, "conv2d_tc: cuTensorMapEncodeTiled(B) failed");
-    }
-    P.num_m_tiles = mt;
-    P.num_tiles = mt * P.n_tiles_n * ksplit;
-    P.ksplit = ksplit;
-    P.fd_ks.set((uint32_t)ksplit);
-    P.ks_stride = (long long)P.prob[0].N * P.prob[0].Ho * P.prob[0].Wo * Cout;
-    // TMA epilogue: 16-bit outputs whose channel count is a multiple of 64
-    bool any_res = false;
-    for (int i = 0; i < nprob; ++i) any_res = any_res || (probs[i].residual_bf16 != nullptr);
-    // (f16x3 also takes channel counts that are only a multiple of 8 - Swin's 96 / 288: the TMA unit clips the last box)
-    P.tma_epi = (!out_f32 && ((Cout % 64 == 0) || (split && Cout % 8 == 0)) && BN >= 64) ? 1 : 0;
-    if (getenv("ORP_TC_NO_TMA_EPI") && !split) P.tma_epi = 0;
-    if (split && !out_f32 && !P.tma_epi) return fail(ORP_EINVAL, "conv2d_f16x3: 16-bit outputs need Cout % 8 == 0 and weights padded to a multiple of 64 rows");
-    if (split && out_f32 && any_res) return fail(ORP_EINVAL, "conv2d_f16x3: fp32 outputs take an fp32 residual only");
-    // GroupNorm statistics: fused into the TMA epilogue when every warp's 32 rows lie in one image
-    bool want_gn = false, gn_ok = (P.tma_epi != 0) && Cout == 256 && !bias && !relu;
-    for (int i = 0; i < nprob; ++i) {
-        want_gn = want_gn || (probs[i].gn_stats != nullptr);
-        if (P.prob[i].BW * P.prob[i].BH < 32) gn_ok = false;
-    }
-    P.gn_fused = (want_gn && gn_ok) ? 1 : 0;
-    const bool mem_bound = any_res || (KH * KW * (Cin / kBK) <= 8);
-    P.epi_bufs = mem_bound ? 2 : 1;          // a second staging tile costs compute-bound layers a main-loop stage
-    if (const char *e = getenv("ORP_TC_EPI_BUFS")) P.epi_bufs = atoi(e) == 1 ? 1 : 2;
-    P.epi_merge = (split && P.tma_epi && (mem_bound || stem == 2) && !getenv("ORP_TC_NO_MERGE")) ? 1 : 0;
-    // terms concatenated along N for narrow layers (kernel header); the residual / deformable / fp32-output variants keep
-    // the K-concatenated walk
-    P.dcat = (split && deform) ? 1 : 0;
-    P.ncat = (split && P.tma_epi && BN <= 128 && !deform && !any_res && !getenv("ORP_TC_NO_NCAT")) ? 1 : 0;
-    // residual through the tensor core (TMA epilogue only; the staged epilogue adds it itself)
-    P.res_mma = (P.tma_epi && any_res) ? 1 : 0;
-    if (P.res_mma) {
-        if (deform) return fail(ORP_EINVAL, "conv2d_tc: residual is not supported on the deformable path");
-        for (int i = 0; i < nprob; ++i)
-            if (!probs[i].residual_bf16) return fail(ORP_EINVAL, "conv2d_tc: residual must be given for every problem or none");
-        void *ident_ptr = nullptr;
-        if (split) {
-            ORP_CUDA(cudaGetSymbolAddress(&ident_ptr, g_ident16));
-            ident_ptr = static_cast<char *>(ident_ptr) + (size_t)wscale_log2 * 8192;
-        } else {
-            ORP_CUDA(cudaGetSymbolAddress(&ident_ptr, g_ident));
-        }
-        cuuint64_t gdim[2] = {64, 64};
-        cuuint64_t gstr[1] = {128};
-        cuuint32_t box[2] = {64, 64};
-        cuuint32_t estr[2] = {1, 1};
-        CUresult r = enc(&P.tmI, dt16, 2, ident_ptr, gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                         CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) return fail(ORP_ECUDA, "conv2d_tc: cuTensorMapEncodeTiled(identity) failed");
-    }
-    // layers whose whole weight slab for one N tile is <= 72 KiB keep it resident; stages then carry only the A tile
-    P.b_resident = (!deform && ksplit == 1 && KH * KW * T * P.cin_blocks * BN * kBK * 2 <= 72 * 1024 && !getenv("ORP_TC_NO_BRES")) ? 1 : 0;
-    if (P.tma_epi) {
-        for (int i = 0; i < nprob; ++i) {
-            const Problem &pr = P.prob[i];
-            cuuint64_t gdim[5] = {(cuuint64_t)Cout, (cuuint64_t)T, (cuuint64_t)pr.Wo, (cuuint64_t)pr.Ho, (cuuint64_t)pr.N};
-            cuuint64_t gstr[4] = {(cuuint64_t)Cout * 2, (cuuint64_t)Cout * 2 * T, (cuuint64_t)pr.Wo * Cout * 2 * T,
-                                  (cuuint64_t)pr.Ho * pr.Wo * Cout * 2 * T};
-            cuuint32_t box[5] = {64u, 1u, (cuuint32_t)pr.BW, (cuuint32_t)pr.BH, (cuuint32_t)pr.BI};
-            cuuint32_t estr[5] = {1, 1, 1, 1, 1};
-            CUresult r = enc(&P.tmOut[i], dt16, 5, pr.out, gdim, gstr, box, estr,
-                             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
-                             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-            if (r != CUDA_SUCCESS) return fail(ORP_ECUDA, "conv2d_tc: cuTensorMapEncodeTiled(out) failed");
-            if (pr.res) {
-                r = enc(&P.tmRes[i], dt16, 5, const_cast<__nv_bfloat16 *>(pr.res), gdim, gstr, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-                if (r != CUDA_SUCCESS) return fail(ORP_ECUDA, "conv2d_tc: cuTensorMapEncodeTiled(residual) failed");
-            }
-        }
-    }
-    int sms = kNumSMs;
-    {
-        int dev = 0;
-        ORP_CUDA(cudaGetDevice(&dev));
-        ORP_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    }
-    int grid = P.num_tiles < sms ? P.num_tiles : sms;
-    if (P.b_resident && grid >= P.n_tiles_n) grid -= grid % P.n_tiles_n;       // fixed N tile per CTA
-    else if (P.b_resident) P.b_resident = 0;
-    // shared-memory budget: staged accumulator pass + output staging + resident weights + main-loop stages.  When the extras
-    // leave fewer than three stages they are given up in order of least value: the second staging slot, the resident slab.
-    int stage_bytes = 0, bres_bytes = 0, staging = 0, stages = 0;
-    for (;;) {
-        stage_bytes = (P.ncat || P.dcat) ? (P.b_resident ? 2 * kABytes : 2 * kABytes + 2 * BN * kBK * 2)
-                                         : (P.b_resident ? kABytes : kABytes + BN * kBK * 2);
-        bres_bytes = (P.b_resident ? KH * KW * T * P.cin_blocks * BN * kBK * 2 : 0) + (P.res_mma ? 8192 : 0);
-        const int hc = BN < 64 ? BN : 64;
-        staging = out_f32 ? 0 : 128 * (hc * 2 + 16);
-        if (P.tma_epi) staging = P.epi_bufs * (P.epi_merge ? 32768 : 16384);
-        stages = (int)((227 * 1024 - (deform ? 14336 : 4096) - 1024 - kAccBytes - staging - bres_bytes) / stage_bytes);   // static shared memory of the variant
-        if (stages >= 3) break;
-        if (P.epi_bufs == 2) { P.epi_bufs = 1; continue; }
-        if (P.b_resident) { P.b_resident = 0; continue; }
-        if (stages >= 2) break;
-        return fail(ORP_EINVAL, "conv2d_tc: shared-memory budget cannot hold two main-loop stages");
-    }
-    if (stages > kStagesMax) stages = kStagesMax;
-    if (const char *e = getenv("ORP_TC_STAGES")) { const int v = atoi(e); if (v >= 2 && v < stages) stages = v; }   // experiments
-    if (deform && stages > 3) stages = 3;     // leave L1 capacity for the bilinear gather (corner reuse between neighbouring pixels)
-    {
-        // the plan as launched, for orp_tc_last_plan
-        orp_tc_plan &pl = g_tc_plan;
-        memset(&pl, 0, sizeof(pl));
-        pl.BN = BN; pl.stages = stages; pl.grid = grid; pl.num_tiles = P.num_tiles; pl.n_tiles_n = P.n_tiles_n;
-        pl.ksplit = ksplit; pl.nprob = nprob; pl.Cout = Cout; pl.Cout_padded = Cout_padded;
-        pl.split = P.split; pl.deform = deform ? 1 : 0; pl.out_f32 = out_f32 ? 1 : 0; pl.stem = stem; pl.relu = relu;
-        pl.bias = bias ? 1 : 0;
-        for (int i = 0; i < nprob; ++i) {
-            if (probs[i].residual_bf16) pl.residual = 1;
-            else if (probs[i].residual_f32) pl.residual = 2;
-            pl.BW[i] = P.prob[i].BW; pl.BH[i] = P.prob[i].BH; pl.BI[i] = P.prob[i].BI;
-        }
-        pl.tma_epi = P.tma_epi; pl.ncat = P.ncat; pl.dcat = P.dcat; pl.res_mma = P.res_mma; pl.b_resident = P.b_resident;
-        pl.epi_merge = P.epi_merge; pl.epi_bufs = P.epi_bufs; pl.gn_fused = P.gn_fused;
-        g_tc_plan_set = true;
-    }
-    int lrc = ORP_EINVAL;
-    bool launched = false;
-#define ORP_TC_DISPATCH(BNV)                                                                     \
-    if (!launched && BN == BNV) {                                                                \
-        launched = true;                                                                         \
-        if (deform) {                                                                            \
-            if constexpr (BNV <= 128)                                                            \
-                lrc = out_f32 ? launch_plan<BNV, true, true>(P, stages, grid, st, staging + bres_bytes) : launch_plan<BNV, false, true>(P, stages, grid, st, staging + bres_bytes); \
-        }                                                                                        \
-        else lrc = out_f32 ? launch_plan<BNV, true, false>(P, stages, grid, st, staging + bres_bytes) : launch_plan<BNV, false, false>(P, stages, grid, st, staging + bres_bytes);       \
-    }
-    ORP_TC_DISPATCH(256)
-    ORP_TC_DISPATCH(128)
-    ORP_TC_DISPATCH(64)
-    ORP_TC_DISPATCH(32)
-#undef ORP_TC_DISPATCH
-    if (!launched) return fail(ORP_EINVAL, "conv2d_tc: unsupported tile width");
-    if (lrc) return lrc;
-    if (want_gn && !P.gn_fused) {
-        // statistics requested but not fusable for this shape: separate pass over the bf16 output
-        if (out_f32 || Cout != 256) return fail(ORP_EINVAL, "conv2d_tc: gn_stats needs a 16-bit output with 256 channels");
-        for (int i = 0; i < nprob; ++i)
-            if (probs[i].gn_stats) {
-                int r2 = split ? orp_gn_stats_f16x3(P.prob[i].out, P.prob[i].N, P.prob[i].Ho * P.prob[i].Wo, 256, 32, probs[i].gn_stats, stream)
-                               : orp_gn_stats_bf16(P.prob[i].out, P.prob[i].N, P.prob[i].Ho * P.prob[i].Wo, 256, 32, probs[i].gn_stats, stream);
-                if (r2) return r2;
-            }
     }
     return ORP_OK;
 }

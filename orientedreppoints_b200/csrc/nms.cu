@@ -420,8 +420,7 @@ __device__ __forceinline__ bool frame_prune(const float *p, const float *q, floa
 // start left of i's right edge; lanes test AABBs (coalesced float4 reads of the sorted array), survivors of the area bound
 // are compacted into a per-warp shared-memory queue, filtered by the projection bounds in both boxes' frames, and emitted
 // as candidate pairs (better-ranked box, worse-ranked box) by ORIGINAL index.
-template <int MINB>
-__global__ void __launch_bounds__(kSweepWarps * 32, MINB)
+__global__ void __launch_bounds__(kSweepWarps * 32, 4)
 nms_sweep_kernel(SweepParams P)
 {
     __shared__ int32_t q1[kSweepWarps][64];    // AABB + area-bound survivors: box id,
@@ -1037,10 +1036,7 @@ int run_nms(const float *dets, const int32_t *segments, int n, double thr, int i
                 if (!g_ev[0]) { ORP_CUDA(cudaEventCreate(&g_ev[0])); ORP_CUDA(cudaEventCreate(&g_ev[1])); }
                 ORP_CUDA(cudaEventRecord(g_ev[0], st));
             }
-            static const int minb = getenv("ORP_NMS_SWEEP_MINB") ? atoi(getenv("ORP_NMS_SWEEP_MINB")) : 4;
-            if (minb == 6) nms_sweep_kernel<6><<<grid, kSweepWarps * 32, 0, st>>>(P);
-            else if (minb == 3) nms_sweep_kernel<3><<<grid, kSweepWarps * 32, 0, st>>>(P);
-            else nms_sweep_kernel<4><<<grid, kSweepWarps * 32, 0, st>>>(P);
+            nms_sweep_kernel<<<grid, kSweepWarps * 32, 0, st>>>(P);
             ORP_LAUNCHED();
             if (g_timing) ORP_CUDA(cudaEventRecord(g_ev[1], st));
         } else {

@@ -1,13 +1,15 @@
 """GPU: the wgmma convolution kernel (csrc/dense_tc.cu) against fp64, once per launch plan the detector uses.
 
-For every launch the host code of conv2d_bf16_impl picks a plan from the shapes: accumulator width BN, TMA or staged
+For every launch the host code of conv2d_tc picks a plan from the shapes: accumulator width BN, TMA or staged
 epilogue, the ncat / dcat / res_mma / b_resident / epi_merge / gn_fused variants, output staging buffers, pipeline stages
-and how many tiles each persistent CTA processes.  orp_tc_last_plan reports the plan as launched.
+and how many tiles each persistent CTA processes.  orp_tc_last_plan reports the plan as launched.  The cases (PARITY) live
+in tests/conv_plan_cases.py.
 
 - test_production_plans_are_covered runs the benchmark workloads once and reduces every convolution launch to a plan
   signature (SIG_FIELDS); each one must be pinned by a case of PARITY, so a heuristic change that moves production onto an
   untested plan fails here.
-- test_conv_plan_vs_fp64: one case per signature.  It asserts the plan it reaches, compares with an fp64 reference, and
+- test_conv_plan_vs_fp64: one case per signature.  It asserts the plan it reaches (and that the dry run orp_tc_plan_conv
+  plans the same launch, field for field), compares with an fp64 reference, and
   launches twice into outputs pre-filled with different NaN patterns between guard regions: the two results must be
   bitwise equal and the guards untouched (every output element written exactly once, nothing outside).
 - test_deform_edges: the production DCN plans with zero offsets, samples exactly on the image border and DCNv2 masks."""
@@ -16,6 +18,8 @@ import torch
 import torch.nn.functional as F
 
 from orientedreppoints_b200 import _lib
+
+from conv_plan_cases import PARITY, SIG_FIELDS, case_id, planned, signature
 
 pytestmark = pytest.mark.gpu
 
@@ -26,225 +30,6 @@ BF16_F32_TOL = 2e-5     # bf16 operands, fp32 output: fp32 accumulation of exact
 BF16_TOL = 6e-3         # bf16 output: one rounding to bf16 (2^-8 of the largest value)
 DCN_BF16_TOL = 1.5e-2   # bf16 deformable: the sample is rounded to bf16 before the MMA, the output again
 GN_TOL = 1e-5           # GroupNorm statistics and f16x3 GroupNorm output
-
-SIG_FIELDS = ("precision", "deform", "out", "BN", "tma_epi", "ncat", "dcat", "residual", "b_resident", "epi_merge", "epi_bufs",
-              "gn_fused", "stages", "relu", "bias", "ksplit>1", "nprob>1", "tiles>grid", "Cout%BN", "stem")
-
-
-def signature(p):
-    """the plan reduced to what selects kernel code paths (residual: 0 none, 1 16-bit, 2 fp32; stem: 2 space-to-depth conv1)"""
-    return ("f16x3" if p["split"] else "bf16", p["deform"], "f32" if p["out_f32"] else ("split" if p["split"] else "bf16"),
-            p["BN"], p["tma_epi"], p["ncat"], p["dcat"], p["residual"], p["b_resident"], p["epi_merge"], p["epi_bufs"],
-            p["gn_fused"], p["stages"], p["relu"], p["bias"], int(p["ksplit"] > 1), int(p["nprob"] > 1),
-            int(p["num_tiles"] > p["grid"]), int(p["Cout"] % p["BN"] != 0), p["stem"])
-
-
-# One case per production plan signature: (signature, precision, kind, Cin, Cout, k, stride, bias, act, out_f32, residual,
-# gn, problems).  kind "conv": a k x k convolution (pad k // 2) of every problem (N, H, W), launched the way the engine
-# launches it (split-K where EngineTC._ksplit picks it); "deform": the head's DCN over the problems; "stem": conv1 in
-# space-to-depth form over N images of H x W.  act: 1 ReLU, 2 exact GELU; residual: 1 16-bit, 2 fp32.  The comment above
-# a case names the production layers (workload, layer) that launch its plan.  Shapes are the smallest that reach the
-# plan with output maps that are not multiples of the tile box (or image counts not multiples of BI) and, where production
-# runs several tiles per CTA, more than two tiles per CTA.
-PARITY = [
-    # r101 stem, r50 stem
-    (('f16x3', 0, 'split', 64, 1, 1, 0, 0, 0, 1, 1, 0, 3, 1, 1, 0, 0, 1, 0, 2), 'f16x3', 'stem', 64, 64, 4, 1, 1, 1, 0, 0, 0, [(5, 106, 130)]),
-    # r101 ds0, r50 ds0
-    (('f16x3', 0, 'split', 256, 1, 0, 0, 0, 1, 1, 2, 0, 3, 0, 1, 0, 0, 1, 0, 0), 'f16x3', 'conv', 64, 256, 1, 1, 1, 0, 0, 0, 0, [(1, 133, 130)]),
-    # r101 c1_0, r50 c1_0
-    (('f16x3', 0, 'split', 64, 1, 1, 0, 0, 1, 1, 2, 0, 3, 1, 1, 0, 0, 1, 0, 0), 'f16x3', 'conv', 64, 64, 1, 1, 1, 1, 0, 0, 0, [(1, 133, 130)]),
-    # r101 c2_0, r50 c2_0
-    (('f16x3', 0, 'split', 64, 1, 1, 0, 0, 0, 0, 1, 0, 3, 1, 1, 0, 0, 1, 0, 0), 'f16x3', 'conv', 64, 64, 3, 1, 1, 1, 0, 0, 0, [(1, 133, 130)]),
-    # r101 c3_0, r50 c3_0
-    (('f16x3', 0, 'split', 256, 1, 0, 0, 1, 1, 1, 2, 0, 3, 1, 1, 0, 0, 1, 0, 0), 'f16x3', 'conv', 64, 256, 1, 1, 1, 1, 0, 1, 0, [(1, 133, 130)]),
-    # r101 c1_0, r50 c1_0
-    (('f16x3', 0, 'split', 64, 1, 1, 0, 0, 0, 1, 1, 0, 3, 1, 1, 0, 0, 1, 0, 0), 'f16x3', 'conv', 256, 64, 1, 1, 1, 1, 0, 0, 0, [(1, 133, 130)]),
-    # r101 ds1, r101 ds2, r50 ds1, r50 ds2
-    (('f16x3', 0, 'split', 256, 1, 0, 0, 0, 0, 1, 1, 0, 3, 0, 1, 0, 0, 1, 0, 0), 'f16x3', 'conv', 256, 512, 1, 2, 1, 0, 0, 0, 0, [(2, 133, 130)]),
-    # r101 c1_1, r50 c1_1
-    (('f16x3', 0, 'split', 128, 1, 1, 0, 0, 0, 1, 1, 0, 2, 1, 1, 0, 0, 1, 0, 0), 'f16x3', 'conv', 256, 128, 1, 1, 1, 1, 0, 0, 0, [(1, 133, 130)]),
-    # r101 c2_1, r50 c2_1
-    (('f16x3', 0, 'split', 128, 1, 1, 0, 0, 0, 0, 1, 0, 2, 1, 1, 0, 0, 1, 0, 0), 'f16x3', 'conv', 128, 128, 3, 1, 1, 1, 0, 0, 0, [(1, 133, 130)]),
-    # r101 c3_1, r101 c3_2, r101 c3_3, r50 c3_1, r50 c3_2, r50 c3_3
-    (('f16x3', 0, 'split', 256, 1, 0, 0, 1, 0, 1, 1, 0, 3, 1, 1, 0, 0, 1, 0, 0), 'f16x3', 'conv', 128, 512, 1, 1, 1, 1, 0, 1, 0, [(2, 67, 67)]),
-    # r101 c1_2, r50 c1_2
-    (('f16x3', 0, 'split', 256, 1, 0, 0, 0, 0, 1, 1, 0, 3, 1, 1, 0, 0, 1, 0, 0), 'f16x3', 'conv', 512, 256, 1, 1, 1, 1, 0, 0, 0, [(1, 133, 130)]),
-    # r101 c1_3, r50 c1_2, r50 c1_3, r50 c2_2, r50 c2_3
-    (('f16x3', 0, 'split', 256, 1, 0, 0, 0, 0, 0, 1, 0, 3, 1, 1, 0, 0, 1, 0, 0), 'f16x3', 'conv', 1024, 256, 1, 1, 1, 1, 0, 0, 0, [(1, 133, 130)]),
-    # r101 ds3, r50 ds3, swin qkv3
-    (('f16x3', 0, 'split', 256, 1, 0, 0, 0, 0, 0, 1, 0, 3, 0, 1, 0, 0, 1, 0, 0), 'f16x3', 'conv', 768, 2304, 1, 1, 1, 0, 0, 0, 0, [(4, 25, 17)]),
-    # r101 lat, r50 lat, swin lat
-    (('f16x3', 0, 'split', 256, 1, 0, 0, 0, 0, 1, 1, 1, 3, 0, 0, 0, 0, 1, 0, 0), 'f16x3', 'conv', 192, 256, 1, 1, 0, 0, 0, 0, 1, [(1, 133, 130)]),
-    # r101 fpn, r50 fpn, r50 lat, swin fpn
-    (('f16x3', 0, 'split', 256, 1, 0, 0, 0, 0, 0, 1, 1, 3, 0, 0, 0, 0, 1, 0, 0), 'f16x3', 'conv', 1024, 256, 1, 1, 0, 0, 0, 0, 1, [(1, 133, 130)]),
-    # r101 fpn, r101 lat, r50 fpn, r50 lat
-    (('f16x3', 0, 'split', 256, 1, 0, 0, 0, 0, 0, 1, 1, 3, 0, 0, 0, 0, 0, 0, 0), 'f16x3', 'conv', 1024, 256, 1, 1, 0, 0, 0, 0, 1, [(1, 130, 118)]),
-    # r101 fpn, r101 lat, r50 fpn, r50 lat, r50 p6
-    (('f16x3', 0, 'split', 64, 1, 1, 0, 0, 0, 0, 1, 1, 3, 0, 0, 0, 0, 0, 0, 0), 'f16x3', 'conv', 1024, 256, 1, 1, 0, 0, 0, 0, 1, [(1, 4, 8)]),
-    # r101 p6, r50 fpn, r50 p7
-    (('f16x3', 0, 'f32', 128, 0, 0, 0, 0, 0, 0, 1, 0, 5, 0, 0, 1, 0, 1, 0, 0), 'f16x3', 'conv', 256, 256, 3, 1, 0, 0, 0, 0, 1, [(4, 11, 18)]),
-    # r101 tower, r50 tower, swin tower
-    (('f16x3', 0, 'split', 256, 1, 0, 0, 0, 0, 0, 1, 1, 3, 0, 0, 0, 1, 1, 0, 0), 'f16x3', 'conv', 256, 256, 3, 1, 0, 0, 0, 0, 1, [(2, 115, 79), (2, 58, 40), (2, 29, 20), (2, 15, 10), (2, 8, 5)]),
-    # r101 init_conv, r50 init_conv, swin init_conv
-    (('f16x3', 0, 'split', 256, 1, 0, 0, 0, 0, 0, 1, 0, 3, 1, 1, 0, 1, 1, 0, 0), 'f16x3', 'conv', 256, 256, 3, 1, 1, 1, 0, 0, 0, [(2, 97, 67), (2, 49, 34), (2, 25, 17), (2, 13, 9), (2, 7, 5)]),
-    # r101 cls_out, r101 init_out, r50 cls_out, r50 init_out, swin cls_out, swin init_out
-    (('f16x3', 0, 'f32', 32, 0, 0, 0, 0, 1, 0, 2, 0, 6, 0, 1, 0, 1, 1, 1, 0), 'f16x3', 'conv', 256, 15, 1, 1, 1, 0, 1, 0, 0, [(2, 97, 67), (2, 49, 34), (2, 25, 17), (2, 13, 9), (2, 7, 5)]),
-    # r101 dcn, r50 dcn, swin dcn
-    (('f16x3', 1, 'split', 128, 1, 0, 1, 0, 0, 0, 1, 0, 2, 1, 0, 0, 1, 1, 0, 0), 'f16x3', 'deform', 256, 256, 3, 1, 0, 1, 0, 0, 0, [(5, 33, 33), (5, 17, 17), (5, 9, 9), (5, 5, 5), (5, 3, 3)]),
-    # r101 ref_out, r50 ref_out, swin ref_out
-    (('f16x3', 0, 'f32', 32, 0, 0, 0, 2, 1, 0, 2, 0, 6, 0, 1, 0, 1, 1, 1, 0), 'f16x3', 'conv', 256, 18, 1, 1, 1, 0, 1, 2, 0, [(2, 97, 67), (2, 49, 34), (2, 25, 17), (2, 13, 9), (2, 7, 5)]),
-    # r101 c1_3, r101 c2_3, r50 c1_3, r50 c2_1
-    (('f16x3', 0, 'split', 128, 1, 1, 0, 0, 0, 0, 1, 0, 2, 1, 1, 0, 0, 0, 0, 0), 'f16x3', 'conv', 1024, 512, 1, 1, 1, 1, 0, 0, 0, [(3, 40, 31)]),
-    # r50 c1_1
-    (('f16x3', 0, 'split', 128, 1, 1, 0, 0, 0, 1, 1, 0, 2, 1, 1, 0, 0, 0, 0, 0), 'f16x3', 'conv', 512, 128, 1, 1, 1, 1, 0, 0, 0, [(1, 130, 118)]),
-    # r50 ds2
-    (('f16x3', 0, 'split', 256, 1, 0, 0, 0, 0, 1, 1, 0, 3, 0, 1, 0, 0, 0, 0, 0), 'f16x3', 'conv', 512, 1024, 1, 2, 1, 0, 0, 0, 0, [(3, 79, 61)]),
-    # r50 c1_2
-    (('f16x3', 0, 'split', 256, 1, 0, 0, 0, 0, 1, 1, 0, 3, 1, 1, 0, 0, 0, 0, 0), 'f16x3', 'conv', 512, 256, 1, 1, 1, 1, 0, 0, 0, [(1, 130, 118)]),
-    # r50 c1_2, r50 c1_3, r50 c2_2
-    (('f16x3', 0, 'split', 64, 1, 1, 0, 0, 0, 0, 1, 0, 3, 1, 1, 0, 0, 0, 0, 0), 'f16x3', 'conv', 1024, 256, 1, 1, 1, 1, 0, 0, 0, [(1, 4, 4)]),
-    # r50 c3_2
-    (('f16x3', 0, 'split', 256, 1, 0, 0, 1, 0, 1, 1, 0, 3, 1, 1, 0, 0, 0, 0, 0), 'f16x3', 'conv', 256, 1024, 1, 1, 1, 1, 0, 1, 0, [(3, 40, 31)]),
-    # r50 ds3
-    (('f16x3', 0, 'split', 128, 1, 1, 0, 0, 0, 0, 1, 0, 2, 0, 1, 0, 0, 0, 0, 0), 'f16x3', 'conv', 1024, 2048, 1, 2, 1, 0, 0, 0, 0, [(4, 29, 29)]),
-    # r50 c2_3
-    (('f16x3', 0, 'f32', 256, 0, 0, 0, 0, 0, 0, 1, 0, 3, 0, 0, 1, 0, 1, 0, 0), 'f16x3', 'conv', 512, 512, 3, 1, 1, 1, 0, 0, 0, [(4, 11, 18)]),
-    # r50 c3_3
-    (('f16x3', 0, 'split', 128, 1, 0, 0, 1, 0, 1, 2, 0, 3, 1, 1, 0, 0, 0, 0, 0), 'f16x3', 'conv', 512, 2048, 1, 1, 1, 1, 0, 1, 0, [(1, 29, 31)]),
-    # r50 lat
-    (('f16x3', 0, 'split', 256, 1, 0, 0, 0, 0, 1, 1, 1, 3, 0, 0, 0, 0, 0, 0, 0), 'f16x3', 'conv', 512, 256, 1, 1, 0, 0, 0, 0, 1, [(1, 130, 118)]),
-    # r101 p7, r50 p6, r50 p7
-    (('f16x3', 0, 'f32', 64, 0, 0, 0, 0, 0, 0, 1, 0, 6, 0, 0, 1, 0, 0, 0, 0), 'f16x3', 'conv', 256, 256, 3, 2, 0, 0, 0, 0, 1, [(1, 4, 4)]),
-    # r101 c1_2, r101 c2_2
-    (('f16x3', 0, 'split', 256, 1, 0, 0, 0, 0, 0, 1, 0, 3, 1, 1, 0, 0, 0, 0, 0), 'f16x3', 'conv', 1024, 256, 1, 1, 1, 1, 0, 0, 0, [(1, 130, 118)]),
-    # swin embed
-    (('f16x3', 0, 'split', 128, 1, 1, 0, 0, 1, 1, 1, 0, 3, 0, 1, 0, 0, 1, 1, 0), 'f16x3', 'conv', 64, 96, 1, 1, 1, 0, 0, 0, 0, [(1, 133, 130)]),
-    # swin qkv0
-    (('f16x3', 0, 'split', 64, 1, 1, 0, 0, 1, 1, 1, 0, 3, 0, 1, 0, 0, 1, 1, 0), 'f16x3', 'conv', 96, 288, 1, 1, 1, 0, 0, 0, 0, [(3, 33, 33)]),
-    # swin proj0
-    (('f16x3', 0, 'split', 128, 1, 0, 0, 1, 1, 1, 2, 0, 3, 0, 1, 0, 0, 1, 1, 0), 'f16x3', 'conv', 96, 96, 1, 1, 1, 0, 0, 1, 0, [(1, 133, 130)]),
-    # swin fc1_0
-    (('f16x3', 0, 'split', 128, 1, 1, 0, 0, 0, 1, 1, 0, 2, 2, 1, 0, 0, 1, 0, 0), 'f16x3', 'conv', 96, 384, 1, 1, 1, 2, 0, 0, 0, [(5, 33, 33)]),
-    # swin fc2_0
-    (('f16x3', 0, 'split', 128, 1, 0, 0, 1, 0, 1, 2, 0, 3, 0, 1, 0, 0, 1, 1, 0), 'f16x3', 'conv', 384, 96, 1, 1, 1, 0, 0, 1, 0, [(1, 133, 130)]),
-    # swin red0
-    (('f16x3', 0, 'split', 256, 1, 0, 0, 0, 0, 1, 1, 0, 3, 0, 0, 0, 0, 1, 1, 0), 'f16x3', 'conv', 384, 192, 1, 1, 0, 0, 0, 0, 0, [(1, 133, 130)]),
-    # swin qkv1
-    (('f16x3', 0, 'split', 64, 1, 1, 0, 0, 1, 1, 1, 0, 3, 0, 1, 0, 0, 1, 0, 0), 'f16x3', 'conv', 192, 576, 1, 1, 1, 0, 0, 0, 0, [(5, 17, 17)]),
-    # swin fc2_1, swin proj1
-    (('f16x3', 0, 'split', 256, 1, 0, 0, 1, 0, 1, 1, 0, 3, 0, 1, 0, 0, 1, 1, 0), 'f16x3', 'conv', 192, 192, 1, 1, 1, 0, 0, 1, 0, [(1, 133, 130)]),
-    # swin fc1_1, swin fc1_2
-    (('f16x3', 0, 'split', 256, 1, 0, 0, 0, 0, 1, 1, 0, 3, 2, 1, 0, 0, 1, 0, 0), 'f16x3', 'conv', 192, 768, 1, 1, 1, 2, 0, 0, 0, [(5, 33, 33)]),
-    # swin red1
-    (('f16x3', 0, 'split', 128, 1, 1, 0, 0, 0, 0, 1, 0, 2, 0, 0, 0, 0, 1, 0, 0), 'f16x3', 'conv', 768, 384, 1, 1, 0, 0, 0, 0, 0, [(5, 33, 33)]),
-    # swin qkv2
-    (('f16x3', 0, 'split', 128, 1, 1, 0, 0, 0, 1, 1, 0, 2, 0, 1, 0, 0, 1, 0, 0), 'f16x3', 'conv', 384, 1152, 1, 1, 1, 0, 0, 0, 0, [(4, 25, 17)]),
-    # swin fc2_2, swin proj2
-    (('f16x3', 0, 'split', 128, 1, 0, 0, 1, 0, 1, 2, 0, 3, 0, 1, 0, 0, 1, 0, 0), 'f16x3', 'conv', 384, 384, 1, 1, 1, 0, 0, 1, 0, [(5, 33, 33)]),
-    # swin red2
-    (('f16x3', 0, 'split', 256, 1, 0, 0, 0, 0, 0, 1, 0, 3, 0, 0, 0, 0, 1, 0, 0), 'f16x3', 'conv', 1536, 768, 1, 1, 0, 0, 0, 0, 0, [(5, 33, 33)]),
-    # swin fc2_3, swin proj3
-    (('f16x3', 0, 'split', 256, 1, 0, 0, 1, 0, 1, 1, 0, 3, 0, 1, 0, 0, 1, 0, 0), 'f16x3', 'conv', 768, 768, 1, 1, 1, 0, 0, 1, 0, [(5, 33, 33)]),
-    # swin fc1_3
-    (('f16x3', 0, 'split', 256, 1, 0, 0, 0, 0, 0, 1, 0, 3, 2, 1, 0, 0, 1, 0, 0), 'f16x3', 'conv', 768, 3072, 1, 1, 1, 2, 0, 0, 0, [(4, 17, 17)]),
-    # swin fpn, swin lat
-    (('f16x3', 0, 'split', 128, 1, 1, 0, 0, 0, 0, 1, 1, 2, 0, 0, 0, 0, 0, 0, 0), 'f16x3', 'conv', 768, 256, 1, 1, 0, 0, 0, 0, 1, [(2, 61, 64)]),
-    # swin embed, swin qkv0
-    (('bf16', 0, 'bf16', 32, 0, 0, 0, 0, 1, 0, 2, 0, 6, 0, 1, 0, 0, 1, 0, 0), 'bf16', 'conv', 64, 96, 1, 1, 1, 0, 0, 0, 0, [(5, 33, 33)]),
-    # swin fc2_0, swin proj0
-    (('bf16', 0, 'bf16', 32, 0, 0, 0, 1, 1, 0, 2, 0, 6, 0, 1, 0, 0, 1, 0, 0), 'bf16', 'conv', 96, 96, 1, 1, 1, 0, 0, 1, 0, [(5, 33, 33)]),
-    # swin fc1_0
-    (('bf16', 0, 'bf16', 128, 1, 0, 0, 0, 1, 0, 2, 0, 6, 2, 1, 0, 0, 1, 0, 0), 'bf16', 'conv', 96, 384, 1, 1, 1, 2, 0, 0, 0, [(5, 33, 33)]),
-    # swin red0
-    (('bf16', 0, 'bf16', 64, 1, 0, 0, 0, 1, 0, 2, 0, 6, 0, 0, 0, 0, 1, 0, 0), 'bf16', 'conv', 384, 192, 1, 1, 0, 0, 0, 0, 0, [(5, 33, 33)]),
-    # swin qkv1
-    (('bf16', 0, 'bf16', 64, 1, 0, 0, 0, 1, 0, 2, 0, 6, 0, 1, 0, 0, 1, 0, 0), 'bf16', 'conv', 192, 576, 1, 1, 1, 0, 0, 0, 0, [(5, 17, 17)]),
-    # swin proj1
-    (('bf16', 0, 'bf16', 64, 1, 0, 0, 1, 1, 0, 2, 0, 6, 0, 1, 0, 0, 1, 0, 0), 'bf16', 'conv', 192, 192, 1, 1, 1, 0, 0, 1, 0, [(5, 33, 33)]),
-    # swin fc1_1, swin fc1_2
-    (('bf16', 0, 'bf16', 256, 1, 0, 0, 0, 0, 0, 2, 0, 3, 2, 1, 0, 0, 1, 0, 0), 'bf16', 'conv', 192, 768, 1, 1, 1, 2, 0, 0, 0, [(5, 33, 33)]),
-    # swin fc2_1
-    (('bf16', 0, 'bf16', 64, 1, 0, 0, 1, 0, 0, 2, 0, 6, 0, 1, 0, 0, 1, 0, 0), 'bf16', 'conv', 768, 192, 1, 1, 1, 0, 0, 1, 0, [(5, 33, 33)]),
-    # swin red1
-    (('bf16', 0, 'bf16', 128, 1, 0, 0, 0, 0, 0, 1, 0, 5, 0, 0, 0, 0, 1, 0, 0), 'bf16', 'conv', 768, 384, 1, 1, 0, 0, 0, 0, 0, [(5, 33, 33)]),
-    # swin qkv2
-    (('bf16', 0, 'bf16', 128, 1, 0, 0, 0, 0, 0, 2, 0, 4, 0, 1, 0, 0, 1, 0, 0), 'bf16', 'conv', 384, 1152, 1, 1, 1, 0, 0, 0, 0, [(4, 25, 17)]),
-    # swin fc2_2, swin proj2
-    (('bf16', 0, 'bf16', 128, 1, 0, 0, 1, 0, 0, 2, 0, 4, 0, 1, 0, 0, 1, 0, 0), 'bf16', 'conv', 384, 384, 1, 1, 1, 0, 0, 1, 0, [(5, 33, 33)]),
-    # swin red2
-    (('bf16', 0, 'bf16', 256, 1, 0, 0, 0, 0, 0, 1, 0, 3, 0, 0, 0, 0, 1, 0, 0), 'bf16', 'conv', 1536, 768, 1, 1, 0, 0, 0, 0, 0, [(5, 33, 33)]),
-    # r50 ds3, swin qkv3
-    (('bf16', 0, 'bf16', 256, 1, 0, 0, 0, 0, 0, 1, 0, 3, 0, 1, 0, 0, 1, 0, 0), 'bf16', 'conv', 768, 2304, 1, 1, 1, 0, 0, 0, 0, [(4, 25, 17)]),
-    # swin fc2_3, swin proj3
-    (('bf16', 0, 'bf16', 256, 1, 0, 0, 1, 0, 0, 2, 0, 3, 0, 1, 0, 0, 1, 0, 0), 'bf16', 'conv', 768, 768, 1, 1, 1, 0, 0, 1, 0, [(5, 33, 33)]),
-    # swin fc1_3
-    (('bf16', 0, 'bf16', 256, 1, 0, 0, 0, 0, 0, 1, 0, 3, 2, 1, 0, 0, 1, 0, 0), 'bf16', 'conv', 768, 3072, 1, 1, 1, 2, 0, 0, 0, [(4, 17, 17)]),
-    # r50 lat, swin lat
-    (('bf16', 0, 'bf16', 256, 1, 0, 0, 0, 0, 0, 2, 1, 3, 0, 0, 0, 0, 1, 0, 0), 'bf16', 'conv', 192, 256, 1, 1, 0, 0, 0, 0, 1, [(1, 133, 130)]),
-    # swin fpn, swin lat
-    (('bf16', 0, 'bf16', 128, 1, 0, 0, 0, 0, 0, 1, 1, 5, 0, 0, 0, 0, 0, 0, 0), 'bf16', 'conv', 768, 256, 1, 1, 0, 0, 0, 0, 1, [(2, 61, 64)]),
-    # r50 fpn, r50 lat, swin fpn
-    (('bf16', 0, 'bf16', 256, 1, 0, 0, 0, 0, 0, 1, 1, 3, 0, 0, 0, 0, 1, 0, 0), 'bf16', 'conv', 1024, 256, 1, 1, 0, 0, 0, 0, 1, [(1, 133, 130)]),
-    # r50 tower, swin tower
-    (('bf16', 0, 'bf16', 256, 1, 0, 0, 0, 0, 0, 1, 1, 3, 0, 0, 0, 1, 1, 0, 0), 'bf16', 'conv', 256, 256, 3, 1, 0, 0, 0, 0, 1, [(2, 115, 79), (2, 58, 40), (2, 29, 20), (2, 15, 10), (2, 8, 5)]),
-    # r50 init_conv, swin init_conv
-    (('bf16', 0, 'bf16', 256, 1, 0, 0, 0, 0, 0, 1, 0, 3, 1, 1, 0, 1, 1, 0, 0), 'bf16', 'conv', 256, 256, 3, 1, 1, 1, 0, 0, 0, [(2, 97, 67), (2, 49, 34), (2, 25, 17), (2, 13, 9), (2, 7, 5)]),
-    # r50 cls_out, r50 init_out, swin cls_out, swin init_out
-    (('bf16', 0, 'f32', 32, 0, 0, 0, 0, 1, 0, 2, 0, 6, 0, 1, 0, 1, 1, 1, 0), 'bf16', 'conv', 256, 15, 1, 1, 1, 0, 1, 0, 0, [(2, 97, 67), (2, 49, 34), (2, 25, 17), (2, 13, 9), (2, 7, 5)]),
-    # r50 dcn, swin dcn
-    (('bf16', 1, 'bf16', 128, 1, 0, 0, 0, 0, 0, 1, 0, 3, 1, 0, 0, 1, 1, 0, 0), 'bf16', 'deform', 256, 256, 3, 1, 0, 1, 0, 0, 0, [(5, 33, 33), (5, 17, 17), (5, 9, 9), (5, 5, 5), (5, 3, 3)]),
-    # r50 ref_out, swin ref_out
-    (('bf16', 0, 'f32', 32, 0, 0, 0, 2, 1, 0, 2, 0, 6, 0, 1, 0, 1, 1, 1, 0), 'bf16', 'conv', 256, 18, 1, 1, 1, 0, 1, 2, 0, [(2, 97, 67), (2, 49, 34), (2, 25, 17), (2, 13, 9), (2, 7, 5)]),
-    # r50 stem
-    (('bf16', 0, 'bf16', 64, 1, 0, 0, 0, 1, 0, 2, 0, 6, 1, 1, 0, 0, 1, 0, 2), 'bf16', 'stem', 64, 64, 4, 1, 1, 1, 0, 0, 0, [(5, 106, 130)]),
-    # r50 ds0
-    (('bf16', 0, 'bf16', 256, 1, 0, 0, 0, 1, 0, 2, 0, 6, 0, 1, 0, 0, 1, 0, 0), 'bf16', 'conv', 64, 256, 1, 1, 1, 0, 0, 0, 0, [(1, 133, 130)]),
-    # r50 c1_0
-    (('bf16', 0, 'bf16', 64, 1, 0, 0, 0, 1, 0, 2, 0, 6, 1, 1, 0, 0, 1, 0, 0), 'bf16', 'conv', 64, 64, 1, 1, 1, 1, 0, 0, 0, [(1, 133, 130)]),
-    # r50 c2_0
-    (('bf16', 0, 'bf16', 64, 1, 0, 0, 0, 1, 0, 1, 0, 6, 1, 1, 0, 0, 1, 0, 0), 'bf16', 'conv', 64, 64, 3, 1, 1, 1, 0, 0, 0, [(1, 133, 130)]),
-    # r50 c3_0
-    (('bf16', 0, 'bf16', 256, 1, 0, 0, 1, 1, 0, 2, 0, 6, 1, 1, 0, 0, 1, 0, 0), 'bf16', 'conv', 64, 256, 1, 1, 1, 1, 0, 1, 0, [(1, 133, 130)]),
-    # r50 ds1, r50 ds2
-    (('bf16', 0, 'bf16', 256, 1, 0, 0, 0, 0, 0, 2, 0, 3, 0, 1, 0, 0, 1, 0, 0), 'bf16', 'conv', 256, 512, 1, 2, 1, 0, 0, 0, 0, [(2, 133, 130)]),
-    # r50 c1_1
-    (('bf16', 0, 'bf16', 128, 1, 0, 0, 0, 1, 0, 2, 0, 5, 1, 1, 0, 0, 1, 0, 0), 'bf16', 'conv', 256, 128, 1, 1, 1, 1, 0, 0, 0, [(1, 133, 130)]),
-    # r50 c2_1
-    (('bf16', 0, 'bf16', 128, 1, 0, 0, 0, 0, 0, 1, 0, 5, 1, 1, 0, 0, 1, 0, 0), 'bf16', 'conv', 128, 128, 3, 1, 1, 1, 0, 0, 0, [(1, 133, 130)]),
-    # r50 c3_1
-    (('bf16', 0, 'bf16', 256, 1, 0, 0, 1, 1, 0, 2, 0, 5, 1, 1, 0, 0, 1, 0, 0), 'bf16', 'conv', 128, 512, 1, 1, 1, 1, 0, 1, 0, [(2, 67, 67)]),
-    # r50 c1_1
-    (('bf16', 0, 'bf16', 128, 1, 0, 0, 0, 0, 0, 2, 0, 4, 1, 1, 0, 0, 1, 0, 0), 'bf16', 'conv', 512, 128, 1, 1, 1, 1, 0, 0, 0, [(1, 133, 130)]),
-    # r50 c1_2
-    (('bf16', 0, 'bf16', 256, 1, 0, 0, 0, 0, 0, 2, 0, 3, 1, 1, 0, 0, 1, 0, 0), 'bf16', 'conv', 512, 256, 1, 1, 1, 1, 0, 0, 0, [(1, 133, 130)]),
-    # r50 c1_2, r50 c1_3, r50 c2_2, r50 c2_3
-    (('bf16', 0, 'bf16', 256, 1, 0, 0, 0, 0, 0, 1, 0, 3, 1, 1, 0, 0, 1, 0, 0), 'bf16', 'conv', 1024, 256, 1, 1, 1, 1, 0, 0, 0, [(1, 133, 130)]),
-    # r50 c3_2, r50 c3_3
-    (('bf16', 0, 'bf16', 256, 1, 0, 0, 1, 0, 0, 2, 0, 3, 1, 1, 0, 0, 1, 0, 0), 'bf16', 'conv', 256, 1024, 1, 1, 1, 1, 0, 1, 0, [(5, 25, 33)]),
-    # r50 fpn, r50 lat
-    (('bf16', 0, 'bf16', 256, 1, 0, 0, 0, 0, 0, 1, 1, 3, 0, 0, 0, 0, 0, 0, 0), 'bf16', 'conv', 2048, 256, 1, 1, 0, 0, 0, 0, 1, [(1, 130, 118)]),
-    # r50 p6
-    (('bf16', 0, 'bf16', 64, 1, 0, 0, 0, 0, 0, 1, 1, 6, 0, 0, 0, 0, 0, 0, 0), 'bf16', 'conv', 2048, 256, 3, 2, 0, 0, 0, 0, 1, [(5, 37, 43)]),
-    # r50 p7
-    (('bf16', 0, 'f32', 128, 0, 0, 0, 0, 0, 0, 1, 0, 5, 0, 0, 1, 0, 1, 0, 0), 'bf16', 'conv', 256, 256, 3, 2, 0, 0, 0, 0, 1, [(4, 33, 23)]),
-]
-
-
-def _case_id(c):
-    sig, prec, kind, cin, cout, k, s = c[:7]
-    d = dict(zip(SIG_FIELDS, sig))
-    tags = ["BN%d" % d["BN"], "st%d" % d["stages"]]
-    for f in ("ncat", "dcat", "b_resident", "epi_merge", "gn_fused"):
-        if d[f]:
-            tags.append(f)
-    tags.append("bufs%d" % d["epi_bufs"])
-    if d["residual"]:
-        tags.append("res%s" % ("16" if d["residual"] == 1 else "32"))
-    if d["ksplit>1"]:
-        tags.append("splitk")
-    tags += ["act%d" % d["relu"]] + (["bias"] if d["bias"] else []) + (["multitile"] if d["tiles>grid"] else [])
-    return "%s-%s-%dx%dk%ds%d-%s" % (prec, kind, cin, cout, k, s, "-".join(tags))
-
 
 # ------------------------------------------------------------------------------------------------------------- helpers
 @pytest.fixture(scope="module")
@@ -494,14 +279,15 @@ def _check_gn(case, plan):
 
 
 # ---------------------------------------------------------------------------------------------------------------- tests
-@pytest.mark.parametrize("c", PARITY, ids=[_case_id(c) for c in PARITY])
+@pytest.mark.parametrize("c", PARITY, ids=[case_id(c) for c in PARITY])
 def test_conv_plan_vs_fp64(cuda, engines, c):
     case = Case(c, engines[c[1]], cuda, seed=sum(c[3:7]) + len(c[-1]))
     plan = _check_written_once(case)
     assert signature(plan) == c[0], "the case left its plan: %s" % dict(zip(SIG_FIELDS, signature(plan)))
+    assert plan == planned(c), "the dry run plans another launch: %s" % planned(c)
     err = _check_values(case, plan)
     print("%s: grid %d, %d tiles (%.1f per CTA), %d N tiles, rel err %.2e (tol %.1e)"
-          % (_case_id(c), plan["grid"], plan["num_tiles"], plan["num_tiles"] / plan["grid"], plan["n_tiles_n"], err, case.tol))
+          % (case_id(c), plan["grid"], plan["num_tiles"], plan["num_tiles"] / plan["grid"], plan["n_tiles_n"], err, case.tol))
 
 
 DCN_CASES = [c for c in PARITY if c[2] == "deform"]
@@ -515,6 +301,7 @@ def test_deform_edges(cuda, engines, c, mode):
     case = Case(c, engines[c[1]], cuda, seed=7, offsets=offsets, masks=masks)
     plan = _check_written_once(case)
     assert signature(plan) == c[0]
+    assert plan == planned(c)
     if mode == "zero":
         # zero offsets: every sample is the input pixel itself - the plain 3x3 convolution
         for i, ref in enumerate(case.refs):
