@@ -153,7 +153,7 @@ int orp_tc_timing_collect(float *total_ms, int *launches, double *flops);
  * for tests and traces: there is no way to request a plan (orp_tc_plan_conv only reports one).  ORP_EINVAL before the
  * first launch on the thread. */
 typedef struct {
-    int BN;                  /* accumulator width: 256, 128, 64 or 32 output channels per tile              */
+    int BN;                  /* N-tile width = accumulator width: 256, 128, 64 or 32 output channels         */
     int stages;              /* main-loop pipeline stages                                                    */
     int grid;                /* persistent CTAs                                                              */
     int num_tiles;           /* (m tile, n tile, k split) units; num_tiles > grid: a CTA runs several        */
@@ -170,6 +170,9 @@ typedef struct {
     int residual;            /* 0 none, 1 16-bit residual (bf16 / split), 2 fp32 residual                    */
     int tma_epi, ncat, dcat, res_mma, b_resident, epi_merge, epi_bufs, gn_fused;   /* see csrc/dense_tc.cu      */
     int BW[5], BH[5], BI[5]; /* per problem: the 128-pixel tile box (width, height, images)                  */
+    int n_pair;              /* N tiles a CTA computes together on one A operand: 2 for f16x3 deformable      */
+                             /* launches with 16-bit outputs, no GELU and an even N-tile count (one gather   */
+                             /* per M tile), otherwise 1                                                     */
 } orp_tc_plan;
 int orp_tc_last_plan(orp_tc_plan *out);
 

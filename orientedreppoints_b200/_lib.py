@@ -47,7 +47,7 @@ class TcPlan(ctypes.Structure):
     _fields_ = [(k, _i) for k in ("BN", "stages", "grid", "num_tiles", "n_tiles_n", "ksplit", "nprob", "Cout", "Cout_padded",
                                   "split", "deform", "out_f32", "stem", "relu", "bias", "residual", "tma_epi", "ncat", "dcat",
                                   "res_mma", "b_resident", "epi_merge", "epi_bufs", "gn_fused")] + \
-              [(k, _i * 5) for k in ("BW", "BH", "BI")]
+              [(k, _i * 5) for k in ("BW", "BH", "BI")] + [("n_pair", _i)]
 
     def as_dict(self):
         d = {k: getattr(self, k) for k, _ in self._fields_}

@@ -11,7 +11,8 @@
 //               output rows [64 g, 64 g + 64), accumulating fp32 in registers, and releases the stage once the
 //               MMAs that read it have retired.  After the last K block the same warps run the epilogue: the
 //               accumulator is staged in shared memory 64 columns at a time (fp32, one row per pixel), then
-//               bias / residual / ReLU and bf16, split-fp16 or fp32 NHWC stores.
+//               bias / residual / ReLU and bf16, split-fp16 or fp32 NHWC stores.  (The deformable f16x3 variant that
+//               computes N-tile pairs, 256 columns wide, finishes straight from its register fragments: frag_epilogue.)
 //   warp 8      TMA producer (plain variant): the A tile of one (tap, channel block) is ONE box {64 ch, BW, BH, BI}
 //               of the NHWC activation (tensor-map element strides = conv stride; out-of-bounds
 //               coordinates are zero-filled by the TMA unit = the convolution's zero padding), landing in
@@ -20,7 +21,10 @@
 //   warps 8-15  (deformable variant only) A-operand producers: per output pixel and tap the 4-corner
 //               bilinear sample of the reference (deform_conv_cuda_kernel.cu:84-115) is computed in
 //               fp32 from bf16 features and written to shared memory in the same swizzled layout; their first
-//               thread also issues the TMA loads of the B tiles.
+//               thread also issues the TMA loads of the B tiles.  In f16x3 with 16-bit outputs (the detector's head)
+//               a CTA computes two adjacent 128-wide N tiles as one 256-wide tile (plan field n_pair), so every sample
+//               is taken once: setmaxnreg moves registers from these warps to the consumers, whose fragment is then
+//               64 x 256 fp32.
 // Several "problems" (the five FPN levels, which share the head weights) are served by ONE launch.
 //
 // Two operand modes share the kernel.  bf16: activations / weights rounded to bf16, one MMA per K step.
@@ -208,6 +212,36 @@ __device__ __forceinline__ void acc_ld32(uint32_t addr, uint32_t (&r)[32])
 __device__ __forceinline__ float2 ffma2_rn(float2 a, float2 b, float2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
 __device__ __forceinline__ float2 fadd2_rn(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
 
+// One split-mode deformable sample of 8 channels: the (hi, lo) fp16 rows u[c][0 / 1] of the four corners c blended with
+// the corner weights (wv in fp32; wh the same four as fp16), formed in fp32 and split again into x_hi and x_lo.
+__device__ __forceinline__ void split_sample(const uint4 (&u)[4][2], float4 wv, uint2 wh, uint32_t (&hi)[4], uint32_t (&lo)[4])
+{
+    const float2 wc[4] = {make_float2(wv.x, wv.x), make_float2(wv.y, wv.y), make_float2(wv.z, wv.z), make_float2(wv.w, wv.w)};
+    const __half2 wl[4] = {__low2half2(*reinterpret_cast<const __half2 *>(&wh.x)), __high2half2(*reinterpret_cast<const __half2 *>(&wh.x)),
+                           __low2half2(*reinterpret_cast<const __half2 *>(&wh.y)), __high2half2(*reinterpret_cast<const __half2 *>(&wh.y))};
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        // hi halves: fp32, two channels per packed FMA; lo halves (<= 2^-11 of the value): blended in half2 arithmetic with
+        // fp16 weights - an error of 2^-11 on a 2^-11 term
+        float2 acc = make_float2(0.f, 0.f);
+        __half2 accl = __float2half2_rn(0.f);
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+            const uint32_t uh = reinterpret_cast<const uint32_t *>(&u[c][0])[k];
+            const uint32_t ul = reinterpret_cast<const uint32_t *>(&u[c][1])[k];
+            acc = ffma2_rn(wc[c], __half22float2(*reinterpret_cast<const __half2 *>(&uh)), acc);
+            accl = __hfma2(wl[c], *reinterpret_cast<const __half2 *>(&ul), accl);
+        }
+        acc = fadd2_rn(acc, __half22float2(accl));
+        const __half2 h2 = __floats2half2_rn(acc.x, acc.y);
+        const float2 hf = __half22float2(h2);
+        const float2 rem = fadd2_rn(acc, make_float2(-hf.x, -hf.y));
+        const __half2 l2 = __floats2half2_rn(rem.x, rem.y);
+        hi[k] = *reinterpret_cast<const uint32_t *>(&h2);
+        lo[k] = *reinterpret_cast<const uint32_t *>(&l2);
+    }
+}
+
 // epilogue activation: 0 none, 1 ReLU, 2 exact (erf) GELU as nn.GELU (swin_transformer.py:24-29)
 __device__ __forceinline__ float act_fn(float v, int act)
 {
@@ -315,9 +349,15 @@ __host__ __device__ constexpr int stage_bytes(int BN, bool cat, bool b_resident)
 {
     return cat ? (b_resident ? 2 * kABytes : 2 * kABytes + 2 * BN * kBK * 2) : (b_resident ? kABytes : kABytes + BN * kBK * 2);
 }
-// dynamic shared memory of a launch: 1 KiB alignment slack, the staged accumulator pass, `stages` main-loop stages and
-// `extra` bytes (identity block, resident weight slab, output staging)
-constexpr int dyn_smem_bytes(int stage_b, int stages, int extra) { return 1024 + kAccBytes + stages * stage_b + extra; }
+// The deformable f16x3 variant of N-tile pairs (256 accumulator columns) runs its epilogue straight from the fragments: its two 96 KiB stages
+// leave no room for the staged accumulator pass.  Every other variant stages the accumulator (stage_acc).
+__host__ __device__ constexpr bool frag_epilogue(int BN, bool deform) { return deform && BN == 256; }
+// dynamic shared memory of a launch: 1 KiB alignment slack, the staged accumulator pass (unless frag_epi), `stages`
+// main-loop stages and `extra` bytes (identity block, resident weight slab, output staging)
+constexpr int dyn_smem_bytes(int stage_b, int stages, int extra, bool frag_epi)
+{
+    return 1024 + (frag_epi ? 0 : kAccBytes) + stages * stage_b + extra;
+}
 
 // Columns [64 pass, 64 pass + 64) of this thread's accumulator fragment -> the staged rows (ncat: main + cross columns,
 // added here in fp32 with round-to-nearest).  The pass loop is unrolled with a compile-time index so that the fragment
@@ -361,11 +401,31 @@ __device__ __forceinline__ void wgmma_cols64(float (&acc)[R], uint64_t da, uint6
     if constexpr (G + 1 < NG) wgmma_cols64<NG, BF16, R, G + 1>(acc, da, db, accumulate);
 }
 
+// accumulator (+)= A * B^T over BN columns (dcat walk): one MMA, or at BN = 256 two of 128 columns each - an m64n256 MMA
+// names 128 accumulator registers, all that the 512-thread launch of the deformable variant gives a thread (ptxas allots
+// an instruction's operands against the launch's count, not the setmaxnreg budget).  The B rows of the second half start
+// 128 rows = 16 KiB further, 1024 in the descriptor's address field.  Every column sees the MMA sequence of the 128-wide plan.
+template <int BN, bool BF16>
+__device__ __forceinline__ void wgmma_dcat(float (&acc)[BN / 2], uint64_t da, uint64_t db, uint32_t accumulate)
+{
+    if constexpr (BN == 256) {
+        wgmma_n<128, BF16>(acc_view<0, 64>(acc), da, db, accumulate);
+        wgmma_n<128, BF16>(acc_view<64, 64>(acc), da, db + (uint64_t)1024, accumulate);
+    } else {
+        wgmma_n<BN, BF16>(acc, da, db, accumulate);
+    }
+}
+
 // Register budgets of the plain variant (384 threads launched with 168 registers each = 64 512 of the SM's 65 536): the
 // TMA producer's warpgroup gives registers back, the two consumer warpgroups take them for the accumulator and the
 // epilogue.  2 * 128 * 232 + 128 * 40 = 64 512.
 constexpr int kProducerRegs = 40;
 constexpr int kConsumerRegs = 232;
+// ... and of the wide deformable variant (512 threads launched with 128 registers each): the two gathering warpgroups
+// give registers to the two consumer warpgroups, whose 64 x 256 fp32 fragment alone takes 128.  96 keep two items' corner
+// loads in flight per producer thread, as in the 128-wide variant.  2 * 128 * 160 + 2 * 128 * 96 = 65 536.
+constexpr int kWideConsumerRegs = 160;
+constexpr int kWideProducerRegs = 96;
 
 // BN: accumulator width (32..256).  OUT_F32: fp32 output (head predictions) instead of bf16.  DEFORM: A operand produced
 // by the warps from 8 on (bilinear gather) instead of TMA.  SPLIT: f16x3 (fp16 operand pairs) instead of bf16.  WALK:
@@ -383,6 +443,10 @@ conv_tc_kernel(const __grid_constant__ TcParams P, int stages)
     constexpr bool kCat = WALK == kWalkNcat || WALK == kWalkDcat;             // a stage holds both halves of both operands
     constexpr int kKMode = (SPLIT && !kCat) ? 1 : 0;   // KIter mode: a stage per term
     static_assert(kConsumers + 128 == 384 && 2 * 128 * kConsumerRegs + 128 * kProducerRegs <= 65536, "register split");
+    constexpr bool kFragEpi = frag_epilogue(BN, DEFORM);
+    static_assert(!kFragEpi || (SPLIT && !OUT_F32), "fragment epilogue: deformable f16x3 with a TMA epilogue");
+    static_assert(kConsumers == 256 && kDP == 256 && 2 * 128 * kWideConsumerRegs + 2 * 128 * kWideProducerRegs <= 65536,
+                  "register split (wide deformable)");
     // warp roles.  0-7: consumer warpgroups (wgmma main loop, then epilogue).  plain: 8 TMA producer (9-11 idle).
     // deformable: 8-15 A-operand producers, their thread 0 also loads the B tiles.
     constexpr int kEpiThreads = kConsumers;
@@ -393,7 +457,7 @@ conv_tc_kernel(const __grid_constant__ TcParams P, int stages)
     // dynamic: [staged accumulator pass][identity][resident B][stages: A 16K | B BN*128] then the output staging tile
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     float *s_acc = reinterpret_cast<float *>(smem);
-    smem += kAccBytes;
+    if constexpr (!kFragEpi) smem += kAccBytes;
     constexpr int kBBytes = BN * kBK * 2;
     // b_resident: [B slab: kblocks x kBBytes] then A-only stages; otherwise every stage carries A | B
     const int kStageBytes = stage_bytes(BN, kCat, P.b_resident);
@@ -444,6 +508,7 @@ conv_tc_kernel(const __grid_constant__ TcParams P, int stages)
     if (warp < kConsumers / 32) {
         // ===================================================== consumers: main loop
         if constexpr (!DEFORM) setmaxnreg_inc<kConsumerRegs>();
+        if constexpr (kFragEpi) setmaxnreg_inc<kWideConsumerRegs>();
         const int cw = warp >> 2;                          // consumer warpgroup: accumulator rows [64 cw, 64 cw + 64)
         const uint32_t a_off = (uint32_t)cw * 8192u;       // its 64 rows of a 128-row A tile (64 x 128 B)
         const bool leader = (threadIdx.x & 127) == 0;
@@ -476,6 +541,13 @@ conv_tc_kernel(const __grid_constant__ TcParams P, int stages)
                 held = next;
             };
             for (int kb = 0; kb < kblocks; ++kb, it.next()) {
+                if constexpr (kFragEpi) {
+                    // The wide deformable variant is bound by its gather and has two stages only: the previous K block's
+                    // MMAs retire and free their stage BEFORE the wait for the next one, so that the producers, which
+                    // write a stage as they sample it, find it free when they start on it.
+                    wgmma_wait<0>();
+                    release(-1);
+                }
                 mbar_wait(&full[r.stage], r.phase);
                 const uint32_t sa = smem_u32(smem + (size_t)r.stage * kStageBytes);
                 const uint64_t da = make_desc_sw128(sa + a_off);
@@ -501,9 +573,9 @@ conv_tc_kernel(const __grid_constant__ TcParams P, int stages)
                     const uint64_t dbh = make_desc_sw128(sa + 2 * kABytes), dbl = make_desc_sw128(sa + 2 * kABytes + kBBytes);
 #pragma unroll
                     for (int k = 0; k < kBK / 16; ++k) {
-                        wgmma_n<BN, kBF16>(acc, dl + (uint64_t)(k * 2), dbh + (uint64_t)(k * 2), (kb | k) ? 1u : 0u);   // x_lo * w_hi
-                        wgmma_n<BN, kBF16>(acc, da + (uint64_t)(k * 2), dbl + (uint64_t)(k * 2), 1u);                   // x_hi * w_lo
-                        wgmma_n<BN, kBF16>(acc, da + (uint64_t)(k * 2), dbh + (uint64_t)(k * 2), 1u);                   // x_hi * w_hi
+                        wgmma_dcat<BN, kBF16>(acc, dl + (uint64_t)(k * 2), dbh + (uint64_t)(k * 2), (kb | k) ? 1u : 0u);   // x_lo * w_hi
+                        wgmma_dcat<BN, kBF16>(acc, da + (uint64_t)(k * 2), dbl + (uint64_t)(k * 2), 1u);                   // x_hi * w_lo
+                        wgmma_dcat<BN, kBF16>(acc, da + (uint64_t)(k * 2), dbh + (uint64_t)(k * 2), 1u);                   // x_hi * w_hi
                     }
                 } else {
                     const uint64_t db = make_desc_sw128(P.b_resident ? smem_u32(bres + (size_t)slab * kBBytes) : sa + kABytes);
@@ -569,7 +641,77 @@ conv_tc_kernel(const __grid_constant__ TcParams P, int stages)
             };
             size_t pix;
             const bool valid = row_pixel(rrow, pix);
-            if (OUT_F32) {
+            if constexpr (kFragEpi) {
+                // Epilogue from the fragments (no staged accumulator pass): every consumer thread finishes its own values
+                // with the arithmetic of the staged TMA epilogue below, in the same order, and writes them to the
+                // 128-byte-swizzled staging tile 4 bytes (a column pair) at a time - the 8 rows x 4 column pairs of a
+                // warp's store fall in 32 distinct banks.  A hi and a lo pass per 64 columns, each leaving with one TMA store.
+                const uint32_t obuf_u = smem_u32(stage_out);             // [epi_bufs][16 KiB]
+                const bool io = (et == 0);
+                if (nt != bias_nt) {
+                    bar_sync(bar_a, nthr);                               // previous tile's bias reads are done
+                    for (int c = et; c < BN; c += nthr) s_bias[c] = (P.bias && nt * BN + c < P.Cout) ? P.bias[nt * BN + c] : 0.f;
+                    bias_nt = nt;
+                }
+                size_t pix_r[2];
+                const bool valid_r[2] = {row_pixel(frow, pix_r[0]), row_pixel(frow + 8, pix_r[1])};
+                // per fragment row (frow, frow + 8) and 32-column half of the passes: the staged epilogue's per-thread maxima
+                float amax[2][2] = {{0.f, 0.f}, {0.f, 0.f}};
+#pragma unroll
+                for (int pass = 0; pass < 2 * (BN / 64); ++pass) {
+                    const int half = pass >> 1, oterm = pass & 1;
+                    if (io) {
+                        if (P.epi_bufs == 2) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
+                        else asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+                    }
+                    bar_sync(bar_a, nthr);                               // staging buffer `ob` is free, bias staged
+                    const uint32_t obase = obuf_u + (uint32_t)ob * 16384u;
+#pragma unroll
+                    for (int i = 0; i < 8; ++i) {
+                        const int g = half * 8 + i;                      // 8-column group of the fragment
+                        const float2 bv = *reinterpret_cast<const float2 *>(&s_bias[g * 8 + fcol]);
+#pragma unroll
+                        for (int hr = 0; hr < 2; ++hr) {
+                            const int row = frow + 8 * hr;
+                            float f0 = acc[4 * g + 2 * hr], f1 = acc[4 * g + 2 * hr + 1];
+                            f0 *= P.oscale; f1 *= P.oscale;              // exact: power of two
+                            f0 += bv.x; f1 += bv.y;
+                            if (P.relu) { f0 = fmaxf(f0, 0.f); f1 = fmaxf(f1, 0.f); }     // (n_pair plans have no GELU)
+                            if (oterm == 0) amax[hr][i >> 2] = fmaxf(fmaxf(amax[hr][i >> 2], fabsf(f0)), fabsf(f1));
+                            const __half2 h2 = __floats2half2_rn(f0, f1);
+                            uint32_t v = *reinterpret_cast<const uint32_t *>(&h2);
+                            if (oterm) {
+                                const float2 hf = __half22float2(h2);
+                                const __half2 l2 = __floats2half2_rn(f0 - hf.x, f1 - hf.y);
+                                v = *reinterpret_cast<const uint32_t *>(&l2);
+                            }
+                            const uint32_t at = obase + (uint32_t)row * 128u + ((uint32_t)(i ^ (row & 7)) << 4) + (uint32_t)fcol * 2u;
+                            asm volatile("st.shared.b32 [%0], %1;" ::"r"(at), "r"(v) : "memory");
+                        }
+                    }
+                    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+                    bar_sync(bar_b, nthr);                               // staging written by all
+                    if (io) {
+                        asm volatile(
+                            "cp.async.bulk.tensor.5d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5, %6}], [%1];"
+                            ::"l"(&P.tmOut[pi]), "r"(obase), "r"(nt * BN + half * 64), "r"(oterm),
+                              "r"(wb * pr.BW), "r"(hb * pr.BH), "r"(ib * pr.BI) : "memory");
+                        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+                    }
+                    if (++ob == P.epi_bufs) ob = 0;
+                }
+                // the overflow count of the staged epilogue: one per output pixel and 32-column half with a value beyond the
+                // fp16 range (the four lanes of a fragment row hold its columns)
+#pragma unroll
+                for (int hr = 0; hr < 2; ++hr)
+#pragma unroll
+                    for (int hc = 0; hc < 2; ++hc) {
+                        float m = amax[hr][hc];
+                        m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
+                        m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
+                        if ((lane & 3) == 0 && valid_r[hr] && m > 65504.f) atomicAdd(P.ovf, 1u);
+                    }
+            } else if (OUT_F32) {
                 // fp32 outputs (head predictions, split-K partial sums): straight from the staged rows
 #pragma unroll 1
                 for (int pass = 0; pass < BN / HC; ++pass) {
@@ -899,6 +1041,7 @@ conv_tc_kernel(const __grid_constant__ TcParams P, int stages)
         __shared__ float4 s_w[2][128];
         __shared__ uint2 s_wh[2][128];                     // the same four weights as fp16 (split mode: blend of the lo halves)
         __shared__ int4 s_o[2][128];
+        if constexpr (kFragEpi) setmaxnreg_dec<kWideProducerRegs>();
         const int pt = threadIdx.x - kConsumers;           // 0..kDP-1
         // the B tile(s) of a stage: thread 0 of the producers adds their bytes to the stage's barrier and issues the TMA loads
         auto load_b = [&](int stage, int tap, int cb, int nt) {
@@ -914,21 +1057,18 @@ conv_tc_kernel(const __grid_constant__ TcParams P, int stages)
             int pi, wb, hb, ib, nt;
             decode_tile(P, tile, pi, wb, hb, ib, nt);
             const Problem &pr = P.prob[pi];
-            bool valid = false;
-            int w = 0, h = 0, n = 0;
-            if (pt < 128) {
-                const int iw = pt & (pr.BW - 1), ih = (pt >> pr.lbw) & (pr.BH - 1), ii = pt >> (pr.lbw + pr.lbh);
-                w = wb * pr.BW + iw; h = hb * pr.BH + ih; n = ib * pr.BI + ii;
-                valid = (w < pr.Wo) && (h < pr.Ho) && (n < pr.N);
-            }
             const int taps = P.KH * P.KW;
-            const size_t opix = ((size_t)(valid ? n : 0) * pr.Ho + (valid ? h : 0)) * pr.Wo + (valid ? w : 0);
-            const float *offp = pr.offset + opix * (2 * taps);
-            const float *mskp = pr.mask ? pr.mask + opix * taps : nullptr;
-            const int cpp = P.Cin * (P.split ? 2 : 1);                  // 16-bit elements per pixel (hi and lo halves in split mode)
-            const int img0 = (valid ? n : 0) * pr.H * pr.W * cpp;
             for (int tap = 0; tap < taps; ++tap) {
                 if (pt < 128) {
+                    // this thread's output pixel, derived again for every tap: nothing of it stays live through the gather
+                    const int iw = pt & (pr.BW - 1), ih = (pt >> pr.lbw) & (pr.BH - 1), ii = pt >> (pr.lbw + pr.lbh);
+                    const int w = wb * pr.BW + iw, h = hb * pr.BH + ih, n = ib * pr.BI + ii;
+                    const bool valid = (w < pr.Wo) && (h < pr.Ho) && (n < pr.N);
+                    const size_t opix = ((size_t)(valid ? n : 0) * pr.Ho + (valid ? h : 0)) * pr.Wo + (valid ? w : 0);
+                    const float *offp = pr.offset + opix * (2 * taps);
+                    const float *mskp = pr.mask ? pr.mask + opix * taps : nullptr;
+                    const int cpp = P.Cin * (SPLIT ? 2 : 1);            // 16-bit elements per pixel (hi and lo halves in split mode)
+                    const int img0 = (valid ? n : 0) * pr.H * pr.W * cpp;
                     const int kh = tap / P.KW, kw = tap - kh * P.KW;
                     float4 wv = make_float4(0.f, 0.f, 0.f, 0.f);
                     int4 ov = make_int4(img0, img0, img0, img0);
@@ -960,7 +1100,7 @@ conv_tc_kernel(const __grid_constant__ TcParams P, int stages)
                 }
                 asm volatile("bar.sync 2, %0;" ::"n"(kDP) : "memory");
                 for (int cb = 0; cb < P.cin_blocks; ++cb) {
-                    if (!P.split) {
+                    if constexpr (!SPLIT) {
                         mbar_wait(&empty[r.stage], r.phase ^ 1);
                         if (pt == 0) load_b(r.stage, tap, cb, nt);
                         uint8_t *sa = smem + (size_t)r.stage * kStageBytes;
@@ -1006,69 +1146,72 @@ conv_tc_kernel(const __grid_constant__ TcParams P, int stages)
                         // the reference does (deform_conv_cuda_kernel.cu:84-115), split again, and written as the x_hi and
                         // x_lo tiles of this K block's stage
                         const __half *xh = reinterpret_cast<const __half *>(pr.x);
-                        uint32_t phi[kDItems][4], plo[kDItems][4];
+                        auto load_item = [&](int it, uint4 (&u)[4][2]) {       // item `it` of this thread: its four corners
+                            const int item = pt + it * kDP, row = item >> 3, c16 = item & 7;
+                            const int4 ov = s_o[tb][row];
+                            const int co = cb * kBK + c16 * 8;
+                            const int oo[4] = {ov.x, ov.y, ov.z, ov.w};
 #pragma unroll
-                        for (int i2 = 0; i2 < 2; ++i2) {
-                            uint4 u[kDRound][4][2];
+                            for (int c = 0; c < 4; ++c) {
+                                u[c][0] = *reinterpret_cast<const uint4 *>(xh + oo[c] + co);
+                                u[c][1] = *reinterpret_cast<const uint4 *>(xh + oo[c] + P.Cin + co);
+                            }
+                        };
+                        auto item_at = [&](int it) {                           // its byte offset in the x_hi / x_lo tile
+                            const int item = pt + it * kDP, row = item >> 3, c16 = item & 7;
+                            return (uint32_t)(row * 128 + ((c16 ^ (row & 7)) << 4));
+                        };
+                        if constexpr (!kFragEpi) {
+                            // the samples of all four items are held until the stage is free
+                            uint32_t phi[kDItems][4], plo[kDItems][4];
 #pragma unroll
-                            for (int i1 = 0; i1 < kDRound; ++i1) {
-                                const int item = pt + (i2 * kDRound + i1) * kDP, row = item >> 3, c16 = item & 7;
-                                const int4 ov = s_o[tb][row];
-                                const int co = cb * kBK + c16 * 8;
-                                const int oo[4] = {ov.x, ov.y, ov.z, ov.w};
+                            for (int i2 = 0; i2 < kDItems / kDRound; ++i2) {
+                                uint4 u[kDRound][4][2];
 #pragma unroll
-                                for (int c = 0; c < 4; ++c) {
-                                    u[i1][c][0] = *reinterpret_cast<const uint4 *>(xh + oo[c] + co);
-                                    u[i1][c][1] = *reinterpret_cast<const uint4 *>(xh + oo[c] + P.Cin + co);
+                                for (int i1 = 0; i1 < kDRound; ++i1) load_item(i2 * kDRound + i1, u[i1]);
+#pragma unroll
+                                for (int i1 = 0; i1 < kDRound; ++i1) {
+                                    const int it = i2 * kDRound + i1, row = (pt + it * kDP) >> 3;
+                                    split_sample(u[i1], s_w[tb][row], s_wh[tb][row], phi[it], plo[it]);
                                 }
                             }
-#pragma unroll
-                            for (int i1 = 0; i1 < kDRound; ++i1) {
-                                const int it = i2 * kDRound + i1, item = pt + it * kDP, row = item >> 3;
-                                const float4 wv = s_w[tb][row];
-                                const uint2 wh = s_wh[tb][row];
-                                const float2 wc[4] = {make_float2(wv.x, wv.x), make_float2(wv.y, wv.y), make_float2(wv.z, wv.z), make_float2(wv.w, wv.w)};
-                                const __half2 wl[4] = {__low2half2(*reinterpret_cast<const __half2 *>(&wh.x)), __high2half2(*reinterpret_cast<const __half2 *>(&wh.x)),
-                                                       __low2half2(*reinterpret_cast<const __half2 *>(&wh.y)), __high2half2(*reinterpret_cast<const __half2 *>(&wh.y))};
-#pragma unroll
-                                for (int k = 0; k < 4; ++k) {
-                                    // hi halves: fp32, two channels per packed FMA; lo halves (<= 2^-11 of the value): blended in
-                                    // half2 arithmetic with fp16 weights - an error of 2^-11 on a 2^-11 term
-                                    float2 acc = make_float2(0.f, 0.f);
-                                    __half2 accl = __float2half2_rn(0.f);
-#pragma unroll
-                                    for (int c = 0; c < 4; ++c) {
-                                        const uint32_t uh = reinterpret_cast<const uint32_t *>(&u[i1][c][0])[k];
-                                        const uint32_t ul = reinterpret_cast<const uint32_t *>(&u[i1][c][1])[k];
-                                        acc = ffma2_rn(wc[c], __half22float2(*reinterpret_cast<const __half2 *>(&uh)), acc);
-                                        accl = __hfma2(wl[c], *reinterpret_cast<const __half2 *>(&ul), accl);
-                                    }
-                                    acc = fadd2_rn(acc, __half22float2(accl));
-                                    const __half2 h2 = __floats2half2_rn(acc.x, acc.y);
-                                    const float2 hf = __half22float2(h2);
-                                    const float2 rem = fadd2_rn(acc, make_float2(-hf.x, -hf.y));
-                                    const __half2 l2 = __floats2half2_rn(rem.x, rem.y);
-                                    phi[it][k] = *reinterpret_cast<const uint32_t *>(&h2);
-                                    plo[it][k] = *reinterpret_cast<const uint32_t *>(&l2);
-                                }
-                            }
-                        }
-                        {
                             mbar_wait(&empty[r.stage], r.phase ^ 1);
                             if (pt == 0) load_b(r.stage, tap, cb, nt);
                             uint8_t *sa = smem + (size_t)r.stage * kStageBytes;
 #pragma unroll
                             for (int it = 0; it < kDItems; ++it) {
-                                const int item = pt + it * kDP, row = item >> 3, c16 = item & 7;
-                                const size_t at = (size_t)row * 128 + ((c16 ^ (row & 7)) << 4);
+                                const uint32_t at = item_at(it);
                                 *reinterpret_cast<uint4 *>(sa + at) = make_uint4(phi[it][0], phi[it][1], phi[it][2], phi[it][3]);
                                 *reinterpret_cast<uint4 *>(sa + kABytes + at) = make_uint4(plo[it][0], plo[it][1], plo[it][2], plo[it][3]);
                             }
-                            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                            __syncwarp();
-                            if ((pt & 31) == 0) mbar_arrive(&full[r.stage]);
-                            r.next();
+                        } else {
+                            // wide variant (96 registers: no room to hold the samples): the first round's loads are in
+                            // flight while the stage is awaited, and every sample goes to the stage as soon as it is formed
+                            const uint32_t sa = smem_u32(smem + (size_t)r.stage * kStageBytes);
+#pragma unroll
+                            for (int i2 = 0; i2 < kDItems / kDRound; ++i2) {
+                                uint4 u[kDRound][4][2];
+#pragma unroll
+                                for (int i1 = 0; i1 < kDRound; ++i1) load_item(i2 * kDRound + i1, u[i1]);
+                                if (i2 == 0) {
+                                    mbar_wait(&empty[r.stage], r.phase ^ 1);
+                                    if (pt == 0) load_b(r.stage, tap, cb, nt);
+                                }
+#pragma unroll
+                                for (int i1 = 0; i1 < kDRound; ++i1) {
+                                    const int it = i2 * kDRound + i1, row = (pt + it * kDP) >> 3;
+                                    uint32_t hi[4], lo[4];
+                                    split_sample(u[i1], s_w[tb][row], s_wh[tb][row], hi, lo);
+                                    const uint32_t at = sa + item_at(it);
+                                    sts128(at, make_uint4(hi[0], hi[1], hi[2], hi[3]));
+                                    sts128(at + kABytes, make_uint4(lo[0], lo[1], lo[2], lo[3]));
+                                }
+                            }
                         }
+                        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+                        __syncwarp();
+                        if ((pt & 31) == 0) mbar_arrive(&full[r.stage]);
+                        r.next();
                     }
                 }
                 tb ^= 1;
@@ -1133,6 +1276,7 @@ struct ConvPlan {
     orp_tc_plan rep;
     Problem prob[kMaxProb];
     int num_m_tiles;
+    int kbn;                                  // the kernel's accumulator width: BN, or 2 BN when a CTA computes an N-tile pair
     int extra_bytes;                          // dynamic shared memory beside the stages: identity, resident slab, output staging
 };
 
@@ -1180,11 +1324,17 @@ int plan_conv(const ConvDesc &d, int sms, ConvPlan &pl)
         while (BN > 64 && mtiles * (d.Cout_padded / BN) * ksplit < 120) BN /= 2;
     }
     // the deformable variant's 512 threads leave 128 registers each: a 64 x 128 fp32 accumulator fragment (64 per thread)
-    // fits beside the epilogue, a 64 x 256 one does not
+    // fits beside the staged epilogue, a 64 x 256 one does not
     if (d.deform && BN > 128) BN = 128;
     // a partial last channel block is zero-filled by TMA (A operand) and by the weight layout (B operand)
     const int cin_blocks = (d.Cin + kBK - 1) / kBK;
     const int n_tiles_n = d.Cout_padded / BN;
+    // N-tile pairs: in f16x3 with 16-bit outputs and no GELU (the detector's head) a deformable launch computes two adjacent
+    // 128-wide N tiles of an M tile in one CTA, on ONE sampled A operand - every sample is gathered once per M tile instead
+    // of once per N tile, half the gathered bytes.  The kernel runs them as one 256-wide tile, in the variant whose consumers
+    // take registers from the producers and finish from the fragments (frag_epilogue).
+    const int n_pair = (d.deform && d.split && !d.out_f32 && d.Cout % 8 == 0 && d.relu != 2 && BN == 128 && n_tiles_n % 2 == 0) ? 2 : 1;
+    const int kbn = BN * n_pair;
     int mt = 0;
     for (int i = 0; i < nprob; ++i) {
         const orp_tc_problem &q = probs[i];
@@ -1217,7 +1367,8 @@ int plan_conv(const ConvDesc &d, int sms, ConvPlan &pl)
     if (d.split && !d.out_f32 && !tma_epi) return fail(ORP_EINVAL, "conv2d_f16x3: 16-bit outputs need Cout % 8 == 0 and weights padded to a multiple of 64 rows");
     if (d.split && d.out_f32 && any_res) return fail(ORP_EINVAL, "conv2d_f16x3: fp32 outputs take an fp32 residual only");
     // GroupNorm statistics: fused into the TMA epilogue when every warp's 32 rows lie in one image
-    bool want_gn = false, gn_ok = tma_epi && d.Cout == 256 && !d.bias && !d.relu;
+    const bool frag_epi = frag_epilogue(kbn, d.deform != 0);     // (fuses no GroupNorm statistics, merges no hi / lo tiles)
+    bool want_gn = false, gn_ok = tma_epi && d.Cout == 256 && !d.bias && !d.relu && !frag_epi;
     for (int i = 0; i < nprob; ++i) {
         want_gn = want_gn || (probs[i].gn_stats != nullptr);
         if (pl.prob[i].BW * pl.prob[i].BH < 32) gn_ok = false;
@@ -1225,7 +1376,7 @@ int plan_conv(const ConvDesc &d, int sms, ConvPlan &pl)
     const int gn_fused = (want_gn && gn_ok) ? 1 : 0;
     const bool mem_bound = any_res || (d.KH * d.KW * (d.Cin / kBK) <= 8);
     int epi_bufs = mem_bound ? 2 : 1;          // a second staging tile costs compute-bound layers a main-loop stage
-    const int epi_merge = (d.split && tma_epi && (mem_bound || d.stem == 2)) ? 1 : 0;
+    const int epi_merge = (d.split && tma_epi && !frag_epi && (mem_bound || d.stem == 2)) ? 1 : 0;
     // terms concatenated along N for narrow layers (kernel header); the residual / deformable / fp32-output variants keep
     // the K-concatenated walk
     const int dcat = (d.split && d.deform) ? 1 : 0;
@@ -1240,19 +1391,19 @@ int plan_conv(const ConvDesc &d, int sms, ConvPlan &pl)
     // layers whose whole weight slab for one N tile is <= 72 KiB keep it resident; stages then carry only the A tile
     const int slab_bytes = d.KH * d.KW * T * cin_blocks * BN * kBK * 2;
     int b_resident = (!d.deform && ksplit == 1 && slab_bytes <= 72 * 1024) ? 1 : 0;
-    int grid = num_tiles < sms ? num_tiles : sms;
+    int grid = num_tiles / n_pair < sms ? num_tiles / n_pair : sms;      // a CTA takes an N-tile pair at a time
     if (b_resident && grid >= n_tiles_n) grid -= grid % n_tiles_n;       // fixed N tile per CTA
     else if (b_resident) b_resident = 0;
     // shared-memory budget: staged accumulator pass + output staging + resident weights + main-loop stages.  When the extras
     // leave fewer than three stages they are given up in order of least value: the second staging slot, the resident slab.
     int stage_b = 0, extra = 0, stages = 0;
     for (;;) {
-        stage_b = stage_bytes(BN, ncat || dcat, b_resident);
+        stage_b = stage_bytes(kbn, ncat || dcat, b_resident);
         const int hc = BN < 64 ? BN : 64;
         int staging = d.out_f32 ? 0 : 128 * (hc * 2 + 16);
         if (tma_epi) staging = epi_bufs * (epi_merge ? 32768 : 16384);
         extra = (res_mma ? 8192 : 0) + (b_resident ? slab_bytes : 0) + staging;
-        stages = (kSmemPerBlock - (d.deform ? kStaticSmemDeform : kStaticSmemPlain) - dyn_smem_bytes(stage_b, 0, extra)) / stage_b;
+        stages = (kSmemPerBlock - (d.deform ? kStaticSmemDeform : kStaticSmemPlain) - dyn_smem_bytes(stage_b, 0, extra, frag_epi)) / stage_b;
         if (stages >= 3) break;
         if (epi_bufs == 2) { epi_bufs = 1; continue; }
         if (b_resident) { b_resident = 0; continue; }
@@ -1263,6 +1414,7 @@ int plan_conv(const ConvDesc &d, int sms, ConvPlan &pl)
     if (d.deform && stages > 3) stages = 3;     // leave L1 capacity for the bilinear gather (corner reuse between neighbouring pixels)
 
     pl.num_m_tiles = mt;
+    pl.kbn = kbn;
     pl.extra_bytes = extra;
     orp_tc_plan &r = pl.rep;
     r.BN = BN; r.stages = stages; r.grid = grid; r.num_tiles = num_tiles; r.n_tiles_n = n_tiles_n;
@@ -1275,7 +1427,7 @@ int plan_conv(const ConvDesc &d, int sms, ConvPlan &pl)
         r.BW[i] = pl.prob[i].BW; r.BH[i] = pl.prob[i].BH; r.BI[i] = pl.prob[i].BI;
     }
     r.tma_epi = tma_epi; r.ncat = ncat; r.dcat = dcat; r.res_mma = res_mma; r.b_resident = b_resident;
-    r.epi_merge = epi_merge; r.epi_bufs = epi_bufs; r.gn_fused = gn_fused;
+    r.epi_merge = epi_merge; r.epi_bufs = epi_bufs; r.gn_fused = gn_fused; r.n_pair = n_pair;
     return ORP_OK;
 }
 
@@ -1293,7 +1445,7 @@ int make_params(const ConvDesc &d, const ConvPlan &pl, TcParams &P)
         ORP_CUDA(cudaGetSymbolAddress(&ovf, g_f16_overflow));
         P.ovf = static_cast<unsigned int *>(ovf);
     }
-    P.n_tiles_n = pl.rep.n_tiles_n;
+    P.n_tiles_n = pl.rep.n_tiles_n / pl.rep.n_pair;              // the kernel's N tiles are kbn wide
     P.fd_ntn.set((uint32_t)P.n_tiles_n);
     for (int i = 0; i < d.nprob; ++i) {
         const orp_tc_problem &q = d.probs[i];
@@ -1303,7 +1455,7 @@ int make_params(const ConvDesc &d, const ConvPlan &pl, TcParams &P)
         pr.x = static_cast<const __nv_bfloat16 *>(q.x); pr.offset = q.offset; pr.gn_stats = q.gn_stats; pr.mask = q.mask;
     }
     P.num_m_tiles = pl.num_m_tiles;
-    P.num_tiles = pl.rep.num_tiles;
+    P.num_tiles = pl.rep.num_tiles / pl.rep.n_pair;
     P.ksplit = d.ksplit;
     P.fd_ks.set((uint32_t)d.ksplit);
     P.ks_stride = (long long)P.prob[0].N * P.prob[0].Ho * P.prob[0].Wo * d.Cout;
@@ -1350,7 +1502,7 @@ int encode_maps(const ConvDesc &d, const ConvPlan &pl, TcParams &P)
         const cuuint64_t K = (cuuint64_t)d.KH * d.KW * T * P.cin_blocks * kBK;
         cuuint64_t gdim[2] = {K, (cuuint64_t)d.Cout_padded};
         cuuint64_t gstr[1] = {K * 2};
-        cuuint32_t box[2] = {(cuuint32_t)kBK, (cuuint32_t)pl.rep.BN};
+        cuuint32_t box[2] = {(cuuint32_t)kBK, (cuuint32_t)pl.kbn};
         cuuint32_t estr[2] = {1, 1};
         CUresult r = enc(&P.tmB, dt16, 2, const_cast<void *>(d.w), gdim, gstr, box, estr,
                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -1400,7 +1552,7 @@ template <int BN, bool OUT_F32, bool DEFORM, bool SPLIT, int WALK>
 int launch_tc(const TcParams &P, int stages, int grid, cudaStream_t st, int extra_bytes)
 {
     constexpr bool kCat = WALK == kWalkNcat || WALK == kWalkDcat;
-    const int smem = dyn_smem_bytes(stage_bytes(BN, kCat, P.b_resident), stages, extra_bytes);
+    const int smem = dyn_smem_bytes(stage_bytes(BN, kCat, P.b_resident), stages, extra_bytes, frag_epilogue(BN, DEFORM));
     auto kern = conv_tc_kernel<BN, OUT_F32, DEFORM, SPLIT, WALK>;
     static int smem_max = -1;                  // dynamic shared memory beside this instantiation's static shared memory
     if (smem_max < 0) {
@@ -1458,8 +1610,14 @@ int launch_plan(const TcParams &P, int stages, int grid, cudaStream_t st, int ex
 {
     if constexpr (DEFORM) {
         if (P.dcat != P.split || P.ncat || P.res_mma) return fail(ORP_EINVAL, "conv2d_tc: deformable plan outside dcat == split");
-        return P.split ? launch_tc<BN, OUT_F32, true, true, kWalkDcat>(P, stages, grid, st, extra_bytes)
-                       : launch_tc<BN, OUT_F32, true, false, kWalkK>(P, stages, grid, st, extra_bytes);
+        if constexpr (frag_epilogue(BN, true)) {
+            if (!P.split || OUT_F32 || !P.tma_epi || P.epi_merge || P.gn_fused || P.relu == 2)
+                return fail(ORP_EINVAL, "conv2d_tc: deformable N-tile pair outside f16x3 with an unmerged TMA epilogue and no GELU");
+            return launch_tc<BN, false, true, true, kWalkDcat>(P, stages, grid, st, extra_bytes);
+        } else {
+            return P.split ? launch_tc<BN, OUT_F32, true, true, kWalkDcat>(P, stages, grid, st, extra_bytes)
+                           : launch_tc<BN, OUT_F32, true, false, kWalkK>(P, stages, grid, st, extra_bytes);
+        }
     } else {
         if (P.ncat && P.res_mma) return fail(ORP_EINVAL, "conv2d_tc: ncat plan with a residual");
         if (P.ncat) {
@@ -1479,14 +1637,15 @@ int launch_plan(const TcParams &P, int stages, int grid, cudaStream_t st, int ex
     }
 }
 
-// the plan's accumulator width as a template argument (the deformable variant is built up to BN = 128)
+// the kernel's accumulator width as a template argument (the deformable variant is built up to 128, and 256 wide for the
+// N-tile pairs of f16x3 with 16-bit outputs)
 template <bool OUT_F32, bool DEFORM>
 int launch_bn(const TcParams &P, const ConvPlan &pl, cudaStream_t st)
 {
     const int s = pl.rep.stages, g = pl.rep.grid, e = pl.extra_bytes;
-    switch (pl.rep.BN) {
+    switch (pl.kbn) {
     case 256:
-        if constexpr (!DEFORM) return launch_plan<256, OUT_F32, false>(P, s, g, st, e);
+        if constexpr (!DEFORM || !OUT_F32) return launch_plan<256, OUT_F32, DEFORM>(P, s, g, st, e);
         break;
     case 128: return launch_plan<128, OUT_F32, DEFORM>(P, s, g, st, e);
     case 64: return launch_plan<64, OUT_F32, DEFORM>(P, s, g, st, e);
