@@ -6,7 +6,7 @@
 //   orp_box_iou_rotated        mmdet/ops/box_iou_rotated/src/box_iou_rotated_cuda.cu:13-62
 //
 // Layout: row boxes are converted to corners once and staged in shared memory per tile; a block
-// computes a 32 x 32 output tile, threadIdx.x runs along K so the fp32 stores are coalesced
+// computes 32 x 32 output tiles (one column tile, row tiles gridDim.y apart), threadIdx.x runs along K so the fp32 stores are coalesced
 // (128 B per warp).  The kernels are bound by the output write (4 B per pair) once the AABB
 // early-out removes the clipping work for disjoint pairs.
 #include "common.cuh"
@@ -95,6 +95,11 @@ __device__ __forceinline__ float quad_iou_value(const float *a, const float *b, 
 }
 
 constexpr int kTile = 32;
+// Row tiles sit on grid.y, which stops at 65 535 blocks: a block walks the row tiles gridDim.y apart, so any n
+// (N proposals against a few queries is the common use) fits in one launch.
+constexpr int kMaxRowBlocks = 65535;
+
+static dim3 pair_grid(int n, int k) { return dim3(ceil_div(k, kTile), ceil_div(n, kTile) < kMaxRowBlocks ? ceil_div(n, kTile) : kMaxRowBlocks); }
 
 __global__ void __launch_bounds__(kTile * 8)
 quad_iou_matrix_kernel(const float *__restrict__ qa, int n, const float *__restrict__ qb, int k,
@@ -102,27 +107,29 @@ quad_iou_matrix_kernel(const float *__restrict__ qa, int n, const float *__restr
 {
     __shared__ float sa[kTile][9];
     __shared__ float sb[kTile][9];
-    const int r0 = blockIdx.y * kTile, c0 = blockIdx.x * kTile;
+    const int c0 = blockIdx.x * kTile;
     const int tid = threadIdx.y * kTile + threadIdx.x;   // 256 threads
-    {
-        const int row = tid >> 3, c = tid & 7;
-        if (r0 + row < n) sa[row][c] = qa[(size_t)(r0 + row) * 8 + c];
-        if (c0 + row < k) sb[row][c] = qb[(size_t)(c0 + row) * 8 + c];
-    }
-    __syncthreads();
+    const int srow = tid >> 3, sc = tid & 7;
+    if (c0 + srow < k) sb[srow][sc] = qb[(size_t)(c0 + srow) * 8 + sc];
     const int col = c0 + threadIdx.x;
-    if (col >= k) return;
-    float b[8];
+    for (long long r0 = (long long)blockIdx.y * kTile; r0 < n; r0 += (long long)gridDim.y * kTile) {
+        if (r0 + srow < n) sa[srow][sc] = qa[(size_t)(r0 + srow) * 8 + sc];
+        __syncthreads();
+        if (col < k) {
+            float b[8];
 #pragma unroll
-    for (int c = 0; c < 8; ++c) b[c] = sb[threadIdx.x][c];
+            for (int c = 0; c < 8; ++c) b[c] = sb[threadIdx.x][c];
 #pragma unroll 1
-    for (int rr = threadIdx.y; rr < kTile; rr += 8) {
-        const int row = r0 + rr;
-        if (row >= n) break;
-        float a[8];
+            for (int rr = threadIdx.y; rr < kTile; rr += 8) {
+                const long long row = r0 + rr;
+                if (row >= n) break;
+                float a[8];
 #pragma unroll
-        for (int c = 0; c < 8; ++c) a[c] = sa[rr][c];
-        out[(size_t)row * k + col] = quad_iou_value(a, b, iou_mode, union_mode);
+                for (int c = 0; c < 8; ++c) a[c] = sa[rr][c];
+                out[(size_t)row * k + col] = quad_iou_value(a, b, iou_mode, union_mode);
+            }
+        }
+        __syncthreads();                                  // the tile's rows are consumed before the next one is staged
     }
 }
 
@@ -147,49 +154,62 @@ box_iou_rotated_kernel(const float *__restrict__ b1, int n, const float *__restr
 {
     __shared__ float s1[kTile][5];
     __shared__ float s2[kTile][5];
-    const int r0 = blockIdx.y * kTile, c0 = blockIdx.x * kTile;
+    const int c0 = blockIdx.x * kTile;
     const int tid = threadIdx.y * kTile + threadIdx.x;
-    if (tid < kTile * 5) {
-        const int row = tid / 5, c = tid % 5;
-        if (r0 + row < n) s1[row][c] = b1[(size_t)(r0 + row) * 5 + c];
-        if (c0 + row < m) s2[row][c] = b2[(size_t)(c0 + row) * 5 + c];
-    }
-    __syncthreads();
+    const int srow = tid / 5, sc = tid % 5;
+    if (tid < kTile * 5 && c0 + srow < m) s2[srow][sc] = b2[(size_t)(c0 + srow) * 5 + sc];
     const int col = c0 + threadIdx.x;
-    if (col >= m) return;
-    const float x2 = s2[threadIdx.x][0], y2 = s2[threadIdx.x][1], w2 = s2[threadIdx.x][2], h2 = s2[threadIdx.x][3];
-    float sn2, cs2;
-    sincosf(s2[threadIdx.x][4], &sn2, &cs2);
+    for (long long r0 = (long long)blockIdx.y * kTile; r0 < n; r0 += (long long)gridDim.y * kTile) {
+        if (tid < kTile * 5 && r0 + srow < n) s1[srow][sc] = b1[(size_t)(r0 + srow) * 5 + sc];
+        __syncthreads();
+        if (col < m) {
+            const float x2 = s2[threadIdx.x][0], y2 = s2[threadIdx.x][1], w2 = s2[threadIdx.x][2], h2 = s2[threadIdx.x][3];
+            float sn2, cs2;
+            sincosf(s2[threadIdx.x][4], &sn2, &cs2);
 #pragma unroll 1
-    for (int rr = threadIdx.y; rr < kTile; rr += 8) {
-        const int row = r0 + rr;
-        if (row >= n) break;
-        const float x1 = s1[rr][0], y1 = s1[rr][1], w1 = s1[rr][2], h1 = s1[rr][3];
-        const float area1 = w1 * h1, area2 = w2 * h2;
-        float res = 0.f;
-        if (!(area1 < 1e-14f || area2 < 1e-14f)) {
-            float sn1, cs1;
-            sincosf(s1[rr][4], &sn1, &cs1);
-            const float sx = 0.5f * (x1 + x2), sy = 0.5f * (y1 + y2);
-            float a[8], b[8];
-            {
-                const float xc = x1 - sx, yc = y1 - sy, c = 0.5f * cs1, s = 0.5f * sn1;
-                a[0] = xc - s * h1 - c * w1; a[1] = yc + c * h1 - s * w1;
-                a[2] = xc + s * h1 - c * w1; a[3] = yc - c * h1 - s * w1;
-                a[4] = 2.f * xc - a[0]; a[5] = 2.f * yc - a[1];
-                a[6] = 2.f * xc - a[2]; a[7] = 2.f * yc - a[3];
+            for (int rr = threadIdx.y; rr < kTile; rr += 8) {
+                const long long row = r0 + rr;
+                if (row >= n) break;
+                const float x1 = s1[rr][0], y1 = s1[rr][1], w1 = s1[rr][2], h1 = s1[rr][3];
+                const float area1 = w1 * h1, area2 = w2 * h2;
+                float res = 0.f;
+                // the float areas against the double literal, as box_iou_rotated_utils.h:334 compares them: an area of
+                // exactly (float)1e-14 is below 1e-14 and gives 0
+                if (!((double)area1 < 1e-14 || (double)area2 < 1e-14)) {
+                    float sn1, cs1;
+                    sincosf(s1[rr][4], &sn1, &cs1);
+                    const float sx = 0.5f * (x1 + x2), sy = 0.5f * (y1 + y2);
+                    float a[8], b[8];
+                    {
+                        const float xc = x1 - sx, yc = y1 - sy, c = 0.5f * cs1, s = 0.5f * sn1;
+                        a[0] = xc - s * h1 - c * w1; a[1] = yc + c * h1 - s * w1;
+                        a[2] = xc + s * h1 - c * w1; a[3] = yc - c * h1 - s * w1;
+                        a[4] = 2.f * xc - a[0]; a[5] = 2.f * yc - a[1];
+                        a[6] = 2.f * xc - a[2]; a[7] = 2.f * yc - a[3];
+                    }
+                    {
+                        const float xc = x2 - sx, yc = y2 - sy, c = 0.5f * cs2, s = 0.5f * sn2;
+                        b[0] = xc - s * h2 - c * w2; b[1] = yc + c * h2 - s * w2;
+                        b[2] = xc + s * h2 - c * w2; b[3] = yc - c * h2 - s * w2;
+                        b[4] = 2.f * xc - b[0]; b[5] = 2.f * yc - b[1];
+                        b[6] = 2.f * xc - b[2]; b[7] = 2.f * yc - b[3];
+                    }
+                    // disjoint corner hulls: the intersection is empty.  The clip alone does not give 0 when the centre
+                    // shift has collapsed a tiny box onto one fp32 point far from the other (the reference returns
+                    // garbage there, up to inf)
+                    const float axmin = fminf(fminf(a[0], a[2]), fminf(a[4], a[6])), axmax = fmaxf(fmaxf(a[0], a[2]), fmaxf(a[4], a[6]));
+                    const float aymin = fminf(fminf(a[1], a[3]), fminf(a[5], a[7])), aymax = fmaxf(fmaxf(a[1], a[3]), fmaxf(a[5], a[7]));
+                    const float bxmin = fminf(fminf(b[0], b[2]), fminf(b[4], b[6])), bxmax = fmaxf(fmaxf(b[0], b[2]), fmaxf(b[4], b[6]));
+                    const float bymin = fminf(fminf(b[1], b[3]), fminf(b[5], b[7])), bymax = fmaxf(fmaxf(b[1], b[3]), fmaxf(b[5], b[7]));
+                    if (axmin < bxmax && bxmin < axmax && aymin < bymax && bymin < aymax) {
+                        FastRes r = fast_quad_pair(a, b);
+                        res = r.inter / (area1 + area2 - r.inter);
+                    }
+                }
+                out[(size_t)row * m + col] = res;
             }
-            {
-                const float xc = x2 - sx, yc = y2 - sy, c = 0.5f * cs2, s = 0.5f * sn2;
-                b[0] = xc - s * h2 - c * w2; b[1] = yc + c * h2 - s * w2;
-                b[2] = xc + s * h2 - c * w2; b[3] = yc - c * h2 - s * w2;
-                b[4] = 2.f * xc - b[0]; b[5] = 2.f * yc - b[1];
-                b[6] = 2.f * xc - b[2]; b[7] = 2.f * yc - b[3];
-            }
-            FastRes r = fast_quad_pair(a, b);
-            res = r.inter / (area1 + area2 - r.inter);
         }
-        out[(size_t)row * m + col] = res;
+        __syncthreads();                                  // the tile's rows are consumed before the next one is staged
     }
 }
 
@@ -197,8 +217,7 @@ static int quad_matrix(const float *qa, int n, const float *qb, int k, int iou_m
                        float *out, cudaStream_t st)
 {
     if (n == 0 || k == 0) return ORP_OK;
-    dim3 grid(ceil_div(k, kTile), ceil_div(n, kTile)), block(kTile, 8);
-    quad_iou_matrix_kernel<<<grid, block, 0, st>>>(qa, n, qb, k, iou_mode, union_mode, out);
+    quad_iou_matrix_kernel<<<pair_grid(n, k), dim3(kTile, 8), 0, st>>>(qa, n, qb, k, iou_mode, union_mode, out);
     ORP_LAUNCHED();
     return ORP_OK;
 }
@@ -286,8 +305,7 @@ extern "C" int orp_box_iou_rotated(const float *boxes1, int n, const float *boxe
     int rc = ensure_device();
     if (rc) return rc;
     if (n == 0 || m == 0) return ORP_OK;
-    dim3 grid(ceil_div(m, kTile), ceil_div(n, kTile)), block(kTile, 8);
-    box_iou_rotated_kernel<<<grid, block, 0, static_cast<cudaStream_t>(stream)>>>(boxes1, n, boxes2, m, out);
+    box_iou_rotated_kernel<<<pair_grid(n, m), dim3(kTile, 8), 0, static_cast<cudaStream_t>(stream)>>>(boxes1, n, boxes2, m, out);
     ORP_LAUNCHED();
     return ORP_OK;
 }

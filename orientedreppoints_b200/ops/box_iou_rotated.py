@@ -4,8 +4,16 @@ import torch
 from .. import _lib
 
 
+def _check_rows(name, t, width):
+    """the kernels read `width` floats per row: any other shape would read past the buffer"""
+    if t.dim() != 2 or t.shape[1] != width:
+        raise ValueError("%s: expected a [N, %d] tensor, got %s" % (name, width, list(t.shape)))
+
+
 def box_iou_rotated(boxes1, boxes2):
     """boxes [N,5], [M,5] = (cx, cy, w, h, theta in radians) -> IoU [N,M] float32 (CUDA only)."""
+    _check_rows("box_iou_rotated boxes1", boxes1, 5)
+    _check_rows("box_iou_rotated boxes2", boxes2, 5)
     if not (boxes1.is_cuda and boxes2.is_cuda):
         raise RuntimeError("box_iou_rotated: this build has no CPU path; tensors must be CUDA")
     b1 = boxes1.float().contiguous()
@@ -22,6 +30,8 @@ def box_iou_rotated(boxes1, boxes2):
 
 def quad_iou_matrix(quads_a, quads_b, mode="exact64", union_mode=_lib.ORP_UNION_NAN_KEEPS):
     """N x K IoU of 8-coordinate quadrilaterals (the rnms/poly_nms IoU as a matrix)."""
+    _check_rows("quad_iou_matrix quads_a", quads_a, 8)
+    _check_rows("quad_iou_matrix quads_b", quads_b, 8)
     a = quads_a.float().contiguous()
     b = quads_b.float().contiguous()
     n, k = a.shape[0], b.shape[0]
