@@ -260,6 +260,30 @@ int orp_dcn_offsets_multi(int nprob, const float *const *pts, float *const *off,
                           float gradient_mul, const float *base18, void *stream);
 
 /* ------------------------------------------------------------------------------------------
+ * DOTA Task1 evaluation
+ * ---------------------------------------------------------------------------------------- */
+
+/* voc_eval (DOTA_devkit/dota_evaluation_task1.py:87-248) for every class in one call, device pointers, asynchronous.
+ *   detections   det_cls / det_img int32 [nd], det_score fp64 [nd], det_quad fp64 [nd, 8]
+ *   ground truth gt_cls / gt_img int32 [ng], gt_quad fp64 [ng, 8], gt_difficult uint8 [ng] (nonzero: difficult)
+ *   ids are class in [0, ncls), image in [0, nimg); a detection with an id outside them belongs to no class range and is
+ *   matched to nothing, a ground-truth box with one is ignored
+ *   thresholds11 HOST fp64 [11]: the recall thresholds of the 11-point metric (np.arange(0., 1.1, 0.1)), read when
+ *   use_07_metric != 0
+ * Outputs (device): npos_out int64 [ncls] non-difficult boxes per class (:139); cls_off_out int64 [ncls + 1] class ranges of
+ * the per-detection arrays; order_out int32 [nd] input index of each position (class ascending, score descending, equal
+ * scores in input order - a stable sort where the reference's np.argsort is not); rec_out / prec_out fp64 [nd] (:239-245,
+ * bit-identical); ap_out fp64 [ncls] voc_ap (:53-84; the area metric sums its terms in a fixed order of its own).
+ * Matching is the reference's: the "+1 pixel" AABB prefilter (:176-205), iou_poly(gt, det) in fp64 (:211), numpy max /
+ * argmax (a NaN candidate makes the detection a false positive), no fall back to the next-best box (:222-230).  A class
+ * without detections gets an empty range and ap = voc_ap([], []) = 0. */
+int orp_dota_eval_task1(const int32_t *det_cls, const int32_t *det_img, const double *det_score, const double *det_quad,
+                        int nd, const int32_t *gt_cls, const int32_t *gt_img, const double *gt_quad,
+                        const uint8_t *gt_difficult, int ng, int ncls, int nimg, double ovthresh, int use_07_metric,
+                        const double *thresholds11, int64_t *npos_out, int64_t *cls_off_out, int32_t *order_out,
+                        double *rec_out, double *prec_out, double *ap_out, void *stream);
+
+/* ------------------------------------------------------------------------------------------
  * Dense layers, fp32 (CUDA cores) - the parity arithmetic of the backbone / FPN / head
  * All activations are NHWC ("channels last") contiguous device tensors; weights are
  * [Cout][KH][KW][Cin] (the reference's [Cout][Cin][KH][KW] permuted once at load time).

@@ -119,6 +119,8 @@ SIGNATURES = {
     "orp_stem_im2col_bf16": (_i, [_vp, _i, _i, _i, _vp, _vp]),
     "orp_stem_s2d_bf16": (_i, [_vp, _i, _i, _i, _vp, _vp]),
     "orp_convex_iou": (_i, [_vp, _i, _vp, _i, _vp, _vp]),
+    "orp_dota_eval_task1": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _d, _i, _vp, _vp, _vp, _vp, _vp,
+                                 _vp, _vp, _vp]),
     "orp_split_tiles_u8": (_i, [_vp, _i, _i, _i, _vp, _i, _i, _vp, _vp]),
     "orp_resize_u8": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
     "orp_stem_s2d_u8_padded_bf16": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, _vp, _vp, _vp]),
