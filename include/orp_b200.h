@@ -284,15 +284,20 @@ int orp_dota_eval_task1(const int32_t *det_cls, const int32_t *det_img, const do
                         double *rec_out, double *prec_out, double *ap_out, void *stream);
 
 /* ------------------------------------------------------------------------------------------
- * Dense layers, fp32 (CUDA cores) - the parity arithmetic of the backbone / FPN / head
+ * Dense layers, fp32 (CUDA cores) - the reference's fp32 arithmetic of the backbone / FPN / head
  * All activations are NHWC ("channels last") contiguous device tensors; weights are
  * [Cout][KH][KW][Cin] (the reference's [Cout][Cin][KH][KW] permuted once at load time).
+ * ReLU and max-pool propagate NaN (nn.ReLU / nn.MaxPool2d).  Arguments outside the ranges stated
+ * below return ORP_EINVAL before anything is launched.
  * ---------------------------------------------------------------------------------------- */
 
 /* y = relu?( conv(x, w) + bias + residual ), optionally accumulating the GroupNorm statistics of y:
  * gn_stats is device double [N, groups, 2] (sum, sum of squares), must be zeroed by the caller.
  * Replaces nn.Conv2d / ConvModule.conv (mmdet/ops/conv_module.py:124-132) on the cuDNN path; with
- * eval-mode BatchNorm folded into w and bias beforehand (the fold of tools/fuse_conv_bn.py:10-24). */
+ * eval-mode BatchNorm folded into w and bias beforehand (the fold of tools/fuse_conv_bn.py:10-24).
+ * Accepted: x, w, y non-NULL; N, H, W, Cout, KH, KW >= 1; Cin >= 1 and a multiple of 4; stride >= 1,
+ * pad >= 0; Ho = (H + 2 pad - KH) / stride + 1 >= 1 and Wo likewise (the kernel fits the padded input);
+ * with gn_stats: groups >= 1 dividing Cout.  bias, residual [N,Ho,Wo,Cout] and gn_stats may be NULL. */
 int orp_conv2d_f32(const float *x, int N, int H, int W, int Cin, const float *w, int Cout, int KH, int KW,
                    int stride, int pad, const float *bias, const float *residual, int relu, float *y,
                    double *gn_stats, int groups, void *stream);
@@ -303,19 +308,24 @@ int orp_conv2d_f32(const float *x, int N, int H, int W, int Cin, const float *w,
  * sampling per deformable_im2col_bilinear (deform_conv_cuda_kernel.cu:84-115), validity test of :229.
  *   offset  device float32 [N, Ho, Wo, 2*KH*KW], channel 2t = dy, 2t+1 = dx of tap t (:222-225)
  *   mask    device float32 [N, Ho, Wo, KH*KW] or NULL
- * Cin must be a multiple of 4 (float4 channel loads); callers zero-pad x and w to it. */
+ * Cin must be a multiple of 4 (float4 channel loads); callers zero-pad x and w to it.
+ * Accepted: as orp_conv2d_f32, plus offset non-NULL and dilation >= 1; Ho / Wo count the dilated kernel
+ * (H + 2 pad - dilation (KH - 1) - 1) / stride + 1. */
 int orp_deform_conv2d_f32(const float *x, int N, int H, int W, int Cin, const float *offset, const float *mask,
                           const float *w, int Cout, int KH, int KW, int stride, int pad, int dilation,
                           const float *bias, int relu, float *y, void *stream);
 
 /* GroupNorm apply: y = relu?( (x - mean) * rstd * gamma + beta ) (+ nearest-2x upsampled up_src,
  * the FPN top-down add of mmdet/models/necks/fpn.py:150-154).  stats as produced by orp_conv2d_f32;
- * biased variance and eps as torch.nn.GroupNorm (mmdet/ops/norm.py:42-50). */
+ * biased variance and eps as torch.nn.GroupNorm (mmdet/ops/norm.py:42-50).
+ * Accepted: x, stats, gamma, beta, y non-NULL; N, H, W >= 1; C >= 1 and a multiple of 4; groups >= 1
+ * dividing C.  up_src (NULL or [N, ceil(H/2), ceil(W/2), C]) is read as F.interpolate(nearest) to H x W. */
 int orp_gn_apply_f32(const float *x, int N, int H, int W, int C, const double *stats, int groups,
                      const float *gamma, const float *beta, float eps, int relu, const float *up_src, float *y,
                      void *stream);
 
-/* nn.MaxPool2d(kernel_size=3, stride=2, padding=1) of the ResNet stem (resnet.py:497) */
+/* nn.MaxPool2d(kernel_size=3, stride=2, padding=1) of the ResNet stem (resnet.py:497): y [N, (H+1)/2, (W+1)/2, C].
+ * Accepted: x, y non-NULL; N, H, W >= 1; C >= 1 and a multiple of 4. */
 int orp_maxpool3x3s2_f32(const float *x, int N, int H, int W, int C, float *y, void *stream);
 
 /* ------------------------------------------------------------------------------------------

@@ -1,22 +1,26 @@
 // dense_f32.cu - fp32 (CUDA-core) dense layers of the OrientedRepPoints inference path, NHWC.
 //
-// This is the PARITY arithmetic of the dense path: plain fp32 multiply-adds like the reference's
-// fp32 cuDNN/cuBLAS convolutions (mmdet/models/backbones/resnet.py:203-239,495-506,
+// The CUDA-core mirror of the reference's fp32 arithmetic: plain fp32 multiply-adds like its fp32
+// cuDNN/cuBLAS convolutions (mmdet/models/backbones/resnet.py:203-239,495-506,
 // necks/fpn.py:138-178, anchor_heads/orientedreppoints_head.py:148-171) and its deformable im2col +
 // SGEMM (mmdet/ops/dcn/src/deform_conv_cuda_kernel.cu:84-115,190-243, deform_conv_cuda.cpp:152-260).
-// The bf16 wgmma kernels in dense_tc.cu compute the same layers on the tensor pipe; tests compare
-// the two against each other and against a PyTorch fp32 re-declaration of the reference graph.
+// ReLU and max-pool propagate NaN as nn.ReLU / nn.MaxPool2d do.  It is the detector's default
+// precision and the reference engine of several GPU tests; the benchmarked parity arithmetic is
+// f16x3 on the tensor cores (dense_tc.cu), which tests compare with this engine and with fp64.
 //
 // One implicit-GEMM kernel serves ordinary and deformable convolutions: M = output pixels of one
 // image (tiles never straddle images), N = output channels, K = taps x input channels; the
 // deformable variant replaces the A-operand load by the reference's 4-corner bilinear sample, so
 // the 151 MB `columns` scratch of the reference (2304 x H*W floats at stride 8) never exists.
 // Epilogue fuses bias, residual add, ReLU and the per-(image, group) sum / sum-of-squares that
-// GroupNorm needs (double-precision atomics, 2 x groups per CTA).
+// GroupNorm needs (fp32 partials per thread and per CTA, added across CTAs with double atomics).
 #include "common.cuh"
 
 namespace orp {
 namespace {
+
+// max(a, b) that returns a NaN operand, as torch's max-pool and ReLU do (fmaxf drops it)
+__device__ __forceinline__ float max_nan(float a, float b) { return (a > b || a != a) ? a : b; }
 
 struct ConvP {
     const float *x, *w, *bias, *res, *off, *mask;
@@ -175,7 +179,7 @@ conv_f32_kernel(ConvP p)
         }
         if (p.relu) {
 #pragma unroll
-            for (int j = 0; j < 4; ++j) v[j] = fmaxf(v[j], 0.f);
+            for (int j = 0; j < 4; ++j) v[j] = max_nan(v[j], 0.f);
         }
         if (vec_ok) {
             *reinterpret_cast<float4 *>(p.y + base) = make_float4(v[0], v[1], v[2], v[3]);
@@ -227,7 +231,7 @@ gn_apply_f32_kernel(const float *__restrict__ x, int N, int H, int W, int C, con
             var = var < 0 ? 0 : var;
             const float rstd = (float)(1.0 / sqrt(var + (double)eps));
             o[j] = (o[j] - (float)mean) * rstd * gamma[c + j] + beta[c + j];
-            if (relu) o[j] = fmaxf(o[j], 0.f);
+            if (relu) o[j] = max_nan(o[j], 0.f);
         }
         if (up) {
             const int hw = (int)(pix % ((size_t)H * W));
@@ -258,26 +262,38 @@ maxpool3x3s2_f32_kernel(const float *__restrict__ x, int N, int H, int W, int C,
                 const int ih = oh * 2 - 1 + dh, iw = ow * 2 - 1 + dw;
                 if (ih < 0 || ih >= H || iw < 0 || iw >= W) continue;
                 const float4 v = *reinterpret_cast<const float4 *>(x + (((size_t)n * H + ih) * W + iw) * C + c);
-                m.x = fmaxf(m.x, v.x); m.y = fmaxf(m.y, v.y); m.z = fmaxf(m.z, v.z); m.w = fmaxf(m.w, v.w);
+                m.x = max_nan(v.x, m.x); m.y = max_nan(v.y, m.y); m.z = max_nan(v.z, m.z); m.w = max_nan(v.w, m.w);
             }
         reinterpret_cast<float4 *>(y)[i] = m;
     }
 }
 
-int conv_common(const float *x, int N, int H, int W, int Cin, const float *w, int Cout, int KH, int KW, int stride,
-                int pad, int dil, const float *bias, const float *res, int relu, float *y, double *stats, int groups,
-                const float *off, const float *mask, cudaStream_t st)
+// output extent of a convolution: (in + 2 pad - dil (k - 1) - 1) / stride + 1, or 0 when the dilated kernel does not
+// fit the padded input (C division truncates toward zero, so a small negative span would otherwise give 1)
+int conv_out_extent(int in, int k, int stride, int pad, int dil)
 {
-    if (N <= 0 || H <= 0 || W <= 0 || Cin <= 0 || Cout <= 0 || !x || !w || !y) return fail(ORP_EINVAL, "conv2d_f32: bad arguments");
-    if (Cin % 4) return fail(ORP_EINVAL, "conv2d_f32: Cin must be a multiple of 4 (pad the stem input to 4 channels)");
-    if (stats && (groups <= 0 || Cout % groups)) return fail(ORP_EINVAL, "conv2d_f32: Cout must divide into groups");
+    const long long span = (long long)in + 2LL * pad - (long long)dil * (k - 1) - 1;
+    return span < 0 ? 0 : (int)(span / stride + 1);
+}
+
+int conv_common(const char *name, const float *x, int N, int H, int W, int Cin, const float *w, int Cout, int KH, int KW,
+                int stride, int pad, int dil, const float *bias, const float *res, int relu, float *y, double *stats,
+                int groups, const float *off, const float *mask, cudaStream_t st)
+{
+    if (!x || !w || !y) return fail(ORP_EINVAL, "%s: x, w and y must not be NULL", name);
+    if (N < 1 || H < 1 || W < 1 || Cin < 1 || Cout < 1 || KH < 1 || KW < 1)
+        return fail(ORP_EINVAL, "%s: N, H, W, Cin, Cout, KH and KW must be >= 1", name);
+    if (stride < 1 || dil < 1 || pad < 0) return fail(ORP_EINVAL, "%s: stride and dilation must be >= 1, pad >= 0", name);
+    if (Cin % 4) return fail(ORP_EINVAL, "%s: Cin must be a multiple of 4 (pad the stem input to 4 channels)", name);
+    const int Ho = conv_out_extent(H, KH, stride, pad, dil), Wo = conv_out_extent(W, KW, stride, pad, dil);
+    if (Ho < 1 || Wo < 1) return fail(ORP_EINVAL, "%s: the kernel does not fit the padded input (empty output)", name);
+    if (stats && (groups < 1 || Cout % groups)) return fail(ORP_EINVAL, "%s: Cout must divide into groups >= 1", name);
     int rc = ensure_device();
     if (rc) return rc;
     ConvP p;
     p.x = x; p.w = w; p.bias = bias; p.res = res; p.off = off; p.mask = mask; p.y = y; p.stats = stats;
     p.N = N; p.H = H; p.W = W; p.Cin = Cin; p.Cout = Cout; p.KH = KH; p.KW = KW; p.stride = stride; p.pad = pad; p.dil = dil;
-    p.Ho = (H + 2 * pad - dil * (KH - 1) - 1) / stride + 1;
-    p.Wo = (W + 2 * pad - dil * (KW - 1) - 1) / stride + 1;
+    p.Ho = Ho; p.Wo = Wo;
     p.K = KH * KW * Cin; p.relu = relu; p.groups = groups;
     p.tiles_per_img = ceil_div((long long)p.Ho * p.Wo, BM);
     dim3 grid(N * p.tiles_per_img, ceil_div(Cout, BN));
@@ -296,8 +312,8 @@ extern "C" int orp_conv2d_f32(const float *x, int N, int H, int W, int Cin, cons
                               int stride, int pad, const float *bias, const float *residual, int relu, float *y,
                               double *gn_stats, int groups, void *stream)
 {
-    return conv_common(x, N, H, W, Cin, w, Cout, KH, KW, stride, pad, 1, bias, residual, relu, y, gn_stats, groups,
-                       nullptr, nullptr, static_cast<cudaStream_t>(stream));
+    return conv_common("conv2d_f32", x, N, H, W, Cin, w, Cout, KH, KW, stride, pad, 1, bias, residual, relu, y, gn_stats,
+                       groups, nullptr, nullptr, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int orp_deform_conv2d_f32(const float *x, int N, int H, int W, int Cin, const float *offset, const float *mask,
@@ -305,15 +321,18 @@ extern "C" int orp_deform_conv2d_f32(const float *x, int N, int H, int W, int Ci
                                      const float *bias, int relu, float *y, void *stream)
 {
     if (!offset) return fail(ORP_EINVAL, "deform_conv2d_f32: offset is NULL");
-    return conv_common(x, N, H, W, Cin, w, Cout, KH, KW, stride, pad, dilation, bias, nullptr, relu, y, nullptr, 0, offset,
-                       mask, static_cast<cudaStream_t>(stream));
+    return conv_common("deform_conv2d_f32", x, N, H, W, Cin, w, Cout, KH, KW, stride, pad, dilation, bias, nullptr, relu, y,
+                       nullptr, 0, offset, mask, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int orp_gn_apply_f32(const float *x, int N, int H, int W, int C, const double *stats, int groups,
                                 const float *gamma, const float *beta, float eps, int relu, const float *up_src, float *y,
                                 void *stream)
 {
-    if (!x || !y || !stats || !gamma || !beta || C % 4 || C % groups) return fail(ORP_EINVAL, "gn_apply_f32: bad arguments");
+    if (!x || !y || !stats || !gamma || !beta) return fail(ORP_EINVAL, "gn_apply_f32: x, stats, gamma, beta and y must not be NULL");
+    if (N < 1 || H < 1 || W < 1 || C < 1) return fail(ORP_EINVAL, "gn_apply_f32: N, H, W and C must be >= 1");
+    if (C % 4) return fail(ORP_EINVAL, "gn_apply_f32: C must be a multiple of 4");
+    if (groups < 1 || C % groups) return fail(ORP_EINVAL, "gn_apply_f32: C must divide into groups >= 1");
     int rc = ensure_device();
     if (rc) return rc;
     const size_t total4 = (size_t)N * H * W * C / 4;
@@ -327,7 +346,9 @@ extern "C" int orp_gn_apply_f32(const float *x, int N, int H, int W, int C, cons
 
 extern "C" int orp_maxpool3x3s2_f32(const float *x, int N, int H, int W, int C, float *y, void *stream)
 {
-    if (!x || !y || C % 4) return fail(ORP_EINVAL, "maxpool3x3s2_f32: bad arguments");
+    if (!x || !y) return fail(ORP_EINVAL, "maxpool3x3s2_f32: x and y must not be NULL");
+    if (N < 1 || H < 1 || W < 1 || C < 1) return fail(ORP_EINVAL, "maxpool3x3s2_f32: N, H, W and C must be >= 1");
+    if (C % 4) return fail(ORP_EINVAL, "maxpool3x3s2_f32: C must be a multiple of 4");
     int rc = ensure_device();
     if (rc) return rc;
     const int Ho = (H + 2 - 3) / 2 + 1, Wo = (W + 2 - 3) / 2 + 1;
