@@ -260,6 +260,53 @@ int orp_dcn_offsets_multi(int nprob, const float *const *pts, float *const *off,
                           float gradient_mul, const float *base18, void *stream);
 
 /* ------------------------------------------------------------------------------------------
+ * DOTA ResultMerge
+ * ---------------------------------------------------------------------------------------- */
+
+/* bits of orp_result_merge's status word; when it is not 0 the other outputs are not a merge result */
+#define ORP_MERGE_BAD_COUNT 1      /* a selected slot's count is not an integer in [0, cap] (-1 is the NMS overflow mark of
+                                      orp_head_postprocess: such a tile is never taken for an empty one), or the rest of its
+                                      count row is not the zero padding of orp_pack_detections                             */
+#define ORP_MERGE_BAD_TILE 2       /* a tile's slot >= S, its rate is not a positive finite number, or its image is outside
+                                      [0, nimg)                                                                            */
+#define ORP_MERGE_ROWS_OVERFLOW 4  /* the selected slots hold more labelled rows than max_rows                            */
+
+/* ResultMerge over the packed detections: tile coordinates back to the original image, poly NMS per original image and
+ * class, survivors in the order of the merged Task1 files.  Replaces the Task1 writer of
+ * tools/parse_pkl/parse_pkl_mege_results_for_dota_evaluation.py:93-192 and mergesingle with poly2origpoly and nmsbynamedict
+ * (DOTA_devkit/ResultMerge_multi_process.py:156-223) without the text files between them.  Device pointers, asynchronous.
+ *   packed     device fp32 [S, cap + 1, 28], the layout of orp_pack_detections (the all-gather's [world, T, cap + 1, 28]
+ *              buffer is this with S = world * T)
+ *   tile_slot  device int32 [Tn]: the slot of `packed` that holds dataset tile i; negative: the tile is skipped.  Rows are
+ *              numbered in dataset tile order, then in-tile order (the line order of the text path within a class); ties
+ *              in score and the order of the images follow that numbering
+ *   tile_xy    device int32 [Tn, 2] (left, up); tile_rate device fp64 [Tn]; tile_img device int32 [Tn] original image in
+ *              [0, nimg)
+ *   thresh, union_mode: ORP_UNION_NAN_SUPPRESSES is py_cpu_nms_poly_fast (what mergesingle uses, :60-121),
+ *              ORP_UNION_NAN_SUPPRESSES_ALL py_cpu_nms_poly (ResultMerge.py:18-41); other modes are ORP_EINVAL
+ *   max_rows   capacity of the per-survivor outputs and the size the NMS is planned for: at least the number of rows with
+ *              a label in [0, ncls) in the selected slots (the sum of their counts is a bound; Tn * cap always is).  The
+ *              counts are not read back: when the rows outnumber max_rows, ORP_MERGE_ROWS_OVERFLOW is set on the device
+ * A row is restored as poly2origpoly does, q = ((double)p + x) / rate with both operations rounded on their own; its score is
+ * (double)score; a row whose label is not an integer in [0, ncls) is dropped.  The NMS is orp_rnms's ORP_NMS_EXACT64 in
+ * score-descending order over segments class * nimg + image, on fp32 rows translated in fp64 to floor(min x), floor(min y)
+ * of the segment's finite restored coordinates (0 when it has none).  A row with a non-finite coordinate is kept and
+ * suppresses nothing, as orp_rnms treats such a box.
+ * Outputs (device): status_out int32 [1] (ORP_MERGE_* bits, 0: success); count_out int32 [1] survivors; cls_off_out int64
+ * [ncls + 1] class ranges; per survivor cls_out / img_out int32 [max_rows], score_out fp64 [max_rows], quad_out fp64
+ * [max_rows, 8] (the restored doubles), src_row_out int32 [max_rows] (the row number before the merge); entries past
+ * count_out are unspecified.  Order: class ascending, then original image by first appearance among the class's rows, then
+ * score descending with equal scores in row order - the det_* arrays orp_dota_eval_task1 reads.
+ * No N x N memory; the call makes at most one host synchronise, the candidate-list check of the NMS.  Sizes that a host can
+ * check (S, Tn, max_rows < 0, cap < 1, ncls < 1, nimg < 1, Tn * cap >= 2^31 - 1, null pointers, union_mode, NaN thresh) return ORP_EINVAL before
+ * any CUDA call. */
+int orp_result_merge(const float *packed, int S, int cap, const int32_t *tile_slot, const int32_t *tile_xy,
+                     const double *tile_rate, const int32_t *tile_img, int Tn, int ncls, int nimg, double thresh,
+                     int union_mode, int max_rows, int32_t *count_out, int64_t *cls_off_out, int32_t *cls_out,
+                     int32_t *img_out, double *score_out, double *quad_out, int32_t *src_row_out, int32_t *status_out,
+                     void *stream);
+
+/* ------------------------------------------------------------------------------------------
  * DOTA Task1 evaluation
  * ---------------------------------------------------------------------------------------- */
 

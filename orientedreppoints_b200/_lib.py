@@ -12,6 +12,7 @@ LIB_PATH = os.path.join(_HERE, "lib", "liborp_b200.so")
 ORP_NMS_EXACT64, ORP_NMS_COMPAT32 = 0, 1
 ORP_UNION_NAN_KEEPS, ORP_UNION_GUARD, ORP_UNION_NAN_SUPPRESSES, ORP_UNION_NAN_SUPPRESSES_ALL = 0, 1, 2, 3
 ORP_ORDER_INDEX_ASC, ORP_ORDER_SCORE_DESC = 0, 1
+ORP_MERGE_BAD_COUNT, ORP_MERGE_BAD_TILE, ORP_MERGE_ROWS_OVERFLOW = 1, 2, 4
 
 _vp = ctypes.c_void_p
 _i = ctypes.c_int
@@ -121,6 +122,8 @@ SIGNATURES = {
     "orp_convex_iou": (_i, [_vp, _i, _vp, _i, _vp, _vp]),
     "orp_dota_eval_task1": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _d, _i, _vp, _vp, _vp, _vp, _vp,
                                  _vp, _vp, _vp]),
+    "orp_result_merge": (_i, [_vp, _i, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _d, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                              _vp]),
     "orp_split_tiles_u8": (_i, [_vp, _i, _i, _i, _vp, _i, _i, _vp, _vp]),
     "orp_resize_u8": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
     "orp_stem_s2d_u8_padded_bf16": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, _vp, _vp, _vp]),

@@ -162,6 +162,45 @@ def evaluate(dets, gts, classnames=DOTA_CLASSES, ovthresh=0.5, use_07_metric=Tru
     return res
 
 
+def evaluate_merged(merged, gts, image_names, classnames=DOTA_CLASSES, ovthresh=0.5, use_07_metric=True):
+    """`evaluate` over result_merge.MergedDetections (merge_packed, detect_image_tensors): the same dict, with nothing
+    parsed and no detection uploaded - the merge's tensors go to orp_dota_eval_task1 as they are.
+      image_names  name of every image id of the merge.  The ids are mapped to the positions in `gts` on the device; an
+                   image that carries a detection must be a key of `gts` (KeyError, as for a detection line of an unknown
+                   image), one without detections need not be
+      classnames   the merge's classes, in its class order
+    'order' indexes each class's merged rows, i.e. the lines of `merged.to_lines(image_names, classnames)`."""
+    classnames = tuple(classnames)
+    if len(classnames) != merged.ncls or len(image_names) != merged.nimg:
+        raise ValueError("evaluate_merged: %d class names and %d image names expected" % (merged.ncls, merged.nimg))
+    arrays, nimg, _ = _host_arrays({}, gts, classnames)
+    img_index = {name: i for i, name in enumerate(gts)}
+    dev = merged.cls.device
+    missing = [i for i, name in enumerate(image_names) if name not in img_index]
+    if missing and len(merged):
+        hit = torch.isin(merged.img, torch.tensor(missing, dtype=torch.int32, device=dev)).nonzero()
+        if hit.numel():
+            raise KeyError(image_names[int(merged.img[hit[0, 0]])])
+    lut = torch.tensor([img_index.get(name, -1) for name in image_names], dtype=torch.int32).to(dev)
+    inputs = [merged.cls.contiguous(), lut[merged.img.long()].contiguous(), merged.score.contiguous(),
+              merged.quad.contiguous()] + [torch.from_numpy(np.ascontiguousarray(a)).to(dev) for a in arrays[4:]]
+    buf, offs = _launch(inputs, len(classnames), nimg, ovthresh, use_07_metric, dev)
+    out = buf.cpu().numpy()                                                           # the one copy back
+    npos, cls_off, rec, prec, ap, order = (out[offs[k]:offs[k + 1]].view(t) for k, t in enumerate(_OUT_DTYPES))
+    res = {'rec': {}, 'prec': {}, 'ap': {}, 'npos': {}, 'order': {}}
+    total = 0
+    for c, cname in enumerate(classnames):
+        sl = slice(int(cls_off[c]), int(cls_off[c + 1]))
+        res['rec'][cname] = rec[sl].copy()
+        res['prec'][cname] = prec[sl].copy()
+        res['ap'][cname] = float(ap[c])
+        res['npos'][cname] = int(npos[c])
+        res['order'][cname] = order[sl].astype(np.int64) - sl.start     # the merge is sorted by class: a class's rows start at cls_off
+        total = total + res['ap'][cname]
+    res['map'] = total / len(classnames)
+    return res
+
+
 def voc_eval(detpath, annopath, imagesetfile, classname, ovthresh=0.5, use_07_metric=False):
     """rec, prec, ap of one class from files: detpath.format(classname) holds its Task1 lines, annopath.format(name)
     the label file of every image listed in imagesetfile"""

@@ -148,3 +148,98 @@ def write_task1_raw(results, tile_names, class_names, outdir):
     finally:
         for f in files:
             f.close()
+
+
+# --------------------------------------------------------------------------------------------------------------------
+# The same merge over the packed detection buffer (gather.pack / gather.all_gather_detections), without the text
+# --------------------------------------------------------------------------------------------------------------------
+
+class MergedDetections:
+    """Survivors of `merge_packed`, device resident and trimmed to their count, in the order of the merged Task1 files
+    (class ascending; original image by first appearance among the class's rows; score descending, ties in row order):
+      cls, img  int32 [n]    class and original-image id
+      score     fp64 [n]     the fp32 score widened
+      quad      fp64 [n, 8]  x1 y1 ... x4 y4 in original-image coordinates (the doubles poly2origpoly gives)
+      src_row   int32 [n]    row number before the merge (dataset tile order, then in-tile order; unlabelled rows left out)
+      cls_off   int64 [ncls + 1] range of every class
+    These are the detection arrays orp_dota_eval_task1 reads (`evaluation.evaluate_merged`)."""
+
+    def __init__(self, cls, img, score, quad, src_row, cls_off, nimg):
+        self.cls, self.img, self.score, self.quad, self.src_row, self.cls_off = cls, img, score, quad, src_row, cls_off
+        self.nimg, self.ncls = int(nimg), int(cls_off.shape[0]) - 1
+
+    def __len__(self):
+        return int(self.cls.shape[0])
+
+    def to_lines(self, image_names, class_names):
+        """{class name: [`imgname score x1 y1 x2 y2 x3 y3 x4 y4`, ...]}: string for string what `merge_lines` returns for
+        the same detections (python float formatting of the doubles); image_names[i] is the name of image id i"""
+        if len(image_names) != self.nimg or len(class_names) != self.ncls:
+            raise ValueError("to_lines: %d image names and %d class names expected" % (self.nimg, self.ncls))
+        off = self.cls_off.tolist()
+        img, score, quad = self.img.tolist(), self.score.tolist(), self.quad.tolist()
+        return {cname: [image_names[img[k]] + ' ' + str(score[k]) + ' ' + ' '.join(map(str, quad[k]))
+                        for k in range(off[c], off[c + 1])] for c, cname in enumerate(class_names)}
+
+    def write_task1(self, outdir, image_names, class_names):
+        """the merged submission files `Task1_<class>.txt` (what mergebypoly writes), one per class, empty ones included"""
+        os.makedirs(outdir, exist_ok=True)
+        for cname, lines in self.to_lines(image_names, class_names).items():
+            with open(os.path.join(outdir, 'Task1_%s.txt' % cname), 'w') as f:
+                for line in lines:
+                    f.write(line + '\n')
+
+
+def merge_packed(packed, tile_slot, tile_xy, tile_rate, tile_img, nimg, ncls=15, thresh=None, plain=False, max_rows=None):
+    """ResultMerge of packed detections in one device call (orp_result_merge) -> MergedDetections.
+      packed     device fp32 [S, cap + 1, 28] from gather.pack, or the all-gather's [world, T, cap + 1, 28] as
+                 gather.all_gather_detections(buf, packed=True) returns it.  The LAST row of every slot must be its count row:
+                 the (all_buf, all_counts) pair that all_gather_detections returns by default has it cut off and is not an
+                 input of this call (a count row with anything but zeros after the count is refused)
+      tile_slot  int32 [Tn]: slot of `packed` (flattened over world, T) holding dataset tile i, negative to skip it
+                 (gather.dataset_slots for the all-gather's layout, arange for a dataset-order buffer)
+      tile_xy    int32 [Tn, 2] (left, up); tile_rate fp64 [Tn]; tile_img int32 [Tn] original image in [0, nimg)
+                 (tiles of several rates of one image share its id); tensors or array-likes, uploaded when on the host
+      plain      py_cpu_nms_poly (every pair compared) instead of py_cpu_nms_poly_fast, which mergesingle uses
+      max_rows   bound on the rows to merge.  None reads the sum of the selected counts (one scalar) to size the call;
+                 the trimmed result costs one more read of the survivor count and status: two host reads in all.  A
+                 caller that passes a bound (Tn * cap always is one) saves the first, but the NMS is then planned, and its
+                 scratch allocated, for the bound, so a loose one costs more than the read.
+    A slot whose count is the NMS-overflow mark of orp_head_postprocess (-1), a slot outside the buffer, a rate <= 0 or an
+    image id outside [0, nimg) raise OrpError: such a tile is never merged as an empty one."""
+    if packed.dim() == 4:
+        packed = packed.reshape(-1, packed.shape[2], packed.shape[3])
+    if not packed.is_cuda or packed.dtype != torch.float32 or packed.dim() != 3 or packed.shape[2] != 28 or packed.shape[1] < 2:
+        raise ValueError("merge_packed: a CUDA float32 [S, cap + 1, 28] buffer expected")
+    dev = packed.device
+    packed = packed.contiguous()
+    s, cap = int(packed.shape[0]), int(packed.shape[1]) - 1
+    slot = torch.as_tensor(tile_slot, dtype=torch.int32).reshape(-1).to(dev).contiguous()
+    tn = int(slot.shape[0])
+    xy = torch.as_tensor(tile_xy, dtype=torch.int32).reshape(tn, 2).to(dev).contiguous()
+    rate = torch.as_tensor(tile_rate, dtype=torch.float64).reshape(tn).to(dev).contiguous()
+    img = torch.as_tensor(tile_img, dtype=torch.int32).reshape(tn).to(dev).contiguous()
+    if max_rows is None:
+        sel = slot[(slot >= 0) & (slot < s)].long()
+        max_rows = int(packed[sel, cap, 0].nan_to_num(0.0).clamp(0, cap).sum(dtype=torch.float64).item()) if tn else 0
+    max_rows = int(max_rows)
+    head = torch.empty(2, dtype=torch.int32, device=dev)                      # survivor count, status
+    cls_off = torch.empty(ncls + 1, dtype=torch.int64, device=dev)
+    o_cls, o_img, o_row = (torch.empty(max_rows, dtype=torch.int32, device=dev) for _ in range(3))
+    o_score = torch.empty(max_rows, dtype=torch.float64, device=dev)
+    o_quad = torch.empty((max_rows, 8), dtype=torch.float64, device=dev)
+    mode = _lib.ORP_UNION_NAN_SUPPRESSES_ALL if plain else _lib.ORP_UNION_NAN_SUPPRESSES
+    with torch.cuda.device(dev):
+        rc = _lib.lib().orp_result_merge(
+            _lib.ptr(packed), s, cap, _lib.ptr(slot), _lib.ptr(xy), _lib.ptr(rate), _lib.ptr(img), tn, int(ncls), int(nimg),
+            float(nms_thresh if thresh is None else thresh), mode, max_rows, _lib.ptr(head[0:1]), _lib.ptr(cls_off),
+            _lib.ptr(o_cls), _lib.ptr(o_img), _lib.ptr(o_score), _lib.ptr(o_quad), _lib.ptr(o_row), _lib.ptr(head[1:2]),
+            _lib.current_stream_ptr())
+    _lib.check(rc, "orp_result_merge")
+    n, status = head.tolist()
+    if status:
+        why = [text for bit, text in ((_lib.ORP_MERGE_BAD_COUNT, "a tile's count is not in [0, cap] (-1: its NMS overflowed)"),
+                                      (_lib.ORP_MERGE_BAD_TILE, "a tile's slot, rate or image id is out of range"),
+                                      (_lib.ORP_MERGE_ROWS_OVERFLOW, "more rows than max_rows")) if status & bit]
+        raise _lib.OrpError("orp_result_merge refused its input: " + "; ".join(why))
+    return MergedDetections(o_cls[:n], o_img[:n], o_score[:n], o_quad[:n], o_row[:n], cls_off, nimg)

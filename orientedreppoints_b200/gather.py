@@ -32,36 +32,42 @@ def pack(dets, labels, counts):
 
 
 class _Gathered:
-    """result of all_gather_detections(async_op=True): wait() -> (all_buf [world,T,cap,28], all_counts [world,T])"""
+    """result of all_gather_detections(async_op=True): wait() -> (all_buf [world,T,cap,28], all_counts [world,T]), or the
+    whole [world,T,cap+1,28] buffer when the gather was asked for it (packed=True)"""
 
-    def __init__(self, all_buf, work):
-        self._all_buf, self._work = all_buf, work
+    def __init__(self, all_buf, work, packed=False):
+        self._all_buf, self._work, self._packed = all_buf, work, packed
 
     def wait(self):
         if self._work is not None:
             self._work.wait()            # NCCL: the current stream waits for the collective; gloo: the host does
             self._work = None
+        if self._packed:
+            return self._all_buf
         cap = self._all_buf.shape[2] - 1
         return self._all_buf[:, :, :cap], self._all_buf[:, :, cap, 0].to(torch.int32)
 
 
-def all_gather_detections(buf, counts=None, group=None, async_op=False):
+def all_gather_detections(buf, counts=None, group=None, async_op=False, packed=False):
     """buf from pack() -> (all_buf [world,T,cap,28], all_counts [world,T]) with ONE all_gather_into_tensor.
+    packed=True returns the gathered buffer as it is instead, [world,T,cap+1,28] with every tile's count row still in
+    place: the input of dota.result_merge.merge_packed (with dataset_slots), which must not be given the split pair's
+    all_buf - without the count row a tile's last detection row would be read as its count.
     async_op=True returns a handle whose wait() gives the same pair: the collective then overlaps whatever the caller
     launches next (ranks are not forced into lockstep every step)."""
     world = dist.get_world_size(group) if dist.is_initialized() else 1
     if world == 1:
-        h = _Gathered(buf.unsqueeze(0), None)
+        h = _Gathered(buf.unsqueeze(0), None, packed)
         return h if async_op else h.wait()
     if buf.is_cuda:
         all_buf = torch.empty((world,) + tuple(buf.shape), dtype=buf.dtype, device=buf.device)
         work = dist.all_gather_into_tensor(all_buf, buf.contiguous(), group=group, async_op=True)
-        h = _Gathered(all_buf, work)
+        h = _Gathered(all_buf, work, packed)
     else:   # gloo (CPU tests)
         lb = [torch.empty_like(buf) for _ in range(world)]
         work = dist.all_gather(lb, buf, group=group, async_op=True)
         work.wait()
-        h = _Gathered(torch.stack(lb), None)
+        h = _Gathered(torch.stack(lb), None, packed)
     return h if async_op else h.wait()
 
 
@@ -75,3 +81,11 @@ def interleave(all_buf, all_counts, dataset_len):
         rows = all_buf[r, s, :k]
         out.append((rows[:, :27], rows[:, 27].long()))
     return out
+
+
+def dataset_slots(world, t, dataset_len):
+    """int32 [min(dataset_len, world * t)]: for dataset tile i, its slot in the all-gather's buffer flattened to
+    [world * t, cap + 1, 28] - rank i % world, slot i // world, as `interleave` reads it; the sampler's padding tiles
+    (indices >= dataset_len) are left out.  This is the `tile_slot` of dota.result_merge.merge_packed."""
+    i = torch.arange(min(int(dataset_len), int(world) * int(t)), dtype=torch.int32)
+    return (i % world) * t + torch.div(i, world, rounding_mode='floor')
