@@ -330,6 +330,30 @@ int orp_dota_eval_task1(const int32_t *det_cls, const int32_t *det_img, const do
                         const double *thresholds11, int64_t *npos_out, int64_t *cls_off_out, int32_t *order_out,
                         double *rec_out, double *prec_out, double *ap_out, void *stream);
 
+/* poly2rbox_single_v3 (DOTA_devkit/dota_poly2rbox.py:128-190) of n quads, device pointers, asynchronous.
+ *   quad  device fp64 [n, 8] x1 y1 ... x4 y4;  out  device fp64 [n, 5] (x_ctr, y_ctr, w, h, angle)
+ * The reference's arithmetic: the quad cast to float32; edges, their ratio and `ratio < 1.15` in float32 (no FMA); builtin
+ * max / min; angles = norm_angle(arctan2) of the float32 differences widened to double, range [-pi/4, 3pi/4); centres
+ * (float32 sum) / 2 in double.  Centres and sizes are bit-identical to numpy's; angles come from CUDA's atan2 (within
+ * 2 ulp) with every branch decision numpy's, except that |angle1| against |angle2| within ~45 ulp is decided by the
+ * exact angles (numpy's result there depends on its host's atan2).  n < 0 or a NULL pointer with n > 0: ORP_EINVAL. */
+int orp_poly2rbox_v3(const double *quad, int n, double *out, void *stream);
+
+/* aoe_eval (DOTA_devkit/mAOE_evaluation.py:50-169) for every class in one call, device pointers, asynchronous.  Inputs
+ * as orp_dota_eval_task1's without the difficult flags.  A detection's target is the argmax of iou_poly(gt, det) over
+ * ALL boxes of its image and class that pass the "+1 pixel" AABB prefilter (difficult boxes included, no claims: two
+ * detections may share a target); it is matched when ovmax > ovthresh (a NaN candidate leaves it unmatched).
+ * Outputs (device): cls_off_out int64 [ncls + 1] and order_out int32 [nd] as orp_dota_eval_task1's; angle_dif_out fp64
+ * [nd] per position, abs(v3(det) - v3(gt)) * 57.32 in degrees (v3: orp_poly2rbox_v3's angle), NaN when unmatched;
+ * count_out int64 [ncls] matched positions per class; aoe_out fp64 [ncls] the left-to-right sum of the class's matched
+ * angle_dif in rank order over count (0 / 0 = NaN for a class without a match; the reference raises there).  No
+ * floating-point atomics: the same call gives the same bits.  Bad sizes or NULL pointers: ORP_EINVAL before any CUDA
+ * call. */
+int orp_dota_eval_aoe(const int32_t *det_cls, const int32_t *det_img, const double *det_score, const double *det_quad,
+                      int nd, const int32_t *gt_cls, const int32_t *gt_img, const double *gt_quad, int ng, int ncls,
+                      int nimg, double ovthresh, int64_t *cls_off_out, int32_t *order_out, double *angle_dif_out,
+                      int64_t *count_out, double *aoe_out, void *stream);
+
 /* ------------------------------------------------------------------------------------------
  * Dense layers, fp32 (CUDA cores) - the reference's fp32 arithmetic of the backbone / FPN / head
  * All activations are NHWC ("channels last") contiguous device tensors; weights are

@@ -122,6 +122,8 @@ SIGNATURES = {
     "orp_convex_iou": (_i, [_vp, _i, _vp, _i, _vp, _vp]),
     "orp_dota_eval_task1": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _d, _i, _vp, _vp, _vp, _vp, _vp,
                                  _vp, _vp, _vp]),
+    "orp_dota_eval_aoe": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _i, _i, _i, _d, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "orp_poly2rbox_v3": (_i, [_vp, _i, _vp, _vp]),
     "orp_result_merge": (_i, [_vp, _i, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _d, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                               _vp]),
     "orp_split_tiles_u8": (_i, [_vp, _i, _i, _i, _vp, _i, _i, _vp, _vp]),

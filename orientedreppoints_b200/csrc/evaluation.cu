@@ -133,7 +133,8 @@ eval_gt_seg_kernel(const int32_t *__restrict__ gt_cls, const int32_t *__restrict
 }
 
 // ground truth in bucket order (input order inside a bucket: the stable sort keeps it, and np.argmax's first maximum
-// refers to it); npos per class (:139), claims reset
+// refers to it); for the VOC matching (kVoc) also npos per class (:139) and the claims reset
+template <bool kVoc>
 __global__ void __launch_bounds__(kEvalThreads)
 eval_gt_gather_kernel(const double *__restrict__ gt_quad, const uint8_t *__restrict__ gt_difficult,
                       const int32_t *__restrict__ gt_cls, const int32_t *__restrict__ gorder, const uint32_t *__restrict__ gseg,
@@ -147,16 +148,21 @@ eval_gt_gather_kernel(const double *__restrict__ gt_quad, const uint8_t *__restr
 #pragma unroll
         for (int i = 0; i < 8; ++i) { q[i] = gt_quad[(size_t)g * 8 + i]; gq[(size_t)k * 8 + i] = q[i]; }
         gbox[k] = quad_aabb(q);
-        const uint8_t d = gt_difficult[g] != 0;
-        gdiff[k] = d;
-        claim[k] = INT_MAX;
-        if (gseg[k] != none && !d) atomicAdd(&npos[gt_cls[g]], 1ull);
+        if constexpr (kVoc) {
+            const uint8_t d = gt_difficult[g] != 0;
+            gdiff[k] = d;
+            claim[k] = INT_MAX;
+            if (gseg[k] != none && !d) atomicAdd(&npos[gt_cls[g]], 1ull);
+        }
     }
 }
 
-// ovmax / jmax of every detection (:166-220) and the claims of :222-228.  CTA = kEvalThreads consecutive detections of
-// the bucket order; it walks the buckets they cover, staging each bucket's ground truth kGtStage boxes at a time.  One
-// CTA per SM: the call to the fp64 clipping (ref_quad_pair) needs ~190 registers to run without spills.
+// ovmax / jmax of every detection (:166-220).  kVoc: the claims of :222-228 and a status per position; otherwise (the
+// mAOE matching, mAOE_evaluation.py:114-160: no difficult flags, no claims) jm[p] = jmax when ovmax > ovthresh, else -1.
+// CTA = kEvalThreads consecutive detections of the bucket order; it walks the buckets they cover, staging each bucket's
+// ground truth kGtStage boxes at a time.  One CTA per SM: the call to the fp64 clipping (ref_quad_pair) needs ~190
+// registers to run without spills.
+template <bool kVoc>
 __global__ void __launch_bounds__(kEvalThreads, 1)
 eval_match_kernel(const uint32_t *__restrict__ dseg, const int32_t *__restrict__ dpos, const int32_t *__restrict__ order,
                   const double *__restrict__ det_quad, int nd, const uint32_t *__restrict__ gseg, const double *__restrict__ gq,
@@ -223,13 +229,17 @@ eval_match_kernel(const uint32_t *__restrict__ dseg, const int32_t *__restrict__
     }
 
     if (!live) return;
-    uint8_t st = kFalsePos;
-    if (jmax >= 0 && ov > ovthresh) {
-        if (gdiff[jmax]) st = kDifficultHit;
-        else { st = kCandidate; atomicMin(&claim[jmax], p); }
+    if constexpr (kVoc) {
+        uint8_t st = kFalsePos;
+        if (jmax >= 0 && ov > ovthresh) {
+            if (gdiff[jmax]) st = kDifficultHit;
+            else { st = kCandidate; atomicMin(&claim[jmax], p); }
+        }
+        jm[p] = jmax;
+        status[p] = st;
+    } else {
+        jm[p] = (jmax >= 0 && ov > ovthresh) ? jmax : -1;
     }
-    jm[p] = jmax;
-    status[p] = st;
 }
 
 // tp / fp of every position, packed as (tp << 32) | fp for one scan
@@ -321,11 +331,242 @@ eval_ap_kernel(const double *__restrict__ rec, const double *__restrict__ prec, 
     }
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// poly2rbox_single_v3 (DOTA_devkit/dota_poly2rbox.py:128-190) and the mAOE (mAOE_evaluation.py)
+// ---------------------------------------------------------------------------------------------------------------------
+
+constexpr double kQuarterPi = 0.78539816339744830962;   // np.pi / 4; k * kQuarterPi is exact for k = 1 .. 5
+
+struct RBox { double x, y, w, h, a; };
+
+// np.arctan2 of a float32 direction widened to double.  Directions on an axis or a diagonal return numpy's constants
+// k * pi / 4: norm_angle wraps at -pi/4 and 3pi/4, so these must be bit-exact (3pi/4 becomes -pi/4).  Any other float32
+// direction is at least ~2^-25 rad from those, where CUDA's atan2 (<= 2 ulp) cannot move it across the wrap.
+__device__ __forceinline__ double np_atan2(double y, double x)
+{
+    if (x != x || y != y) return x + y;
+    if (y == 0.0) return (x > 0.0 || (x == 0.0 && !signbit(x))) ? copysign(0.0, y) : copysign(4.0 * kQuarterPi, y);
+    if (x == 0.0) return copysign(2.0 * kQuarterPi, y);
+    if (fabs(x) == fabs(y)) return copysign(x > 0.0 ? kQuarterPi : 3.0 * kQuarterPi, y);
+    return atan2(y, x);
+}
+
+// norm_angle(a) = (a + pi/4) % pi - pi/4 with numpy's floor mod (npy_divmod): range [-pi/4, 3pi/4)
+__device__ __forceinline__ double norm_angle(double a)
+{
+    const double pi = 4.0 * kQuarterPi;
+    double m = fmod(__dsub_rn(a, -kQuarterPi), pi);   // fmod is exact
+    if (m != 0.0) { if (m < 0.0) m = __dadd_rn(m, pi); }
+    else m = 0.0;
+    return __dadd_rn(m, -kQuarterPi);
+}
+
+// the exact |norm_angle| of direction (x, y) as a vector of angle in [0, 3pi/4): turned into norm_angle's half-plane,
+// then mirrored into y >= 0
+__device__ __forceinline__ void fold_direction(float x, float y, float &u, float &v)
+{
+    if (!(x > -y || (x == -y && x > 0.f))) { x = -x; y = -y; }
+    u = x;
+    v = fabsf(y);
+}
+
+// abs(a1) > abs(a2) for a1 = norm_angle(atan2(y1, x1)), a2 = norm_angle(atan2(y2, x2)).  Outside a band of ~45 ulp the
+// doubles decide: there numpy's and CUDA's atan2 (each within a few ulp of the exact angle) agree on the order.  Inside
+// it the order of the exact angles decides - the sign of a cross product of float32 values, whose fp64 products are exact
+// - so exact ties (squares, mirrored edges) go to edge 1->2 as the reference's `>` sends them.
+__device__ __forceinline__ bool abs_angle_greater(double a1, double a2, float x1, float y1, float x2, float y2)
+{
+    const double d = __dsub_rn(fabs(a1), fabs(a2));
+    if (!(fabs(d) <= 1e-14)) return d > 0.0;   // also NaN: the reference's comparison is false
+    float u1, v1, u2, v2;
+    fold_direction(x1, y1, u1, v1);
+    fold_direction(x2, y2, u2, v2);
+    if (x2 == 0.f && y2 == 0.f) return v1 > 0.f;   // angle 0
+    return __dmul_rn((double)u2, (double)v1) > __dmul_rn((double)v2, (double)u1);
+}
+
+// poly2rbox_single_v3: the quad cast to float32, edges and ratio in float32 (no FMA), angles of the float32 differences
+// widened to double, builtin max / min (a NaN edge is kept when it comes first), `ratio < 1.15` in float32
+__device__ RBox poly2rbox_v3(const double *q)
+{
+    float p[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) p[i] = __double2float_rn(q[i]);
+    const float ex1 = __fsub_rn(p[0], p[2]), ey1 = __fsub_rn(p[1], p[3]);
+    const float ex2 = __fsub_rn(p[2], p[4]), ey2 = __fsub_rn(p[3], p[5]);
+    const float e1 = __fsqrt_rn(__fadd_rn(__fmul_rn(ex1, ex1), __fmul_rn(ey1, ey1)));
+    const float e2 = __fsqrt_rn(__fadd_rn(__fmul_rn(ex2, ex2), __fmul_rn(ey2, ey2)));
+    const float dx1 = __fsub_rn(p[2], p[0]), dy1 = __fsub_rn(p[3], p[1]);   // pt2 - pt1
+    const float dx2 = __fsub_rn(p[6], p[0]), dy2 = __fsub_rn(p[7], p[1]);   // pt4 - pt1
+    const float mx = e2 > e1 ? e2 : e1, mn = e2 < e1 ? e2 : e1;
+    RBox r;
+    if (__fdiv_rn(mx, mn) < 1.15f) {
+        r.w = mx;
+        r.h = mn;
+        const double a1 = norm_angle(np_atan2(dy1, dx1)), a2 = norm_angle(np_atan2(dy2, dx2));
+        r.a = abs_angle_greater(a1, a2, dx1, dy1, dx2, dy2) ? a2 : a1;
+    } else if (e1 > e2) {
+        r.w = e1;
+        r.h = e2;
+        r.a = norm_angle(np_atan2(dy1, dx1));
+    } else if (e2 >= e1) {
+        r.w = e2;
+        r.h = e1;
+        r.a = norm_angle(np_atan2(dy2, dx2));
+    } else {                                       // a NaN edge: neither branch, final_angle = norm_angle(0)
+        r.w = r.h = 0.0;
+        r.a = norm_angle(0.0);
+    }
+    r.x = __ddiv_rn((double)__fadd_rn(p[0], p[4]), 2.0);
+    r.y = __ddiv_rn((double)__fadd_rn(p[1], p[5]), 2.0);
+    return r;
+}
+
+__global__ void __launch_bounds__(kEvalThreads)
+poly2rbox_v3_kernel(const double *__restrict__ quad, int n, double *__restrict__ out)
+{
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const RBox r = poly2rbox_v3(quad + (size_t)i * 8);
+        double *o = out + (size_t)i * 5;
+        o[0] = r.x; o[1] = r.y; o[2] = r.w; o[3] = r.h; o[4] = r.a;
+    }
+}
+
+// angle_dif of every matched position: abs(v3(det) - v3(gt[jmax])) * 57.32 (mAOE_evaluation.py:158-166); NaN unmatched
+__global__ void __launch_bounds__(kEvalThreads)
+aoe_angle_kernel(const int32_t *__restrict__ jm, const int32_t *__restrict__ order, const double *__restrict__ det_quad,
+                 const double *__restrict__ gq, int nd, double *__restrict__ angle_dif)
+{
+    for (int p = blockIdx.x * blockDim.x + threadIdx.x; p < nd; p += gridDim.x * blockDim.x) {
+        const int j = jm[p];
+        double v = __longlong_as_double(0x7ff8000000000000ll);
+        if (j >= 0) {
+            const double a_det = poly2rbox_v3(det_quad + (size_t)order[p] * 8).a;
+            const double a_gt = poly2rbox_v3(gq + (size_t)j * 8).a;
+            v = __dmul_rn(fabs(__dsub_rn(a_det, a_gt)), 57.32);
+        }
+        angle_dif[p] = v;
+    }
+}
+
+// per class, one warp: count of matched positions and aoe = (left-to-right running sum of their angle_dif) / count, the
+// plain loop of mAOE_evaluation.py:192-197.  Lanes load 32 positions at a time; the adds run in rank order on every lane.
+__global__ void __launch_bounds__(kEvalThreads)
+aoe_class_kernel(const double *__restrict__ angle_dif, const int32_t *__restrict__ jm, const int64_t *__restrict__ cls_off,
+                 int ncls, int64_t *__restrict__ count, double *__restrict__ aoe)
+{
+    const int c = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (c >= ncls) return;
+    const int64_t a = cls_off[c], b = cls_off[c + 1];
+    double sum = 0.0;
+    long long n = 0;
+    for (int64_t base = a; base < b; base += 32) {
+        const int64_t k = base + lane;
+        const bool m = k < b && jm[k] >= 0;
+        const double v = m ? angle_dif[k] : 0.0;
+        unsigned mask = __ballot_sync(0xffffffffu, m);
+        n += __popc(mask);
+        while (mask) {
+            const int src = __ffs(mask) - 1;
+            mask &= mask - 1;
+            sum = __dadd_rn(sum, __shfl_sync(0xffffffffu, v, src));
+        }
+    }
+    if (lane == 0) {
+        count[c] = n;
+        aoe[c] = __ddiv_rn(sum, (double)n);   // 0 / 0 = NaN for a class without a match
+    }
+}
+
 int bits_for(uint64_t v)   // key bits that hold every value in [0, v]
 {
     int b = 1;
     while (b < 64 && (v >> b)) ++b;
     return b;
+}
+
+// The front both evaluations share.  Detections ranked by class, then score (order_out, cls_off_out; ckey2 = class key of
+// each position), ground truth in (class, image) bucket order (gq), and per position the target jm of
+// eval_match_kernel<kVoc>.  With kVoc also the difficult flags, npos per class and the claims (status, claim, npos).
+struct EvalFront {
+    uint32_t *ckey2 = nullptr;
+    int32_t *jm = nullptr, *claim = nullptr;
+    uint8_t *status = nullptr, *tmp = nullptr;   // tmp: at least the `min_tmp` bytes asked for, free after the front
+    double *gq = nullptr;
+    unsigned long long *npos = nullptr;
+};
+
+template <bool kVoc>
+int eval_front(Scratch &S, cudaStream_t st, const char *who, const int32_t *det_cls, const int32_t *det_img,
+               const double *det_score, const double *det_quad, int nd, const int32_t *gt_cls, const int32_t *gt_img,
+               const double *gt_quad, const uint8_t *gt_difficult, int ng, int ncls, int nimg, double ovthresh,
+               size_t min_tmp, int32_t *order_out, int64_t *cls_off_out, EvalFront &F)
+{
+    const uint32_t none = (uint32_t)ncls * (uint32_t)nimg;
+    const int cbits = bits_for((uint64_t)ncls), sbits = bits_for((uint64_t)none);
+    const int T = kEvalThreads, GD = grid_for((size_t)nd, T), GG = grid_for((size_t)ng, T);
+
+    uint64_t *skey = S.get<uint64_t>(nd), *skey2 = S.get<uint64_t>(nd);
+    int32_t *iota = S.get<int32_t>(nd), *by_score = S.get<int32_t>(nd), *dpos = S.get<int32_t>(nd);
+    uint32_t *ckey = S.get<uint32_t>(nd);
+    F.ckey2 = S.get<uint32_t>(nd);
+    uint32_t *dseg = S.get<uint32_t>(nd), *dseg2 = S.get<uint32_t>(nd);
+    F.jm = S.get<int32_t>(nd);
+    uint32_t *gseg = S.get<uint32_t>(ng), *gseg2 = S.get<uint32_t>(ng);
+    int32_t *giota = S.get<int32_t>(ng), *gorder = S.get<int32_t>(ng);
+    F.gq = S.get<double>((size_t)ng * 8);
+    double4 *gbox = S.get<double4>(ng);
+    uint8_t *gdiff = nullptr;
+    if (kVoc) {
+        F.status = S.get<uint8_t>(nd);
+        F.claim = S.get<int32_t>(ng);
+        gdiff = S.get<uint8_t>(ng);
+        F.npos = S.get<unsigned long long>(ncls);
+    }
+    if (!gbox || (kVoc && !F.npos)) return fail(ORP_ECUDA, "%s: scratch allocation failed", who);
+    size_t tb1 = 0, tb2 = 0, tb3 = 0, tb4 = 0;
+    cub::DeviceRadixSort::SortPairs(nullptr, tb1, skey, skey2, iota, by_score, nd, 0, 64, st);
+    cub::DeviceRadixSort::SortPairs(nullptr, tb2, ckey, F.ckey2, by_score, order_out, nd, 0, cbits, st);
+    cub::DeviceRadixSort::SortPairs(nullptr, tb3, dseg, dseg2, iota, dpos, nd, 0, sbits, st);
+    cub::DeviceRadixSort::SortPairs(nullptr, tb4, gseg, gseg2, giota, gorder, ng, 0, sbits, st);
+    size_t tb = min_tmp;
+    for (size_t v : {tb1, tb2, tb3, tb4}) tb = tb > v ? tb : v;
+    F.tmp = S.get<uint8_t>(tb);
+    if (!F.tmp) return fail(ORP_ECUDA, "%s: scratch allocation failed", who);
+    uint8_t *tmp = F.tmp;
+
+    if (kVoc) ORP_CUDA(cudaMemsetAsync(F.npos, 0, sizeof(unsigned long long) * (size_t)(ncls ? ncls : 1), st));
+    if (ng > 0) {
+        eval_gt_seg_kernel<<<GG, T, 0, st>>>(gt_cls, gt_img, ng, ncls, nimg, gseg, giota);
+        ORP_LAUNCHED();
+        ORP_CUDA(cub::DeviceRadixSort::SortPairs(tmp, tb4, gseg, gseg2, giota, gorder, ng, 0, sbits, st));
+        count_launches(1);
+        eval_gt_gather_kernel<kVoc><<<GG, T, 0, st>>>(gt_quad, gt_difficult, gt_cls, gorder, gseg2, ng, ncls, nimg, F.gq,
+                                                      gbox, gdiff, F.npos, F.claim);
+        ORP_LAUNCHED();
+    }
+    if (nd > 0) {
+        eval_det_prep_kernel<<<GD, T, 0, st>>>(det_score, nd, skey, iota);
+        ORP_LAUNCHED();
+        ORP_CUDA(cub::DeviceRadixSort::SortPairs(tmp, tb1, skey, skey2, iota, by_score, nd, 0, 64, st));
+        count_launches(1);
+        eval_class_key_kernel<<<GD, T, 0, st>>>(det_cls, by_score, nd, ncls, ckey);
+        ORP_LAUNCHED();
+        ORP_CUDA(cub::DeviceRadixSort::SortPairs(tmp, tb2, ckey, F.ckey2, by_score, order_out, nd, 0, cbits, st));
+        count_launches(1);
+    }
+    eval_class_offsets_kernel<<<grid_for((size_t)ncls + 1, T), T, 0, st>>>(F.ckey2, nd, ncls, cls_off_out);
+    ORP_LAUNCHED();
+    if (nd > 0) {
+        eval_det_seg_kernel<<<GD, T, 0, st>>>(det_img, order_out, F.ckey2, nd, ncls, nimg, dseg, iota);
+        ORP_LAUNCHED();
+        ORP_CUDA(cub::DeviceRadixSort::SortPairs(tmp, tb3, dseg, dseg2, iota, dpos, nd, 0, sbits, st));
+        count_launches(1);
+        eval_match_kernel<kVoc><<<ceil_div(nd, T), T, 0, st>>>(dseg2, dpos, order_out, det_quad, nd, gseg2, F.gq, gbox,
+                                                               gdiff, ng, none, ovthresh, F.claim, F.jm, F.status);
+        ORP_LAUNCHED();
+    }
+    return ORP_OK;
 }
 
 }  // namespace
@@ -350,77 +591,71 @@ extern "C" int orp_dota_eval_task1(const int32_t *det_cls, const int32_t *det_im
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     Thresholds thr{};
     if (use_07_metric) memcpy(thr.t, thresholds11, sizeof(thr.t));
-    const uint32_t none = (uint32_t)ncls * (uint32_t)nimg;
-    const int cbits = bits_for((uint64_t)ncls), sbits = bits_for((uint64_t)none);
-    const int T = kEvalThreads, GD = grid_for((size_t)nd, T), GG = grid_for((size_t)ng, T);
+    const int T = kEvalThreads, GD = grid_for((size_t)nd, T);
 
     Scratch S(st);
-    uint64_t *skey = S.get<uint64_t>(nd), *skey2 = S.get<uint64_t>(nd);
-    int32_t *iota = S.get<int32_t>(nd), *by_score = S.get<int32_t>(nd), *dpos = S.get<int32_t>(nd);
-    uint32_t *ckey = S.get<uint32_t>(nd), *ckey2 = S.get<uint32_t>(nd);
-    uint32_t *dseg = S.get<uint32_t>(nd), *dseg2 = S.get<uint32_t>(nd);
-    int32_t *jm = S.get<int32_t>(nd);
-    uint8_t *status = S.get<uint8_t>(nd);
     unsigned long long *tpfp = S.get<unsigned long long>(nd), *cum = S.get<unsigned long long>(nd);
-    uint32_t *gseg = S.get<uint32_t>(ng), *gseg2 = S.get<uint32_t>(ng);
-    int32_t *giota = S.get<int32_t>(ng), *gorder = S.get<int32_t>(ng), *claim = S.get<int32_t>(ng);
-    double *gq = S.get<double>((size_t)ng * 8);
-    double4 *gbox = S.get<double4>(ng);
-    uint8_t *gdiff = S.get<uint8_t>(ng);
-    unsigned long long *npos = S.get<unsigned long long>(ncls);
-    if (!npos) return fail(ORP_ECUDA, "orp_dota_eval_task1: scratch allocation failed");
-    size_t tb1 = 0, tb2 = 0, tb3 = 0, tb4 = 0, tb5 = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, tb1, skey, skey2, iota, by_score, nd, 0, 64, st);
-    cub::DeviceRadixSort::SortPairs(nullptr, tb2, ckey, ckey2, by_score, order_out, nd, 0, cbits, st);
-    cub::DeviceRadixSort::SortPairs(nullptr, tb3, dseg, dseg2, iota, dpos, nd, 0, sbits, st);
-    cub::DeviceRadixSort::SortPairs(nullptr, tb4, gseg, gseg2, giota, gorder, ng, 0, sbits, st);
+    if (!cum) return fail(ORP_ECUDA, "orp_dota_eval_task1: scratch allocation failed");
+    size_t tb5 = 0;
     cub::DeviceScan::InclusiveSum(nullptr, tb5, tpfp, cum, nd, st);
-    size_t tb = tb1;
-    for (size_t v : {tb2, tb3, tb4, tb5}) tb = tb > v ? tb : v;
-    uint8_t *tmp = S.get<uint8_t>(tb);
-    if (!tmp) return fail(ORP_ECUDA, "orp_dota_eval_task1: scratch allocation failed");
-
-    ORP_CUDA(cudaMemsetAsync(npos, 0, sizeof(unsigned long long) * (size_t)(ncls ? ncls : 1), st));
-    if (ng > 0) {
-        eval_gt_seg_kernel<<<GG, T, 0, st>>>(gt_cls, gt_img, ng, ncls, nimg, gseg, giota);
-        ORP_LAUNCHED();
-        ORP_CUDA(cub::DeviceRadixSort::SortPairs(tmp, tb4, gseg, gseg2, giota, gorder, ng, 0, sbits, st));
-        count_launches(1);
-        eval_gt_gather_kernel<<<GG, T, 0, st>>>(gt_quad, gt_difficult, gt_cls, gorder, gseg2, ng, ncls, nimg, gq, gbox,
-                                                gdiff, npos, claim);
-        ORP_LAUNCHED();
-    }
+    EvalFront F;
+    rc = eval_front<true>(S, st, "orp_dota_eval_task1", det_cls, det_img, det_score, det_quad, nd, gt_cls, gt_img, gt_quad,
+                          gt_difficult, ng, ncls, nimg, ovthresh, tb5, order_out, cls_off_out, F);
+    if (rc) return rc;
     if (nd > 0) {
-        eval_det_prep_kernel<<<GD, T, 0, st>>>(det_score, nd, skey, iota);
+        eval_tpfp_kernel<<<GD, T, 0, st>>>(F.status, F.jm, F.claim, nd, tpfp);
         ORP_LAUNCHED();
-        ORP_CUDA(cub::DeviceRadixSort::SortPairs(tmp, tb1, skey, skey2, iota, by_score, nd, 0, 64, st));
+        ORP_CUDA(cub::DeviceScan::InclusiveSum(F.tmp, tb5, tpfp, cum, nd, st));
         count_launches(1);
-        eval_class_key_kernel<<<GD, T, 0, st>>>(det_cls, by_score, nd, ncls, ckey);
-        ORP_LAUNCHED();
-        ORP_CUDA(cub::DeviceRadixSort::SortPairs(tmp, tb2, ckey, ckey2, by_score, order_out, nd, 0, cbits, st));
-        count_launches(1);
-    }
-    eval_class_offsets_kernel<<<grid_for((size_t)ncls + 1, T), T, 0, st>>>(ckey2, nd, ncls, cls_off_out);
-    ORP_LAUNCHED();
-    if (nd > 0) {
-        eval_det_seg_kernel<<<GD, T, 0, st>>>(det_img, order_out, ckey2, nd, ncls, nimg, dseg, iota);
-        ORP_LAUNCHED();
-        ORP_CUDA(cub::DeviceRadixSort::SortPairs(tmp, tb3, dseg, dseg2, iota, dpos, nd, 0, sbits, st));
-        count_launches(1);
-        eval_match_kernel<<<ceil_div(nd, T), T, 0, st>>>(dseg2, dpos, order_out, det_quad, nd, gseg2, gq, gbox, gdiff, ng,
-                                                         none, ovthresh, claim, jm, status);
-        ORP_LAUNCHED();
-        eval_tpfp_kernel<<<GD, T, 0, st>>>(status, jm, claim, nd, tpfp);
-        ORP_LAUNCHED();
-        ORP_CUDA(cub::DeviceScan::InclusiveSum(tmp, tb5, tpfp, cum, nd, st));
-        count_launches(1);
-        eval_pr_kernel<<<GD, T, 0, st>>>(cum, ckey2, cls_off_out, npos, nd, ncls, rec_out, prec_out);
+        eval_pr_kernel<<<GD, T, 0, st>>>(cum, F.ckey2, cls_off_out, F.npos, nd, ncls, rec_out, prec_out);
         ORP_LAUNCHED();
     }
     if (ncls > 0) {
         eval_ap_kernel<<<ncls, T, 0, st>>>(rec_out, prec_out, cls_off_out, use_07_metric, thr, ap_out);
         ORP_LAUNCHED();
-        ORP_CUDA(cudaMemcpyAsync(npos_out, npos, sizeof(int64_t) * (size_t)ncls, cudaMemcpyDeviceToDevice, st));
+        ORP_CUDA(cudaMemcpyAsync(npos_out, F.npos, sizeof(int64_t) * (size_t)ncls, cudaMemcpyDeviceToDevice, st));
     }
+    return ORP_OK;
+}
+
+extern "C" int orp_dota_eval_aoe(const int32_t *det_cls, const int32_t *det_img, const double *det_score,
+                                 const double *det_quad, int nd, const int32_t *gt_cls, const int32_t *gt_img,
+                                 const double *gt_quad, int ng, int ncls, int nimg, double ovthresh, int64_t *cls_off_out,
+                                 int32_t *order_out, double *angle_dif_out, int64_t *count_out, double *aoe_out,
+                                 void *stream)
+{
+    if (nd < 0 || ng < 0 || ncls < 0 || nimg < 0 || (long long)ncls * nimg >= (long long)INT32_MAX ||
+        (nd > 0 && (!det_cls || !det_img || !det_score || !det_quad || !order_out || !angle_dif_out)) ||
+        (ng > 0 && (!gt_cls || !gt_img || !gt_quad)) || (ncls > 0 && (!count_out || !aoe_out)) || !cls_off_out)
+        return fail(ORP_EINVAL, "orp_dota_eval_aoe: bad arguments");
+    int rc = ensure_device();
+    if (rc) return rc;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int T = kEvalThreads;
+    Scratch S(st);
+    EvalFront F;
+    rc = eval_front<false>(S, st, "orp_dota_eval_aoe", det_cls, det_img, det_score, det_quad, nd, gt_cls, gt_img, gt_quad,
+                           nullptr, ng, ncls, nimg, ovthresh, 0, order_out, cls_off_out, F);
+    if (rc) return rc;
+    if (nd > 0) {
+        aoe_angle_kernel<<<grid_for((size_t)nd, T), T, 0, st>>>(F.jm, order_out, det_quad, F.gq, nd, angle_dif_out);
+        ORP_LAUNCHED();
+    }
+    if (ncls > 0) {
+        aoe_class_kernel<<<ceil_div((long long)ncls * 32, T), T, 0, st>>>(angle_dif_out, F.jm, cls_off_out, ncls, count_out,
+                                                                           aoe_out);
+        ORP_LAUNCHED();
+    }
+    return ORP_OK;
+}
+
+extern "C" int orp_poly2rbox_v3(const double *quad, int n, double *out, void *stream)
+{
+    if (n < 0 || (n > 0 && (!quad || !out))) return fail(ORP_EINVAL, "orp_poly2rbox_v3: bad arguments");
+    if (n == 0) return ORP_OK;
+    int rc = ensure_device();
+    if (rc) return rc;
+    poly2rbox_v3_kernel<<<grid_for((size_t)n, kEvalThreads), kEvalThreads, 0, static_cast<cudaStream_t>(stream)>>>(quad, n, out);
+    ORP_LAUNCHED();
     return ORP_OK;
 }

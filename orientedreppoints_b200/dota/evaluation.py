@@ -162,17 +162,12 @@ def evaluate(dets, gts, classnames=DOTA_CLASSES, ovthresh=0.5, use_07_metric=Tru
     return res
 
 
-def evaluate_merged(merged, gts, image_names, classnames=DOTA_CLASSES, ovthresh=0.5, use_07_metric=True):
-    """`evaluate` over result_merge.MergedDetections (merge_packed, detect_image_tensors): the same dict, with nothing
-    parsed and no detection uploaded - the merge's tensors go to orp_dota_eval_task1 as they are.
-      image_names  name of every image id of the merge.  The ids are mapped to the positions in `gts` on the device; an
-                   image that carries a detection must be a key of `gts` (KeyError, as for a detection line of an unknown
-                   image), one without detections need not be
-      classnames   the merge's classes, in its class order
-    'order' indexes each class's merged rows, i.e. the lines of `merged.to_lines(image_names, classnames)`."""
-    classnames = tuple(classnames)
+def _merged_inputs(merged, gts, image_names, classnames, who):
+    """the device inputs of the evaluation calls (the _host_arrays order) from result_merge.MergedDetections: the merge's
+    tensors as they are, image ids mapped to positions in `gts` on the device -> (inputs, number of images, device).  An
+    image that carries a detection and is not a key of `gts` is a KeyError."""
     if len(classnames) != merged.ncls or len(image_names) != merged.nimg:
-        raise ValueError("evaluate_merged: %d class names and %d image names expected" % (merged.ncls, merged.nimg))
+        raise ValueError("%s: %d class names and %d image names expected" % (who, merged.ncls, merged.nimg))
     arrays, nimg, _ = _host_arrays({}, gts, classnames)
     img_index = {name: i for i, name in enumerate(gts)}
     dev = merged.cls.device
@@ -184,6 +179,19 @@ def evaluate_merged(merged, gts, image_names, classnames=DOTA_CLASSES, ovthresh=
     lut = torch.tensor([img_index.get(name, -1) for name in image_names], dtype=torch.int32).to(dev)
     inputs = [merged.cls.contiguous(), lut[merged.img.long()].contiguous(), merged.score.contiguous(),
               merged.quad.contiguous()] + [torch.from_numpy(np.ascontiguousarray(a)).to(dev) for a in arrays[4:]]
+    return inputs, nimg, dev
+
+
+def evaluate_merged(merged, gts, image_names, classnames=DOTA_CLASSES, ovthresh=0.5, use_07_metric=True):
+    """`evaluate` over result_merge.MergedDetections (merge_packed, detect_image_tensors): the same dict, with nothing
+    parsed and no detection uploaded - the merge's tensors go to orp_dota_eval_task1 as they are.
+      image_names  name of every image id of the merge.  The ids are mapped to the positions in `gts` on the device; an
+                   image that carries a detection must be a key of `gts` (KeyError, as for a detection line of an unknown
+                   image), one without detections need not be
+      classnames   the merge's classes, in its class order
+    'order' indexes each class's merged rows, i.e. the lines of `merged.to_lines(image_names, classnames)`."""
+    classnames = tuple(classnames)
+    inputs, nimg, dev = _merged_inputs(merged, gts, image_names, classnames, "evaluate_merged")
     buf, offs = _launch(inputs, len(classnames), nimg, ovthresh, use_07_metric, dev)
     out = buf.cpu().numpy()                                                           # the one copy back
     npos, cls_off, rec, prec, ap, order = (out[offs[k]:offs[k + 1]].view(t) for k, t in enumerate(_OUT_DTYPES))
