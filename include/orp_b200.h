@@ -249,6 +249,27 @@ int orp_head_postprocess(int nlevels, const float *const *cls, const float *cons
                          const int *W, const int *stride, int B, int num_cls, int nms_pre, float score_thr,
                          double iou_thr, int max_per_img, const float *scale_factor, float *dets_out,
                          int64_t *labels_out, int32_t *counts_out, void *stream);
+/* OrientedRepPointsDetector.aug_test's post-processing (multi-scale / flip testing) for V views of B images, device
+ * resident (mmdet/models/detectors/orientedreppoints_detector.py:48-144: get_bboxes(rescale=False, nms=False) per view,
+ * rbox_mapping_back, torch.cat, ONE multiclass_rnms).  The same pipeline as orp_head_postprocess with a view dimension.
+ *   cls, ref, H, W, stride   [nviews * nlevels] entries, view-major; views may differ in H and W
+ *   view_meta  device fp32 [nviews, B, 3]: flip (0 / 1, horizontal), img_shape width, scale_factor of (view, image)
+ *   out_scale  device fp32 [B] or NULL: the 8 box values of the result are multiplied by it (rescale=False puts the
+ *              first view's scale factor back, :139-141)
+ *   dets_out   device fp32 [B, max_per_img, 27]: columns 0..17 zero (these rows carry no reppoints), box(8) | score in
+ *              columns 18..26 - the row layout of orp_head_postprocess, so orp_pack_detections and orp_result_merge
+ *              take it unchanged;  labels_out, counts_out as there (counts -1: NMS candidate list overflow)
+ * Candidates of an image are ordered view, level, top-k slot (location where H*W <= nms_pre), class - the order of
+ * torch.cat over the views; top-k is per (view, level, image).  The NMS segment is image * num_cls + class, so a box of
+ * one view suppresses its twin of another.  Map-back, each step one fp32 rounding: rect * stride + centre;
+ * flipped views x = (w - x) - 1; then * (1.0f / scale_factor) - the eager code divides a CUDA tensor by a Python float,
+ * which torch evaluates as a product with the fp32 reciprocal, unlike the true division of orp_head_postprocess.
+ * ORP_EINVAL before any device work: nviews < 1, nviews * nlevels > 80, 2^20 or more candidates per image, view_meta
+ * NULL, and the batch bounds of orp_head_postprocess.  Asynchronous. */
+int orp_head_postprocess_aug(int nviews, int nlevels, const float *const *cls, const float *const *ref, const int *H,
+                             const int *W, const int *stride, int B, int num_cls, int nms_pre, float score_thr,
+                             double iou_thr, int max_per_img, const float *view_meta, const float *out_scale,
+                             float *dets_out, int64_t *labels_out, int32_t *counts_out, void *stream);
 /* padded detections of orp_head_postprocess -> the fixed-layout payload of the ONE all-gather that replaces
  * collect_results_gpu (mmdet/apis/test.py:117-147): packed_out device fp32 [B, max_per_img + 1, 28], rows = 27 detection values |
  * label, zero padded; row max_per_img carries the image's count in column 0. */

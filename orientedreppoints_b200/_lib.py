@@ -83,6 +83,7 @@ SIGNATURES = {
     "orp_box_iou_rotated": (_i, [_vp, _i, _vp, _i, _vp, _vp]),
     "orp_minarearect": (_i, [_vp, _i, _vp, _vp, _f, _vp, _vp]),
     "orp_head_postprocess": (_i, [_i, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _f, _d, _i, _vp, _vp, _vp, _vp, _vp]),
+    "orp_head_postprocess_aug": (_i, [_i, _i, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _f, _d, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     "orp_pack_detections": (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp]),
     "orp_dcn_offsets_multi": (_i, [_i, _vp, _vp, _vp, _f, _vp, _vp]),
     "orp_conv2d_f32": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _i, _i, _i, _i, _vp, _vp, _i, _vp, _vp, _i, _vp]),

@@ -396,19 +396,52 @@ class OrientedRepPointsDetector:
             return bboxes
         return bboxes, torch.cat(aug_scores, dim=0)
 
-    def aug_test(self, imgs, img_metas, rescale=False, valid_hws=None):
-        """orientedreppoints_detector.py:112-144.  imgs: list of views, each ONE image (float NCHW [1,3,H,W] or uint8
-        HWC [1,H,W,3]); img_metas: list of [dict(img_shape, scale_factor, flip)]; valid_hws: optional list of per-view
-        device int32 [1,2] extents (views padded by the test pipeline).  Raw candidates of all views
-        (get_bboxes(nms=False), head :778-779) are concatenated and go through ONE multiclass_rnms."""
+    def aug_test(self, imgs, img_metas, rescale=False, valid_hws=None, return_tensors=False):
+        """orientedreppoints_detector.py:112-144 for N >= 1 images.  imgs: list of views, each the N images of that view
+        (float NCHW [N,3,H,W] or uint8 HWC [N,H,W,3]); img_metas: per view the list of N dicts (img_shape, scale_factor,
+        flip); valid_hws: optional list of per-view device int32 [N,2] extents (views padded by the test pipeline).
+        One dense pass per view over the whole batch; the raw candidates of all views of an image (get_bboxes(nms=False),
+        head :778-779) are mapped back, concatenated and go through ONE multiclass_rnms - in one device pipeline
+        (get_bboxes_aug_fused) when fused_post is on and the NMS is 'rnms' in the default arithmetic, else op by op.
+        Returns the rbbox2result list ([k, 9] arrays: box | score) of the image for N == 1, a list of them for N > 1;
+        return_tensors="padded" (fused pipeline only): the device triple (dets [N,max_per_img,27] with box | score in
+        columns 18..26, labels, counts) without a host read."""
+        with torch.cuda.device(self.device):
+            return self._aug_test(imgs, img_metas, rescale, valid_hws, return_tensors)
+
+    def _aug_test(self, imgs, img_metas, rescale, valid_hws, return_tensors):
+        from .core.transforms import rbbox2result
+        n = imgs[0].shape[0]
+        if len(img_metas) != len(imgs) or any(v.shape[0] != n for v in imgs) or any(len(m) != n for m in img_metas):
+            raise ValueError("aug_test: every view needs the same %d images and their metas" % n)
+        dense = [self._forward_dense_opt(img, None if valid_hws is None else valid_hws[k])[0] for k, img in enumerate(imgs)]
+        cls, ref = [[o[0] for o in outs] for outs in dense], [[o[2] for o in outs] for outs in dense]
+        nms_cfg = self.test_cfg['nms']
+        if getattr(self, "fused_post", True) and nms_cfg.get('type', 'rnms') == 'rnms' and nms_cfg.get('mode', 'exact64') == 'exact64':
+            from .core.get_bboxes import get_bboxes_aug_fused
+            dets, labels, counts = get_bboxes_aug_fused(cls, ref, STRIDES, img_metas, self.test_cfg, rescale)
+            if return_tensors == "padded":
+                return dets, labels, counts
+            cnt = counts.tolist()                                      # the one host sync of a call
+            if any(c < 0 for c in cnt):
+                raise _lib.OrpError("rotated NMS candidate list overflowed its buffer (orp_head_postprocess_aug): results invalid")
+            results = [(dets[i, :cnt[i], 18:], labels[i, :cnt[i]]) for i in range(n)]
+        else:
+            if return_tensors == "padded":
+                raise ValueError("aug_test: return_tensors='padded' is the output of the fused post-processing "
+                                 "(fused_post on, nms type 'rnms' in the default arithmetic)")
+            results = [self._aug_merge_eager([[c[i:i + 1] for c in v] for v in cls], [[p[i:i + 1] for p in v] for v in ref],
+                                             [[m[i]] for m in img_metas], rescale) for i in range(n)]
+        out = [rbbox2result(d, l, 16) for d, l in results]
+        return out[0] if n == 1 else out
+
+    def _aug_merge_eager(self, cls, ref, img_metas, rescale):
+        """the op-by-op merge of ONE image's views: (dets [k, 9] box | score, labels [k])"""
         from .core.bbox_nms import multiclass_rnms
         from .core.get_bboxes import get_bboxes
-        from .core.transforms import rbbox2result
         aug_bboxes, aug_scores = [], []
-        for k, (img, meta) in enumerate(zip(imgs, img_metas)):
-            assert img.shape[0] == 1, "aug_test: one image per view"
-            outs, _ = self._forward_dense_opt(img, None if valid_hws is None else valid_hws[k])
-            b, sc = get_bboxes([o[0] for o in outs], [o[2] for o in outs], STRIDES, meta, self.test_cfg, False, nms=False)[0]
+        for c, p, meta in zip(cls, ref, img_metas):
+            b, sc = get_bboxes(c, p, STRIDES, meta, self.test_cfg, False, nms=False)[0]
             aug_bboxes.append(b)
             aug_scores.append(sc)
         merged_bboxes, merged_scores = self.merge_aug_results(aug_bboxes, aug_scores, img_metas)
@@ -417,4 +450,4 @@ class OrientedRepPointsDetector:
         if not rescale:
             det_bboxes = det_bboxes.clone()
             det_bboxes[:, :8] *= img_metas[0][0]['scale_factor']
-        return rbbox2result(det_bboxes, det_labels, 16)
+        return det_bboxes, det_labels

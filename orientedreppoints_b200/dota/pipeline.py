@@ -52,21 +52,28 @@ def detect_image(det, img_u8, name="P0000", rate=1, subsize=1024, gap=200, batch
         if len(views) == 1:
             results.extend(det.simple_test(views[0], metas[0], rescale=True, valid_hw=valids[0]))
         else:
-            results.extend(det.aug_test([v[k:k + 1] for v in views], [[m[k]] for m in metas], rescale=True,
-                                        valid_hws=[v[k:k + 1] for v in valids]) for k in range(views[0].shape[0]))
+            results.extend(_aug_results(det, views, metas, valids))
     per_class = task1_lines(results, names)
     return {cname: merge_lines(lines, merge_thresh) for cname, lines in zip(DOTA_CLASSES, per_class)}
 
 
+def _aug_results(det, views, metas, valids):
+    """one aug_test call for a batch of tiles -> the list of per-tile rbbox2result lists (a batch of one tile comes back
+    as that tile's list itself)"""
+    res = det.aug_test(views, metas, rescale=True, valid_hws=valids)
+    return [res] if views[0].shape[0] == 1 else res
+
+
 def _pack_rows(per_tile, cap, device):
-    """[(dets [k,27], labels [k]) per tile] -> packed [T, cap + 1, 28] (the layout of gather.pack)"""
-    buf = torch.zeros((len(per_tile), cap + 1, 28), dtype=torch.float32, device=device)
+    """[(dets [k,27], labels [k]) per tile] -> packed [T, cap + 1, 28] (the layout of gather.pack).  The buffer is filled
+    where the rows live, so host rows (aug_test's list form) cost one upload per batch"""
+    buf = torch.zeros((len(per_tile), cap + 1, 28), dtype=torch.float32, device=per_tile[0][0].device if per_tile else device)
     for t, (d, l) in enumerate(per_tile):
         k = d.shape[0]
-        buf[t, :k, :27] = d.to(device=device, dtype=torch.float32)
-        buf[t, :k, 27] = l.to(device=device, dtype=torch.float32)
+        buf[t, :k, :27] = d.to(dtype=torch.float32)
+        buf[t, :k, 27] = l.to(dtype=torch.float32)
         buf[t, cap, 0] = k
-    return buf
+    return buf.to(device)
 
 
 def _packed_tiles(det, img_u8, name, rate, subsize, gap, batch, test_pipeline):
@@ -86,9 +93,7 @@ def _packed_tiles(det, img_u8, name, rate, subsize, gap, batch, test_pipeline):
                 out = det.simple_test(views[0], metas[0], rescale=True, valid_hw=valids[0], return_tensors="padded")
             else:
                 out = []
-                for k in range(views[0].shape[0]):
-                    res = det.aug_test([v[k:k + 1] for v in views], [[m[k]] for m in metas], rescale=True,
-                                       valid_hws=[v[k:k + 1] for v in valids])
+                for res in _aug_results(det, views, metas, valids):
                     # aug_test rows are box(8) | score without the reppoints: right-aligned, as the Task1 writer reads
                     # a row from its end (bbox[-9:-1], bbox[-1])
                     rows = torch.zeros((sum(len(a) for a in res), 27), dtype=torch.float32)
@@ -112,8 +117,9 @@ def detect_images_tensors(det, images, rate=1, subsize=1024, gap=200, batch=16, 
     rate: one rate or a sequence of rates; the tiles of every rate of an image share its id, as the reference's
     multi-scale merge joins them through the tile name.
     No count is read per batch and nothing goes through rbbox2result; the merge reads the host twice (the row total that
-    sizes it, then the survivor count with the status - see merge_packed's max_rows).  One exception: a test_pipeline with more than one
-    view (multi-scale / flip) still runs `aug_test` per tile through the existing path, and its result is packed."""
+    sizes it, then the survivor count with the status - see merge_packed's max_rows).  One exception: a test_pipeline with
+    more than one view (multi-scale / flip) makes one batched `aug_test` call per batch of tiles and takes its list form
+    (one count read per batch), which is repacked and uploaded once per batch."""
     rates = tuple(rate) if isinstance(rate, (tuple, list)) else (rate,)
     ids = list(range(len(images))) if image_ids is None else [int(i) for i in image_ids]
     nimg = (max(ids) + 1 if ids else 1) if nimg is None else int(nimg)

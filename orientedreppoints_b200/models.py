@@ -243,8 +243,8 @@ class OrientedRepPointsDetector(nn.Module):
     def simple_test(self, img, img_meta=None, rescale=False):
         return self.engine().simple_test(img, img_meta, rescale=rescale)
 
-    def aug_test(self, imgs, img_metas, rescale=False):
-        return self.engine().aug_test(imgs, img_metas, rescale=rescale)
+    def aug_test(self, imgs, img_metas, rescale=False, valid_hws=None, return_tensors=False):
+        return self.engine().aug_test(imgs, img_metas, rescale, valid_hws, return_tensors=return_tensors)
 
     def forward_test(self, imgs, img_metas, **kwargs):
         """base.py:104-141: lists of augmented views; one view -> simple_test"""
