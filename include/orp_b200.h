@@ -376,6 +376,19 @@ int orp_dota_eval_aoe(const int32_t *det_cls, const int32_t *det_img, const doub
                       int64_t *count_out, double *aoe_out, void *stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Training-side geometry
+ * ---------------------------------------------------------------------------------------- */
+
+/* GIoU between the convex hull of point set i and quadrilateral i, and its gradient with respect to the points (aligned
+ * pairs): pts18 [N,18] (x0,y0,...,x8,y8), quads8 [N,8] -> out19 [N,19], row i = [d giou / d (x0,y0..x8,y8) | giou] fp32,
+ * device resident.  Replaces convex_giou_cuda (mmdet/ops/iou/src/convex_giou_cuda.cpp:8-16,
+ * convex_giou_kernel.cu:806-868, which copies the result through the host); devrIoU (:730-804) in fp64 with every operation
+ * rounded on its own, bit for bit.  Points that are not hull vertices get gradient 0; a duplicated point's gradient goes
+ * to its first copy.  A row with a non-finite input, or one the reference's fixed arrays cannot hold, is all NaN (DESIGN
+ * deviation 13).  n == 0: ORP_OK without a launch; n < 0 or NULL pointers: ORP_EINVAL.  Asynchronous. */
+int orp_convex_giou(const float *pts18, const float *quads8, int n, float *out19, void *stream);
+
+/* ------------------------------------------------------------------------------------------
  * Dense layers, fp32 (CUDA cores) - the reference's fp32 arithmetic of the backbone / FPN / head
  * All activations are NHWC ("channels last") contiguous device tensors; weights are
  * [Cout][KH][KW][Cin] (the reference's [Cout][Cin][KH][KW] permuted once at load time).

@@ -121,6 +121,7 @@ SIGNATURES = {
     "orp_stem_im2col_bf16": (_i, [_vp, _i, _i, _i, _vp, _vp]),
     "orp_stem_s2d_bf16": (_i, [_vp, _i, _i, _i, _vp, _vp]),
     "orp_convex_iou": (_i, [_vp, _i, _vp, _i, _vp, _vp]),
+    "orp_convex_giou": (_i, [_vp, _vp, _i, _vp, _vp]),
     "orp_dota_eval_task1": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _d, _i, _vp, _vp, _vp, _vp, _vp,
                                  _vp, _vp, _vp]),
     "orp_dota_eval_aoe": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _i, _i, _i, _d, _vp, _vp, _vp, _vp, _vp, _vp]),

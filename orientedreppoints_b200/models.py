@@ -20,6 +20,7 @@ BACKBONES = Registry('backbone')
 NECKS = Registry('neck')
 HEADS = Registry('head')
 DETECTORS = Registry('detector')
+LOSSES = Registry('loss')
 
 
 def build(cfg, registry, default_args=None):
@@ -42,6 +43,10 @@ def build_head(cfg):
 
 def build_detector(cfg, train_cfg=None, test_cfg=None):
     return build(cfg, DETECTORS, dict(train_cfg=train_cfg, test_cfg=test_cfg))
+
+
+def build_loss(cfg):
+    return build(cfg, LOSSES)
 
 
 class _EngineOnly(nn.Module):
@@ -260,3 +265,6 @@ class OrientedRepPointsDetector(nn.Module):
         if return_loss:
             raise NotImplementedError("training (forward_train / losses) is out of scope of liborp_b200")
         return self.forward_test(img, img_meta, **kwargs)
+
+
+from . import losses  # noqa: E402,F401  (registers GIoULoss in LOSSES)
