@@ -499,8 +499,11 @@ int orp_conv2d_tc_splitk(const orp_tc_problem *prob, const void *w, int Cout, in
 int orp_tc_plan_conv(int nprob, const orp_tc_problem *probs, const void *w, int Cout, int Cout_padded, int KH, int KW,
                      int Cin, int stride, int pad, const float *bias, int wscale_log2, int relu, int out_f32, int deform,
                      int split, int stem, int ksplit, int sms, orp_tc_plan *out);
-/* number of tile rows that saturated since the last reset (host-blocking read of a device counter) */
-int orp_f16x3_overflow_count(unsigned int *count, int reset);
+/* number of tile rows that saturated since the last reset.  The counter is one per process (device), shared by every
+ * f16x3 launch of every thread and stream.  The read is ordered on `stream`: it sees every launch enqueued on that stream
+ * before the call, and blocks the host until then.  reset != 0 reads and zeroes the counter in one atomic exchange, so a
+ * saturation that a launch on another stream records concurrently is never lost: it stays for the next read. */
+int orp_f16x3_overflow_count(unsigned int *count, int reset, void *stream);
 /* stem in split form: space-to-depth planes fp16 [2][N, H/2+3, W/2+3, 16] (hi plane, lo plane) from the uint8 HWC
  * tiles (Normalize fused) or the NCHW fp32 image, conv1 as a 4x4 stride-1 convolution over them */
 int orp_stem_s2d_u8_f16x3(const uint8_t *img_hwc, int N, int H, int W, const float *mean, const float *std, int to_rgb,

@@ -95,7 +95,7 @@ SIGNATURES = {
     "orp_conv2d_tc_splitk": (_i, [ctypes.POINTER(TcProblem), _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _i, _i, _i, _i, _vp, _vp]),
     "orp_tc_plan_conv": (_i, [_i, ctypes.POINTER(TcProblem), _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _i, _i, _i, _i, _i, _i, _i, _i,
                               ctypes.POINTER(TcPlan)]),
-    "orp_f16x3_overflow_count": (_i, [ctypes.POINTER(ctypes.c_uint), _i]),
+    "orp_f16x3_overflow_count": (_i, [ctypes.POINTER(ctypes.c_uint), _i, _vp]),
     "orp_stem_s2d_u8_f16x3": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, _vp, _vp]),
     "orp_stem_s2d_f16x3": (_i, [_vp, _i, _i, _i, _vp, _vp]),
     "orp_stem_conv_s2d_f16x3": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, _i, _vp, _vp]),

@@ -1887,14 +1887,28 @@ extern "C" int orp_stem_conv_s2d_bf16(const void *x_s2d, int N, int H, int W, co
     return rc ? rc : conv2d_tc(d, stream);
 }
 
-extern "C" int orp_f16x3_overflow_count(unsigned int *count, int reset)
+// one read of the overflow counter in stream order; with reset, read and zero are one atomic exchange, so saturations
+// that a launch on another stream adds meanwhile stay in the counter for the next read
+__global__ void overflow_take_kernel(unsigned int *dst, int reset)
+{
+    *dst = reset ? atomicExch(&g_f16_overflow, 0u) : atomicAdd(&g_f16_overflow, 0u);
+}
+
+/* see include/orp_b200.h */
+extern "C" int orp_f16x3_overflow_count(unsigned int *count, int reset, void *stream)
 {
     if (!count) return fail(ORP_EINVAL, "f16x3_overflow_count: null");
-    ORP_CUDA(cudaMemcpyFromSymbol(count, g_f16_overflow, sizeof(unsigned int)));
-    if (reset) {
-        const unsigned int z = 0;
-        ORP_CUDA(cudaMemcpyToSymbol(g_f16_overflow, &z, sizeof(z)));
+    static thread_local unsigned int *host = nullptr;              // mapped pinned word the kernel writes
+    static thread_local unsigned int *dev = nullptr;
+    if (!host) {
+        ORP_CUDA(cudaHostAlloc(reinterpret_cast<void **>(&host), sizeof(unsigned int), cudaHostAllocMapped));
+        ORP_CUDA(cudaHostGetDevicePointer(reinterpret_cast<void **>(&dev), host, 0));
     }
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    overflow_take_kernel<<<1, 1, 0, st>>>(dev, reset ? 1 : 0);
+    ORP_LAUNCHED();
+    ORP_CUDA(cudaStreamSynchronize(st));
+    *count = *host;
     return ORP_OK;
 }
 

@@ -370,6 +370,10 @@ class EngineTCSplit(EngineTC):
         return b, h, w, c
 
     def overflow_count(self, reset=True):
+        """saturated f16x3 stores since the last reset, after every launch enqueued so far on the current stream (waits
+        for them).  The counter is one per process: it also holds what other engines, threads and streams recorded"""
         c = ctypes.c_uint(0)
-        _lib.check(self.lib.orp_f16x3_overflow_count(ctypes.byref(c), int(reset)), "orp_f16x3_overflow_count")
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.orp_f16x3_overflow_count(ctypes.byref(c), int(reset), _lib.current_stream_ptr()),
+                       "orp_f16x3_overflow_count")
         return int(c.value)

@@ -24,6 +24,19 @@ def test_library_exports_every_declared_symbol():
     assert sorted(_lib.SIGNATURES) == names
 
 
+def test_bindings_match_declared_arity():
+    """every binding passes as many arguments as the header declares: a parameter added to a declaration (a stream, say)
+    and not to _lib.SIGNATURES would make ctypes pass garbage in its place"""
+    src = open(os.path.join(ROOT, "include", "orp_b200.h")).read()
+    src = re.sub(r"/\*.*?\*/", "", src, flags=re.S)
+    decls = dict(re.findall(r"\b(orp_[a-z0-9_]+)\s*\(([^)]*)\)\s*;", src))
+    assert sorted(decls) == _declared()
+    for name, params in decls.items():
+        params = params.strip()
+        n = 0 if params in ("", "void") else params.count(",") + 1
+        assert len(_lib.SIGNATURES[name][1]) == n, (name, n, len(_lib.SIGNATURES[name][1]))
+
+
 def test_version_and_arch():
     l = _lib.lib()
     assert l.orp_version() >= 100
