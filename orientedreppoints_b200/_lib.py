@@ -141,6 +141,11 @@ SIGNATURES = {
     "orp_gn_apply_bf16_multi": (_i, [_i, _vp, _i, _i, _vp, _vp, _f, _i, _vp]),
 }
 
+# name -> (restype, argtypes); every symbol include/orp_b200_dcnv2.h declares
+DCNV2_SIGNATURES = {
+    "orp_dcnv2_offset_mask": (_i, [_vp, ctypes.c_longlong, _vp, _vp, _vp]),
+}
+
 _LIB = None
 
 
@@ -157,7 +162,7 @@ def lib():
                 "liborp_b200.so not found at %s - build it with `python -m orientedreppoints_b200.build` "
                 "(there is no CPU or PyTorch fallback for this path)" % LIB_PATH)
         l = ctypes.CDLL(LIB_PATH)
-        for name, (res, args) in SIGNATURES.items():
+        for name, (res, args) in list(SIGNATURES.items()) + list(DCNV2_SIGNATURES.items()):
             fn = getattr(l, name)   # AttributeError if the symbol is not exported
             fn.restype = res
             fn.argtypes = args

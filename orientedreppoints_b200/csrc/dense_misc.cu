@@ -11,6 +11,7 @@
 
 #include "act.cuh"
 #include "common.cuh"
+#include "../../include/orp_b200_dcnv2.h"
 
 namespace orp {
 namespace {
@@ -336,6 +337,23 @@ transpose_kernel(const float *__restrict__ x, int R, int Cc, void *__restrict__ 
     }
 }
 
+// ---- DCNv2 backbone convolutions (deform_conv.py:411-419): conv_offset output [pixels, 27] -> offset [pixels, 18] (channels
+// 0..17 as they are: cat(o1, o2)) and mask [pixels, 9] = sigmoid(channels 18..26).  One element per thread, both sides
+// coalesced.  The sigmoid is taken in fp64 and rounded once, so the mask is the correctly rounded fp32 value up to the
+// fp64 exp's error.
+__global__ void __launch_bounds__(256)
+dcnv2_offset_mask_kernel(const float *__restrict__ om, size_t pixels, float *__restrict__ offset, float *__restrict__ mask)
+{
+    const size_t total = pixels * 27;
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+        const size_t pix = i / 27;
+        const int c = (int)(i - pix * 27);
+        const float v = om[i];
+        if (c < 18) offset[pix * 18 + c] = v;
+        else mask[pix * 9 + (c - 18)] = (float)(1.0 / (1.0 + exp(-(double)v)));
+    }
+}
+
 }  // namespace
 }  // namespace orp
 
@@ -532,6 +550,18 @@ extern "C" int orp_split_to_f32(const void *x_split, long long pixels, int C, fl
     if (rc) return rc;
     split_to_f32_kernel<<<grid_for((size_t)pixels * (C / 8), 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
         static_cast<const __half *>(x_split), (size_t)pixels, C, y);
+    ORP_LAUNCHED();
+    return ORP_OK;
+}
+
+extern "C" int orp_dcnv2_offset_mask(const float *om, long long pixels, float *offset, float *mask, void *stream)
+{
+    if (!om || !offset || !mask || pixels < 0) return fail(ORP_EINVAL, "dcnv2_offset_mask: bad arguments");
+    if (pixels == 0) return ORP_OK;
+    int rc = ensure_device();
+    if (rc) return rc;
+    dcnv2_offset_mask_kernel<<<grid_for((size_t)pixels * 27, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+        om, (size_t)pixels, offset, mask);
     ORP_LAUNCHED();
     return ORP_OK;
 }

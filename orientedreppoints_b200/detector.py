@@ -57,7 +57,8 @@ class EngineF32:
         x[..., :c] = img_nchw.to(self.device, torch.float32).permute(0, 2, 3, 1)
         return x
 
-    def conv(self, x, L, relu=False, residual=None, want_stats=False):
+    def conv(self, x, L, relu=False, residual=None, want_stats=False, out_f32=False):
+        """out_f32: accepted for the tensor-core engines' interface; every output of this engine is fp32"""
         n, h, w, cin = x.shape
         assert cin == L.cin, (cin, L.cin)
         ho = (h + 2 * L.pad - L.kh) // L.stride + 1
@@ -107,7 +108,8 @@ class EngineF32:
 
     def deform_conv(self, x, offset, L, relu=False, mask=None):
         n, h, w, cin = x.shape
-        y = torch.empty((n, h, w, L.cout), dtype=torch.float32, device=self.device)
+        ho, wo = (h + 2 * L.pad - L.kh) // L.stride + 1, (w + 2 * L.pad - L.kw) // L.stride + 1
+        y = torch.empty((n, ho, wo, L.cout), dtype=torch.float32, device=self.device)
         rc = self.lib.orp_deform_conv2d_f32(_lib.ptr(x), n, h, w, cin, _lib.ptr(offset), _lib.ptr(mask), _lib.ptr(L.w),
                                             L.cout, L.kh, L.kw, L.stride, L.pad, 1, _lib.ptr(L.bias), int(relu),
                                             _lib.ptr(y), _lib.current_stream_ptr())
@@ -118,11 +120,14 @@ class EngineF32:
 class OrientedRepPointsDetector:
     """R-50 / R-101 + FPN(GN) + OrientedRepPointsHead, inference only."""
 
-    def __init__(self, state_dict, depth=50, device="cuda", precision="fp32", test_cfg=None):
+    def __init__(self, state_dict, depth=50, device="cuda", precision="fp32", test_cfg=None, dcn=None):
+        """dcn: the ResNet's deformable conv2 layers per stage and block, None / 'DCN' / 'DCNv2' (models.ResNet.dcn_layout,
+        weights.dcn_layout); None: every conv2 is a plain convolution"""
         self.device = torch.device(device)
         if self.device.type == "cuda" and self.device.index is None:      # 'cuda' -> the current device, with its index
             self.device = torch.device("cuda", torch.cuda.current_device())
         self.depth = depth
+        self.dcn = dcn
         self.test_cfg = dict(nms_pre=2000, min_bbox_size=0, score_thr=0.05, nms=dict(type='rnms', iou_thr=0.4),
                              max_per_img=2000)                         # configs/dota/orientedrepoints_r50_demo.py:62-67
         if test_cfg:
@@ -150,6 +155,8 @@ class OrientedRepPointsDetector:
     def _load(self, sd):
         d = self.device
         if self.depth == "swin_tiny":
+            if self.dcn is not None:
+                raise ValueError("dcn describes the deformable layers of a ResNet backbone; the Swin-T backbone has none")
             return self._load_swin(sd)
 
         def folded(conv, bn, stride, pad, pad_cin_to=None):
@@ -157,6 +164,10 @@ class OrientedRepPointsDetector:
                            sd[bn + ".running_mean"].float(), sd[bn + ".running_var"].float())
             return ConvLayer(w, b, stride, pad, d, pad_cin_to)
 
+        layout = self.dcn if self.dcn is not None else tuple((None,) * n for n in STAGE_BLOCKS[self.depth])
+        if tuple(len(s) for s in layout) != STAGE_BLOCKS[self.depth] or \
+                any(k not in (None, 'DCN', 'DCNv2') for s in layout for k in s):
+            raise ValueError("dcn must give None, 'DCN' or 'DCNv2' for each of the %s blocks of R-%d" % (STAGE_BLOCKS[self.depth], self.depth))
         self.stem = folded("backbone.conv1", "backbone.bn1", 2, 3, pad_cin_to=4)
         self.blocks = []
         for li, nblk in enumerate(STAGE_BLOCKS[self.depth]):
@@ -167,6 +178,8 @@ class OrientedRepPointsDetector:
                 blk = dict(c1=folded(p + ".conv1", p + ".bn1", 1, 0), c2=folded(p + ".conv2", p + ".bn2", s, 1),
                            c3=folded(p + ".conv3", p + ".bn3", 1, 0),
                            ds=folded(p + ".downsample.0", p + ".downsample.1", s, 0) if b == 0 else None)
+                blk["dcn"] = layout[li][b]
+                blk["off"] = self._offset_conv(sd, p + ".conv2", blk["dcn"], 64 << li, s)
                 stage.append(blk)
             self.blocks.append(stage)
         self.lat = [(ConvLayer(sd["neck.lateral_convs.%d.conv.weight" % i].float(), None, 1, 0, d),
@@ -174,6 +187,40 @@ class OrientedRepPointsDetector:
         self.fpn = [(ConvLayer(sd["neck.fpn_convs.%d.conv.weight" % i].float(), None, 2 if i >= 3 else 1, 1, d),
                      Norm(sd, "neck.fpn_convs.%d.gn" % i, d)) for i in range(5)]
         self._load_head(sd)
+
+    def _offset_conv(self, sd, conv2, kind, planes, stride):
+        """the conv_offset of a deformable conv2 (deform_conv.py:258-323, 377-446): a plain 3x3 convolution with bias into
+        2 * 9 (DCN) or 3 * 9 (DCNv2) channels; None for a plain conv2.  The state dict must hold exactly the layers `kind`
+        names, in their shapes"""
+        has = conv2 + ".conv_offset.weight" in sd
+        if kind is None:
+            if has:
+                raise ValueError("%s has a conv_offset but dcn names a plain convolution there" % conv2)
+            return None
+        co = 27 if kind == 'DCNv2' else 18
+        if not has or tuple(sd[conv2 + ".conv_offset.weight"].shape) != (co, planes, 3, 3) or \
+                tuple(sd[conv2 + ".conv_offset.bias"].shape) != (co,) or tuple(sd[conv2 + ".weight"].shape) != (planes, planes, 3, 3):
+            raise ValueError("%s is %s: it needs weight [%d,%d,3,3] and conv_offset weight [%d,%d,3,3] / bias [%d]"
+                             % (conv2, kind, planes, planes, co, planes, co))
+        return ConvLayer(sd[conv2 + ".conv_offset.weight"].float(), sd[conv2 + ".conv_offset.bias"].float(), stride, 1,
+                         self.device)
+
+    def _conv2(self, x, blk):
+        """a block's 3x3 convolution + folded bn2 + ReLU.  Deformable (DCN / DCNv2): the offset convolution writes fp32 NHWC
+        [N,Ho,Wo,18|27]; for DCNv2 one kernel splits that into the offsets (channels 0..17) and the sigmoid mask (18..26),
+        ModulatedDeformConvPack.forward; the deformable convolution then samples x with them"""
+        e = self.eng
+        if blk["dcn"] is None:
+            return e.conv(x, blk["c2"], relu=True)
+        om = e.conv(x, blk["off"], out_f32=True)
+        if blk["dcn"] == 'DCN':
+            return e.deform_conv(x, om, blk["c2"], relu=True)
+        n, ho, wo, _ = om.shape
+        off = torch.empty((n, ho, wo, 18), dtype=torch.float32, device=self.device)
+        mask = torch.empty((n, ho, wo, 9), dtype=torch.float32, device=self.device)
+        _lib.check(_lib.lib().orp_dcnv2_offset_mask(_lib.ptr(om), n * ho * wo, _lib.ptr(off), _lib.ptr(mask),
+                                                    _lib.current_stream_ptr()), "orp_dcnv2_offset_mask")
+        return e.deform_conv(x, off, blk["c2"], relu=True, mask=mask)
 
     def _load_head(self, sd):
         d = self.device
@@ -252,7 +299,7 @@ class OrientedRepPointsDetector:
             for blk in stage:
                 idt = x if blk["ds"] is None else e.conv(x, blk["ds"])
                 o = e.conv(x, blk["c1"], relu=True)
-                o = e.conv(o, blk["c2"], relu=True)
+                o = self._conv2(o, blk)
                 x = e.conv(o, blk["c3"], relu=True, residual=idt)
             feats.append(x)
         c3, c4, c5 = feats[1], feats[2], feats[3]

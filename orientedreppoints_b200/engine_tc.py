@@ -244,7 +244,10 @@ class EngineTC:
 
     def deform_conv_multi(self, xs, offsets, L, relu=False, masks=None):
         tc = self._tc(L)
-        ys = [self.alloc(*self.dims(x)[:3], L.cout) for x in xs]
+        ys = []
+        for x in xs:
+            n, h, w, _ = self.dims(x)
+            ys.append(self.alloc(n, (h + 2 * L.pad - L.kh) // L.stride + 1, (w + 2 * L.pad - L.kw) // L.stride + 1, L.cout))
         self._launch(xs, ys, tc, L.cout, L.kh, L.kw, L.w_raw.shape[3], L.stride, L.pad, L.bias, relu, False, True,
                      offsets=offsets, masks=masks)
         return ys

@@ -11,8 +11,9 @@ layer is a kernel of liborp_b200.so.  Training entry points raise NotImplemented
 import torch
 import torch.nn as nn
 
+from .ops.conv import build_conv_layer
 from .ops.conv_module import ConvModule
-from .ops.dcn import DeformConv
+from .ops.dcn import DeformConv, DeformConvPack, ModulatedDeformConvPack
 from .ops.norm import build_norm_layer
 from .utils.registry import Registry, build_from_cfg
 
@@ -56,14 +57,21 @@ class _EngineOnly(nn.Module):
 
 
 class Bottleneck(_EngineOnly):
-    """resnet.py:84-239 (style 'pytorch': the stride sits on the 3x3)"""
+    """resnet.py:84-239 (style 'pytorch': the stride sits on the 3x3).  dcn: the conv2 config of resnet.py:146-168 - a
+    DCN / DCNv2 layer (DeformConvPack / ModulatedDeformConvPack) unless `fallback_on_stride`, which is popped from the dict
+    itself: ResNet hands every block the same dict, so only the first block built from it sees the value"""
     expansion = 4
 
-    def __init__(self, inplanes, planes, stride, downsample, norm_cfg):
+    def __init__(self, inplanes, planes, stride, downsample, norm_cfg, conv_cfg=None, dcn=None):
         super().__init__()
         self.conv1 = nn.Conv2d(inplanes, planes, 1, bias=False)
         self.add_module('bn1', build_norm_layer(norm_cfg, planes, 1)[1])
-        self.conv2 = nn.Conv2d(planes, planes, 3, stride, 1, bias=False)
+        fallback_on_stride = dcn.pop('fallback_on_stride', False) if dcn is not None else False
+        if dcn is None or fallback_on_stride:
+            self.conv2 = nn.Conv2d(planes, planes, 3, stride, 1, bias=False)
+        else:
+            assert conv_cfg is None, 'conv_cfg cannot be None for DCN'
+            self.conv2 = build_conv_layer(dcn, planes, planes, kernel_size=3, stride=stride, padding=1, dilation=1, bias=False)
         self.add_module('bn2', build_norm_layer(norm_cfg, planes, 2)[1])
         self.conv3 = nn.Conv2d(planes, planes * 4, 1, bias=False)
         self.add_module('bn3', build_norm_layer(norm_cfg, planes * 4, 3)[1])
@@ -82,24 +90,38 @@ class ResNet(_EngineOnly):
         if depth not in self.arch_settings:
             raise KeyError('invalid depth {} for resnet'.format(depth))
         if style != 'pytorch' or num_stages != 4 or tuple(strides) != (1, 2, 2, 2) or tuple(dilations) != (1, 1, 1, 1) \
-                or dcn is not None or gcb is not None or gen_attention is not None:
+                or gcb is not None or gen_attention is not None:
             raise NotImplementedError("liborp_b200 builds the configuration of configs/dota/*.py: 4 stages, style 'pytorch', "
-                                      "strides (1,2,2,2), no dilation / DCN / GCB / attention in the backbone")
+                                      "strides (1,2,2,2), no dilation / GCB / attention in the backbone")
+        if dcn is not None:
+            assert isinstance(dcn, dict) and len(stage_with_dcn) == num_stages
+            if dcn.get('deformable_groups', 1) != 1:
+                raise NotImplementedError("liborp_b200 builds backbone DCN / DCNv2 layers with deformable_groups=1, not "
+                                          "deformable_groups=%r" % (dcn['deformable_groups'],))
         self.depth, self.out_indices, self.frozen_stages, self.norm_eval = depth, out_indices, frozen_stages, norm_eval
         self.zero_init_residual = zero_init_residual
+        self.dcn, self.stage_with_dcn = dcn, tuple(stage_with_dcn)
+        self.dcn_cfg = None if dcn is None else dict(dcn)           # as given, before the blocks pop fallback_on_stride
         self.conv1 = nn.Conv2d(in_channels, 64, 7, 2, 3, bias=False)
         self.add_module('bn1', build_norm_layer(norm_cfg, 64, 1)[1])
         inplanes = 64
         for i, nblk in enumerate(self.arch_settings[depth]):
             planes, blocks = 64 << i, []
+            stage_dcn = dcn if self.stage_with_dcn[i] else None      # the one shared dict (resnet.py:402, 146-147)
             for b in range(nblk):
                 stride = strides[i] if b == 0 else 1
                 ds = None
                 if b == 0:
                     ds = nn.Sequential(nn.Conv2d(inplanes, planes * 4, 1, stride, bias=False), build_norm_layer(norm_cfg, planes * 4)[1])
-                blocks.append(Bottleneck(inplanes, planes, stride, ds, norm_cfg))
+                blocks.append(Bottleneck(inplanes, planes, stride, ds, norm_cfg, conv_cfg, stage_dcn))
                 inplanes = planes * 4
             self.add_module('layer%d' % (i + 1), nn.Sequential(*blocks))
+
+    def dcn_layout(self):
+        """per stage, per block: None for a plain conv2, else 'DCN' or 'DCNv2' - what the engine builds for that conv2"""
+        kinds = {ModulatedDeformConvPack: 'DCNv2', DeformConvPack: 'DCN', nn.Conv2d: None}
+        return tuple(tuple(kinds[type(blk.conv2)] for blk in getattr(self, 'layer%d' % (i + 1)))
+                     for i in range(len(self.arch_settings[self.depth])))
 
 
 @BACKBONES.register_module()
@@ -217,7 +239,8 @@ class OrientedRepPointsDetector(nn.Module):
         import os
         if isinstance(self.backbone, ResNet):
             from .weights import random_state_dict
-            sd = random_state_dict(self.backbone.depth, seed=0, reference_init=True, num_classes=self.bbox_head.num_classes)
+            sd = random_state_dict(self.backbone.depth, seed=0, reference_init=True, num_classes=self.bbox_head.num_classes,
+                                   dcn=self.backbone.dcn_cfg, stage_with_dcn=self.backbone.stage_with_dcn)
         else:
             from .swin import random_swin_state_dict
             sd = random_swin_state_dict(0, num_classes=self.bbox_head.num_classes)
@@ -237,9 +260,11 @@ class OrientedRepPointsDetector(nn.Module):
             dev = torch.device(device) if device is not None else next(self.parameters()).device
             if dev.type != 'cuda':
                 raise NotImplementedError("OrientedRepPointsDetector inference needs a CUDA (sm_90a) device: there is no CPU path")
-            depth = self.backbone.depth if isinstance(self.backbone, ResNet) else "swin_tiny"
+            resnet = isinstance(self.backbone, ResNet)
+            depth = self.backbone.depth if resnet else "swin_tiny"
             self._engine = Engine({k: v.detach() for k, v in self.state_dict().items()}, depth, dev, self.precision,
-                                  test_cfg=dict(self.test_cfg) if self.test_cfg else None)
+                                  test_cfg=dict(self.test_cfg) if self.test_cfg else None,
+                                  dcn=self.backbone.dcn_layout() if resnet else None)
         return self._engine
 
     def extract_feat(self, img):

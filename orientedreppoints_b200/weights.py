@@ -28,13 +28,39 @@ def _xavier_uniform(w, gen):
     return w.uniform_(-a, a, generator=gen)
 
 
-def random_state_dict(depth=50, seed=0, reference_init=True, num_classes=16, feat=256, residual_gain=1.0):
+def dcn_layout(depth, dcn=None, stage_with_dcn=(False, False, False, False)):
+    """what ResNet(depth, dcn=dcn, stage_with_dcn=...) builds as each block's conv2, per stage and block: None (nn.Conv2d),
+    'DCN' or 'DCNv2'.  `fallback_on_stride` applies to the first block built from the dcn dict only (ResNet pops it from
+    the dict all blocks share, resnet.py:146-147); `dcn` itself is left as it is."""
+    fallback = bool(dcn.get('fallback_on_stride', False)) if dcn is not None else False
+    layout = []
+    for li, nblk in enumerate(STAGE_BLOCKS[depth]):
+        stage = []
+        for b in range(nblk):
+            if dcn is None or not stage_with_dcn[li]:
+                stage.append(None)
+            else:
+                stage.append(None if fallback else dcn['type'])
+                fallback = False
+        layout.append(tuple(stage))
+    return tuple(layout)
+
+
+def random_state_dict(depth=50, seed=0, reference_init=True, num_classes=16, feat=256, residual_gain=1.0, dcn=None,
+                      stage_with_dcn=(False, False, False, False), dcn_offset_scale=0.0):
     """reference_init=True reproduces the reference's init_weights (incl. zero_init_residual and all-ones
     norm scales); False randomises norm parameters / running statistics so that every branch of the graph
     carries signal (used by the parity tests); residual_gain scales the randomised scale of every block's last norm
-    (1.0 doubles the activation variance per block: fine for 16 blocks, ~1e5 after R-101's 33 - use 0.3 there)."""
+    (1.0 doubles the activation variance per block: fine for 16 blocks, ~1e5 after R-101's 33 - use 0.3 there).
+    dcn / stage_with_dcn: the backbone's deformable conv2 layers as ResNet takes them (dcn_layout).  Their weights follow
+    the reference (resnet.py:474-484): DeformConv.reset_parameters' uniform +-1/sqrt(9 planes) (kaiming_init skips a layer
+    that is not an nn.Conv2d; with reference_init=False the kaiming draw of a plain conv2 instead) and an all-zero
+    conv_offset.  dcn_offset_scale > 0 (tests only) draws conv_offset from N(0, scale^2 / fan_in) with N(0, scale^2) biases
+    instead, so that the samples leave the grid by about `scale` pixels per unit of input and the DCNv2 mask logits vary;
+    with zero offsets a deformable layer is a plain convolution."""
     g = torch.Generator().manual_seed(seed)
     sd = {}
+    layout = dcn_layout(depth, dcn, stage_with_dcn)
 
     def conv(name, cout, cin, k, init, bias=False, std=0.01):
         w = torch.empty(cout, cin, k, k)
@@ -71,7 +97,21 @@ def random_state_dict(depth=50, seed=0, reference_init=True, num_classes=16, fea
             p = "backbone.layer%d.%d" % (li + 1, b)
             conv(p + ".conv1", planes, inplanes, 1, "kaiming")
             norm(p + ".bn1", planes, True)
-            conv(p + ".conv2", planes, planes, 3, "kaiming")
+            kind = layout[li][b]
+            if kind is None:
+                conv(p + ".conv2", planes, planes, 3, "kaiming")
+            else:
+                if reference_init:
+                    bound = 1.0 / math.sqrt(9 * planes)
+                    sd[p + ".conv2.weight"] = torch.empty(planes, planes, 3, 3).uniform_(-bound, bound, generator=g)
+                else:
+                    conv(p + ".conv2", planes, planes, 3, "kaiming")
+                co = 27 if kind == 'DCNv2' else 18
+                w, bias = torch.zeros(co, planes, 3, 3), torch.zeros(co)
+                if dcn_offset_scale > 0:
+                    w.normal_(0, dcn_offset_scale / math.sqrt(9 * planes), generator=g)
+                    bias.normal_(0, dcn_offset_scale, generator=g)
+                sd[p + ".conv2.conv_offset.weight"], sd[p + ".conv2.conv_offset.bias"] = w, bias
             norm(p + ".bn2", planes, True)
             conv(p + ".conv3", planes * 4, planes, 1, "kaiming")
             norm(p + ".bn3", planes * 4, True, zero_gamma=True)           # zero_init_residual, resnet.py:486-491
