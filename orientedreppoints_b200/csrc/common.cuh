@@ -64,6 +64,24 @@ int run_nms(const float *dets, const int32_t *segments, int n, double thr, int i
 
 static inline int ceil_div(long long a, long long b) { return (int)((a + b - 1) / b); }
 
+// key bits that hold every value in [0, v]
+inline int key_bits(uint64_t v)
+{
+    int b = 1;
+    while (b < 64 && (v >> b)) ++b;
+    return b;
+}
+
+// sort key of a float: ascending key order == ascending float order
+__device__ __forceinline__ uint32_t orderable(float f)
+{
+    uint32_t u = __float_as_uint(f);
+    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+
+// multiprocessors of the current device, looked up once per device
+int device_sms(int &sms);
+
 // streaming multiprocessors of an H100 SXM: caps of grid-stride launches are multiples of it
 constexpr int kNumSMs = 132;
 

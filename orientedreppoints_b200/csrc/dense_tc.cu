@@ -1654,20 +1654,6 @@ int launch_bn(const TcParams &P, const ConvPlan &pl, cudaStream_t st)
     return fail(ORP_EINVAL, "conv2d_tc: unsupported tile width");
 }
 
-// multiprocessors of the current device, looked up once per device
-int device_sms(int &sms)
-{
-    static thread_local int dev_known = -1, sms_known = 0;
-    int dev = 0;
-    ORP_CUDA(cudaGetDevice(&dev));
-    if (dev != dev_known) {
-        ORP_CUDA(cudaDeviceGetAttribute(&sms_known, cudaDevAttrMultiProcessorCount, dev));
-        dev_known = dev;
-    }
-    sms = sms_known;
-    return ORP_OK;
-}
-
 // One tensor-core convolution: plan, parameter block and tensor maps, the launch, then the GroupNorm statistics the epilogue
 // could not fuse.
 int conv2d_tc(const ConvDesc &d, void *stream)

@@ -478,13 +478,6 @@ aoe_class_kernel(const double *__restrict__ angle_dif, const int32_t *__restrict
     }
 }
 
-int bits_for(uint64_t v)   // key bits that hold every value in [0, v]
-{
-    int b = 1;
-    while (b < 64 && (v >> b)) ++b;
-    return b;
-}
-
 // The front both evaluations share.  Detections ranked by class, then score (order_out, cls_off_out; ckey2 = class key of
 // each position), ground truth in (class, image) bucket order (gq), and per position the target jm of
 // eval_match_kernel<kVoc>.  With kVoc also the difficult flags, npos per class and the claims (status, claim, npos).
@@ -503,7 +496,7 @@ int eval_front(Scratch &S, cudaStream_t st, const char *who, const int32_t *det_
                size_t min_tmp, int32_t *order_out, int64_t *cls_off_out, EvalFront &F)
 {
     const uint32_t none = (uint32_t)ncls * (uint32_t)nimg;
-    const int cbits = bits_for((uint64_t)ncls), sbits = bits_for((uint64_t)none);
+    const int cbits = key_bits((uint64_t)ncls), sbits = key_bits((uint64_t)none);
     const int T = kEvalThreads, GD = grid_for((size_t)nd, T), GG = grid_for((size_t)ng, T);
 
     uint64_t *skey = S.get<uint64_t>(nd), *skey2 = S.get<uint64_t>(nd);

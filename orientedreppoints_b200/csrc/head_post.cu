@@ -52,11 +52,6 @@ struct Levels {                 // one entry per (view, level), view-major
 static_assert(sizeof(Levels) <= 4000, "the level table is a kernel argument");
 
 __device__ __forceinline__ float sigmoidf_ref(float x) { return 1.0f / (1.0f + expf(-x)); }   // == torch.sigmoid (fp32)
-__device__ __forceinline__ uint32_t orderable(float f)
-{
-    uint32_t u = __float_as_uint(f);
-    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
 
 __global__ void __launch_bounds__(256)
 maxscore_kernel(const __grid_constant__ Levels L, int lev, uint64_t *__restrict__ keys, int32_t *__restrict__ vals)
@@ -309,8 +304,7 @@ int head_post(const char *who, int nviews, int nlevels, const float *const *cls,
     int32_t *sv1 = Sc.get<int32_t>(total), *sv2 = Sc.get<int32_t>(total);
     size_t tb1 = 0, tb2 = 0;
     if (nsort) cub::DeviceRadixSort::SortPairs(nullptr, tb1, k1, k2, v1, v2, (int)nsort, 0, 64, st);
-    int sel_bits = 33;                                                 // (image << 32 | score key)
-    while ((1ll << (sel_bits - 32)) < (long long)B) ++sel_bits;
+    const int sel_bits = 32 + key_bits((uint64_t)B - 1);              // (image << 32 | score key)
     cub::DeviceRadixSort::SortPairs(nullptr, tb2, sk1, sk2, sv1, sv2, (int)total, 0, sel_bits, st);
     uint8_t *tmp = Sc.get<uint8_t>(tb1 > tb2 ? tb1 : tb2);
     if (!tmp || !sv2 || !keep) return fail(ORP_ECUDA, "%s: scratch allocation failed", who);

@@ -30,6 +30,19 @@ int ensure_device()
     return ORP_OK;
 }
 
+int device_sms(int &sms)
+{
+    static thread_local int dev_known = -1, sms_known = 0;
+    int dev = 0;
+    ORP_CUDA(cudaGetDevice(&dev));
+    if (dev != dev_known) {
+        ORP_CUDA(cudaDeviceGetAttribute(&sms_known, cudaDevAttrMultiProcessorCount, dev));
+        dev_known = dev;
+    }
+    sms = sms_known;
+    return ORP_OK;
+}
+
 }  // namespace orp
 
 extern "C" const char *orp_last_error(void) { return orp::g_err; }

@@ -225,13 +225,6 @@ merge_gather_kernel(const uint64_t *__restrict__ key, const int32_t *__restrict_
     }
 }
 
-int key_bits(uint64_t v)   // key bits that hold every value in [0, v]
-{
-    int b = 1;
-    while (b < 64 && (v >> b)) ++b;
-    return b;
-}
-
 }  // namespace
 }  // namespace orp
 

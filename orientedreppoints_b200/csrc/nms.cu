@@ -4,7 +4,7 @@
 // (DOTA_devkit/poly_nms_gpu/poly_nms_kernel.cu:277-329).  The reference materialises an
 // N x N/64 bit matrix (1.25 GB at N = 100k), copies it to the host and scans it there.  Here:
 //
-//   prep     per box: AABB, validity, score key                                   (1 pass, 36 B/box)
+//   prep     per box: score key                                                    (1 pass, 4 B/box)
 //   sort     CUB radix sorts: by score (rank) and by (segment, xmin) (sweep order)
 //   sweep    one warp per box walks its x-interval in the xmin-sorted arrays, lanes test AABBs
 //            (coalesced float4), survivors are compacted into a per-warp shared-memory queue and
@@ -23,6 +23,7 @@
 // Nothing touches the host; no N^2 memory.
 #include <cooperative_groups.h>
 #include <cub/cub.cuh>
+#include <vector>
 
 #include "common.cuh"
 #include "geom.cuh"
@@ -35,12 +36,10 @@ struct NmsCounters {
     unsigned long long pairs_swept, pairs_aabb, pairs_clipped, pairs_fp64, edges, suppressing;
     int overflow;
     int rounds;
-    unsigned int queue;                       // lazy resolve: work-queue fill of the current round
 };
 
-static thread_local orp_nms_stats g_last_stats;
+static thread_local int g_last_n;
 static thread_local cudaEvent_t g_ev[2] = {nullptr, nullptr};
-static thread_local NmsCounters *g_stats_dev = nullptr;   // device copy of the last call
 static thread_local NmsCounters *g_stats_pinned = nullptr;
 static thread_local orp_rnms_plan g_last_plan;
 static thread_local bool g_have_plan = false;
@@ -49,38 +48,18 @@ static thread_local bool g_have_plan = false;
 // exactly zero; like every negative value it keeps the box out of the fp32 bounds and the fast path
 constexpr float kZeroArea = -2.0f;
 
-__device__ __forceinline__ uint32_t orderable(float f)
-{
-    uint32_t u = __float_as_uint(f);
-    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);   // ascending order == ascending float
-}
-
 // ---------------------------------------------------------------------------------------------
-// prep: keys for the two sorts
+// prep: keys for the rank sort
 // ---------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
-nms_prep_kernel(const float *__restrict__ dets, const int32_t *__restrict__ segments, int n,
-                uint32_t *__restrict__ score_key, uint64_t *__restrict__ sweep_key,
-                int32_t *__restrict__ iota)
+nms_prep_kernel(const float *__restrict__ dets, int n, uint32_t *__restrict__ score_key, int32_t *__restrict__ iota)
 {
     int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const float *d = dets + (size_t)i * 9;
-    float x[4], y[4];
-    bool finite = true;
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-        x[k] = d[2 * k]; y[k] = d[2 * k + 1];
-        finite = finite && isfinite(x[k]) && isfinite(y[k]);
-    }
-    float xmin = fminf(fminf(x[0], x[1]), fminf(x[2], x[3]));
     // -0.0 and +0.0 are equal scores: one key, so that the tie rule (lower index first) holds between them
     const float sc = (__float_as_uint(d[8]) << 1) == 0u ? 0.0f : d[8];
     score_key[i] = ~orderable(sc);                         // ascending key == descending score
-    uint32_t seg = segments ? (uint32_t)segments[i] : 0u;
-    // non-finite boxes go to the very end of the sweep order and never take part in it
-    uint64_t key = finite ? (((uint64_t)(seg & 0x7FFFFFFFu) << 32) | orderable(xmin)) : ~0ull;
-    if (sweep_key) sweep_key[i] = key;                     // COMPAT32 bookkeeping only; EXACT64 registers boxes separately
     iota[i] = i;
 }
 
@@ -274,45 +253,18 @@ nms_zero_pending_kernel(const int32_t *__restrict__ zpos, const int32_t *__restr
     if (i < n && zpos[i] >= 0) pending[i] += zbetter[i];
 }
 
-// gather boxes into structure-of-arrays in `perm` order
+// COMPAT32: the tile kernel's inputs (vertices, segment) in `perm` order
 __global__ void __launch_bounds__(256)
-nms_gather_kernel(const float *__restrict__ dets, const int32_t *__restrict__ segments,
-                  const int32_t *__restrict__ perm, const uint64_t *__restrict__ sorted_key,
-                  const int32_t *__restrict__ rank, int n, float4 *__restrict__ aabb,
-                  float4 *__restrict__ v01, float4 *__restrict__ v23, int32_t *__restrict__ rk,
-                  int32_t *__restrict__ sg, float *__restrict__ area, int32_t *__restrict__ nvalid)
+nms_gather_kernel(const float *__restrict__ dets, const int32_t *__restrict__ segments, const int32_t *__restrict__ perm,
+                  int n, float4 *__restrict__ v01, float4 *__restrict__ v23, int32_t *__restrict__ sg)
 {
     int s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= n) return;
     int i = perm[s];
     const float *d = dets + (size_t)i * 9;
-    float c[8];
-#pragma unroll
-    for (int k = 0; k < 8; ++k) c[k] = d[k];
-    float xmin = fminf(fminf(c[0], c[2]), fminf(c[4], c[6]));
-    float xmax = fmaxf(fmaxf(c[0], c[2]), fmaxf(c[4], c[6]));
-    float ymin = fminf(fminf(c[1], c[3]), fminf(c[5], c[7]));
-    float ymax = fmaxf(fmaxf(c[1], c[3]), fmaxf(c[5], c[7]));
-    aabb[s] = make_float4(xmin, ymin, xmax, ymax);
-    v01[s] = make_float4(c[0], c[1], c[2], c[3]);
-    v23[s] = make_float4(c[4], c[5], c[6], c[7]);
-    rk[s] = rank[i];
+    v01[s] = make_float4(d[0], d[1], d[2], d[3]);
+    v23[s] = make_float4(d[4], d[5], d[6], d[7]);
     sg[s] = segments ? segments[i] : 0;
-    // area about the box's own first vertex (small coordinates -> accurate)
-    float ux = c[2] - c[0], uy = c[3] - c[1], vx = c[4] - c[0], vy = c[5] - c[1];
-    float wx = c[6] - c[0], wy = c[7] - c[1];
-    // negative marks "not a convex quadrilateral": such boxes are never pruned by the area bound and
-    // are always decided by the fp64 reference algorithm (which accepts arbitrary quadrilaterals)
-    area[s] = quad_is_convex(c) ? 0.5f * fabsf((ux * vy - uy * vx) + (vx * wy - vy * wx)) : -1.0f;
-    bool valid = sorted_key ? (sorted_key[s] != ~0ull) : true;
-    // first invalid position = number of valid boxes (keys are sorted, invalid ones last)
-    if (sorted_key) {
-        bool prev_valid = (s == 0) ? true : (sorted_key[s - 1] != ~0ull);
-        if (!valid && prev_valid) *nvalid = s;
-        if (valid && s == n - 1) *nvalid = n;
-    } else if (s == 0) {
-        *nvalid = n;
-    }
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -883,6 +835,21 @@ nms_flags_kernel(const uint8_t *__restrict__ status, const int32_t *__restrict__
     }
 }
 
+// A cooperative resolve launch of 256-thread blocks: as many as can be co-resident (at most 4 per SM), no more than `need`
+static int launch_resolve(const void *kernel, int need, void **args, cudaStream_t st)
+{
+    int sms = 0, per_sm = 0;
+    const int rc = device_sms(sms);
+    if (rc) return rc;
+    ORP_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, 256, 0));
+    if (per_sm > 4) per_sm = 4;
+    int grid = sms * (per_sm > 0 ? per_sm : 1);
+    if (grid > need) grid = need;
+    ORP_CUDA(cudaLaunchCooperativeKernel(kernel, dim3(grid), dim3(256), args, 0, st));
+    ORP_LAUNCHED();
+    return ORP_OK;
+}
+
 // flags_out (optional): uint8 [n], 1 where the box (by ORIGINAL index) survives; when given, keep_out /
 // num_out may be NULL and the compaction is skipped (used by the fused head post-processing).
 int run_nms(const float *dets, const int32_t *segments, int n, double thr, int iou_mode, int union_mode,
@@ -917,13 +884,10 @@ int run_nms(const float *dets, const int32_t *segments, int n, double thr, int i
     const int m = n * R;                                          // registration slots
     // sweep keys: R == 1: (segment : xmin), R == 4: (segment(15) : strip(16) : xmin); only the bits in use are sorted -
     // enough of them that the all-ones keys of padding / non-finite boxes still sort after every real key
-    int sweep_bits = 64;
-    if (seg_limit > 0) {
-        int sb = 1;
-        while ((1ll << sb) <= (long long)seg_limit) ++sb;
-        sweep_bits = (R == 1 ? 32 : 48) + sb;
-        if (sweep_bits > 64) sweep_bits = 64;
-    }
+    const int sweep_bits = seg_limit > 0 ? (R == 1 ? 32 : 48) + key_bits((uint64_t)seg_limit) : 64;
+    // zero-area list sort: as many key bits as the segment ids need, plus the all-ones `none` key of every other box
+    const int zbits = seg_limit > 0 ? key_bits((uint64_t)seg_limit) : 32;
+    const uint32_t znone = zbits == 32 ? 0xFFFFFFFFu : (uint32_t)((1ull << zbits) - 1);
     // candidate-pair buffer: grows on overflow (one retry costs a host sync; sized to make that rare).  Callers that
     // forbid the host round trip (no_sync) get the overflow reported on the device through overflow_out instead.
     unsigned long long cap = (unsigned long long)n * 256ull;
@@ -934,40 +898,40 @@ int run_nms(const float *dets, const int32_t *segments, int n, double thr, int i
     g_last_plan.cap_first = g_last_plan.cap_final = (int64_t)cap;
     Scratch S(st);
     const int T = 256, G = ceil_div(n, T), GM = ceil_div(m, T);
+    // both modes.  iota: the rank sort's values, then (EXACT64) the registrations' box ids; v01 / v23: vertices by original
+    // index (EXACT64) or by rank (COMPAT32); list_len: per box, the edges that name it first = the length of its CSR list
     uint32_t *score_key = S.get<uint32_t>(n), *score_key2 = S.get<uint32_t>(n);
-    uint64_t *sweep_key = S.get<uint64_t>(m), *sweep_key2 = S.get<uint64_t>(m);
-    int32_t *iota = S.get<int32_t>(m), *order_r = S.get<int32_t>(n), *perm = S.get<int32_t>(m);
-    int32_t *rank = S.get<int32_t>(n);
-    float4 *aabb = S.get<float4>(m), *v01 = S.get<float4>(n), *v23 = S.get<float4>(n), *baabb = S.get<float4>(n);
-    int32_t *rk = S.get<int32_t>(m), *sg = S.get<int32_t>(m), *nvalid = S.get<int32_t>(1);
-    int4 *meta_s = lazy ? S.get<int4>(m) : nullptr;
-    float *area = S.get<float>(n);
-    int32_t *indeg = S.get<int32_t>(n + 1), *offs = S.get<int32_t>(n + 1), *cursor = S.get<int32_t>(n + 1);
-    uint8_t *status = S.get<uint8_t>(n), *flags = S.get<uint8_t>(n);
+    int32_t *iota = S.get<int32_t>(m), *order_r = S.get<int32_t>(n), *rank = S.get<int32_t>(n);
+    float4 *v01 = S.get<float4>(n), *v23 = S.get<float4>(n);
+    int32_t *list_len = S.get<int32_t>(n + 1), *offs = S.get<int32_t>(n + 1), *cursor = S.get<int32_t>(n + 1);
+    uint8_t *flags = flags_out ? flags_out : S.get<uint8_t>(n);
     int64_t *vals = S.get<int64_t>(n);
-    int *changed = S.get<int>(2);
-    unsigned int *qcount = S.get<unsigned int>(6);                // frontier / queue fills of the lazy resolve
+    NmsCounters *ctr = S.get<NmsCounters>(1);
+    // EXACT64: per box AABB and area, the registrations in sweep order, the lazy resolve's state
+    uint64_t *sweep_key = lazy ? S.get<uint64_t>(m) : nullptr, *sweep_key2 = lazy ? S.get<uint64_t>(m) : nullptr;
+    int32_t *perm = lazy ? S.get<int32_t>(m) : nullptr, *nvalid = lazy ? S.get<int32_t>(1) : nullptr;
+    float4 *baabb = lazy ? S.get<float4>(n) : nullptr, *aabb_s = lazy ? S.get<float4>(m) : nullptr;
+    int4 *meta_s = lazy ? S.get<int4>(m) : nullptr;
+    float *area = lazy ? S.get<float>(n) : nullptr;
+    NmsGlobal *glob = lazy ? S.get<NmsGlobal>(1) : nullptr;
+    unsigned int *qcount = lazy ? S.get<unsigned int>(6) : nullptr;          // frontier / queue fills of the lazy resolve
     int32_t *worklist = lazy ? S.get<int32_t>(4 * (size_t)n) : nullptr;   // kept and suppressed frontiers, [2][n] each
     int32_t *status32 = lazy ? S.get<int32_t>(n) : nullptr, *pending = lazy ? S.get<int32_t>(n) : nullptr;
     int32_t *zlist = zero_rule ? S.get<int32_t>(n) : nullptr, *zpos = zero_rule ? S.get<int32_t>(n) : nullptr;
     int32_t *zhi = zero_rule ? S.get<int32_t>(n) : nullptr, *zbetter = zero_rule ? S.get<int32_t>(n) : nullptr;
-    NmsGlobal *glob = S.get<NmsGlobal>(1);
-    NmsCounters *ctr = S.get<NmsCounters>(1);
-    if (!ctr || !vals || !changed || !qcount || !glob || (lazy && (!worklist || !status32 || !pending || !meta_s)) || (zero_rule && (!zlist || !zpos || !zhi || !zbetter))) return fail(ORP_ECUDA, "orp_rnms: scratch allocation failed");
+    // COMPAT32: segment ids in rank order, the rescanning resolve's status (by rank) and change flags
+    int32_t *sg = lazy ? nullptr : S.get<int32_t>(n);
+    uint8_t *status = lazy ? nullptr : S.get<uint8_t>(n);
+    int *changed = lazy ? nullptr : S.get<int>(2);
+    if (!ctr || !vals || !flags || (lazy && (!worklist || !status32 || !pending || !meta_s || !qcount || !glob)) ||
+        (zero_rule && (!zlist || !zpos || !zhi || !zbetter)) || (!lazy && (!sg || !status || !changed)))
+        return fail(ORP_ECUDA, "orp_rnms: scratch allocation failed");
 
-    // zero-area list sort: as many key bits as the segment ids need, plus the all-ones `none` key of every other box
-    int zbits = 32;
-    if (seg_limit > 0) {
-        zbits = 1;
-        while ((1ll << zbits) <= (long long)seg_limit) ++zbits;
-        if (zbits > 32) zbits = 32;
-    }
-    const uint32_t znone = zbits == 32 ? 0xFFFFFFFFu : (uint32_t)((1ull << zbits) - 1);
     size_t tb1 = 0, tb2 = 0, tb3 = 0, tb4 = 0, tb5 = 0;
     cub::DeviceRadixSort::SortPairs(nullptr, tb1, score_key, score_key2, iota, order_r, n, 0, 32, st);
+    if (lazy) cub::DeviceRadixSort::SortPairs(nullptr, tb2, sweep_key, sweep_key2, iota, perm, m, 0, sweep_bits, st);
     if (zero_rule) cub::DeviceRadixSort::SortPairs(nullptr, tb5, score_key, score_key2, order_r, zlist, n, 0, zbits, st);
-    cub::DeviceRadixSort::SortPairs(nullptr, tb2, sweep_key, sweep_key2, iota, perm, m, 0, sweep_bits, st);
-    cub::DeviceScan::ExclusiveSum(nullptr, tb3, indeg, offs, n + 1, st);
+    cub::DeviceScan::ExclusiveSum(nullptr, tb3, list_len, offs, n + 1, st);
     if (keep_out && num_out) cub::DeviceSelect::Flagged(nullptr, tb4, vals, flags, keep_out, num_out, n, st);
     size_t tb = tb1 > tb2 ? tb1 : tb2;
     tb = tb > tb3 ? tb : tb3;
@@ -977,58 +941,52 @@ int run_nms(const float *dets, const int32_t *segments, int n, double thr, int i
     if (!tmp) return fail(ORP_ECUDA, "orp_rnms: scratch allocation failed");
 
     ORP_CUDA(cudaMemsetAsync(ctr, 0, sizeof(NmsCounters), st));
-    ORP_CUDA(cudaMemsetAsync(indeg, 0, sizeof(int32_t) * (size_t)(n + 1), st));
+    ORP_CUDA(cudaMemsetAsync(list_len, 0, sizeof(int32_t) * (size_t)(n + 1), st));
     ORP_CUDA(cudaMemsetAsync(cursor, 0, sizeof(int32_t) * (size_t)(n + 1), st));
-    ORP_CUDA(cudaMemsetAsync(status, 0, (size_t)n, st));
-    ORP_CUDA(cudaMemsetAsync(changed, 0, 2 * sizeof(int), st));
-    ORP_CUDA(cudaMemsetAsync(qcount, 0, 6 * sizeof(unsigned int), st));
-    if (lazy) {
-        ORP_CUDA(cudaMemsetAsync(status32, 0, sizeof(int32_t) * (size_t)n, st));
-        ORP_CUDA(cudaMemsetAsync(pending, 0, sizeof(int32_t) * (size_t)n, st));
-    }
-    if (zero_rule) ORP_CUDA(cudaMemsetAsync(zpos, 0xFF, sizeof(int32_t) * (size_t)n, st));   // -1: not a zero-area box
-    {
-        NmsGlobal g0;
-        g0.ymin_key = 0xFFFFFFFFu; g0.maxh_bits = 0u; g0.maxabs_bits = 0u; g0.sumh = 0.0; g0.count = 0u;
-        static thread_local NmsGlobal g0_host;                    // source of an async copy must outlive the call
-        g0_host = g0;
-        ORP_CUDA(cudaMemcpyAsync(glob, &g0_host, sizeof(NmsGlobal), cudaMemcpyHostToDevice, st));
-    }
 
-    nms_prep_kernel<<<G, T, 0, st>>>(dets, segments, n, score_key, lazy ? nullptr : sweep_key, iota);
+    nms_prep_kernel<<<G, T, 0, st>>>(dets, n, score_key, iota);
     ORP_LAUNCHED();
     ORP_CUDA(cub::DeviceRadixSort::SortPairs(tmp, tb1, score_key, score_key2, iota, order_r, n, 0, 32, st));
     count_launches(4);
     nms_rank_kernel<<<G, T, 0, st>>>(order_r, n, rank);
     ORP_LAUNCHED();
 
+    if (lazy) {
+        ORP_CUDA(cudaMemsetAsync(pending, 0, sizeof(int32_t) * (size_t)n, st));
+        ORP_CUDA(cudaMemsetAsync(glob, 0, sizeof(NmsGlobal), st));
+        ORP_CUDA(cudaMemsetAsync(&glob->ymin_key, 0xFF, sizeof(glob->ymin_key), st));   // the identity of atomicMin
+        nms_boxes_kernel<<<G, T, 0, st>>>(dets, n, baabb, v01, v23, area, glob);
+        ORP_LAUNCHED();
+        nms_regs_kernel<<<G, T, 0, st>>>(baabb, segments, n, R, glob, sweep_key, iota);
+        ORP_LAUNCHED();
+        ORP_CUDA(cub::DeviceRadixSort::SortPairs(tmp, tb2, sweep_key, sweep_key2, iota, perm, m, 0, sweep_bits, st));
+        count_launches((sweep_bits + 7) / 8);
+        nms_slots_kernel<<<GM, T, 0, st>>>(sweep_key2, perm, baabb, area, rank, m, aabb_s, meta_s, nvalid);
+        ORP_LAUNCHED();
+        if (zero_rule) {
+            ORP_CUDA(cudaMemsetAsync(zpos, 0xFF, sizeof(int32_t) * (size_t)n, st));   // -1: not a zero-area box
+            // score keys are free after the rank sort: they carry the zero-area list keys
+            nms_zero_keys_kernel<<<G, T, 0, st>>>(order_r, segments, v01, v23, glob, n, znone, area, score_key);
+            ORP_LAUNCHED();
+            ORP_CUDA(cub::DeviceRadixSort::SortPairs(tmp, tb5, score_key, score_key2, order_r, zlist, n, 0, zbits, st));
+            count_launches((zbits + 7) / 8);
+            nms_zero_list_kernel<<<G, T, 0, st>>>(score_key2, zlist, n, znone, zpos, zhi, zbetter);
+            ORP_LAUNCHED();
+        }
+    } else {
+        nms_gather_kernel<<<G, T, 0, st>>>(dets, segments, order_r, n, v01, v23, sg);
+        ORP_LAUNCHED();
+    }
+
+    int2 *edges = nullptr;
     for (int attempt = 0; attempt < 6; ++attempt) {
         g_last_plan.attempts = attempt + 1;
         g_last_plan.cap_final = (int64_t)cap;
         // the buffer turns into the resolve's work queue; the zero-area lists can add one pair per box and round to it
-        int2 *edges = S.get<int2>(cap + (zero_rule ? (unsigned long long)n : 0ull));
+        edges = S.get<int2>(cap + (zero_rule ? (unsigned long long)n : 0ull));
         if (!edges) return fail(ORP_ECUDA, "orp_rnms: edge buffer allocation failed");
         if (lazy) {
-            if (attempt == 0) {
-                nms_boxes_kernel<<<G, T, 0, st>>>(dets, n, baabb, v01, v23, area, glob);
-                ORP_LAUNCHED();
-                nms_regs_kernel<<<G, T, 0, st>>>(baabb, segments, n, R, glob, sweep_key, iota);
-                ORP_LAUNCHED();
-                ORP_CUDA(cub::DeviceRadixSort::SortPairs(tmp, tb2, sweep_key, sweep_key2, iota, perm, m, 0, sweep_bits, st));
-                count_launches((sweep_bits + 7) / 8);
-                nms_slots_kernel<<<GM, T, 0, st>>>(sweep_key2, perm, baabb, area, rank, m, aabb, meta_s, nvalid);
-                ORP_LAUNCHED();
-                if (zero_rule) {
-                    // score keys are free after the rank sort: they carry the zero-area list keys
-                    nms_zero_keys_kernel<<<G, T, 0, st>>>(order_r, segments, v01, v23, glob, n, znone, area, score_key);
-                    ORP_LAUNCHED();
-                    ORP_CUDA(cub::DeviceRadixSort::SortPairs(tmp, tb5, score_key, score_key2, order_r, zlist, n, 0, zbits, st));
-                    count_launches((zbits + 7) / 8);
-                    nms_zero_list_kernel<<<G, T, 0, st>>>(score_key2, zlist, n, znone, zpos, zhi, zbetter);
-                    ORP_LAUNCHED();
-                }
-            }
-            SweepParams P{aabb, meta_s, v01, v23, nvalid, glob, R, edges, indeg, pending, cap, ctr, thr, union_mode};
+            SweepParams P{aabb_s, meta_s, v01, v23, nvalid, glob, R, edges, list_len, pending, cap, ctr, thr, union_mode};
             int grid = ceil_div(m, kSweepWarps);
             const int maxgrid = kNumSMs * 8 * 4;
             if (grid > maxgrid) grid = maxgrid;
@@ -1040,16 +998,11 @@ int run_nms(const float *dets, const int32_t *segments, int n, double thr, int i
             ORP_LAUNCHED();
             if (g_timing) ORP_CUDA(cudaEventRecord(g_ev[1], st));
         } else {
-            if (attempt == 0) {
-                nms_gather_kernel<<<G, T, 0, st>>>(dets, segments, order_r, nullptr, rank, n, aabb, v01, v23, rk,
-                                                   sg, area, nvalid);
-                ORP_LAUNCHED();
-            }
             const long long nb = (n + 63) / 64;
             const long long tiles = nb * (nb + 1) / 2;
             if (tiles > 2147483647LL) return fail(ORP_EINVAL, "orp_rnms: n too large for COMPAT32 mode");
             nms_compat_tiles_kernel<<<(unsigned)tiles, 64, 0, st>>>(v01, v23, sg, n, (float)thr, union_mode, edges,
-                                                                    indeg, cap, ctr);
+                                                                    list_len, cap, ctr);
             ORP_LAUNCHED();
         }
         if (cap >= all_pairs || no_sync) break;   // cannot overflow / caller forbids the host round trip
@@ -1063,77 +1016,54 @@ int run_nms(const float *dets, const int32_t *segments, int n, double thr, int i
         cap = h.edges + h.edges / 8 + 1024;
         if (cap > all_pairs) cap = all_pairs;
         ORP_CUDA(cudaMemsetAsync(ctr, 0, sizeof(NmsCounters), st));
-        ORP_CUDA(cudaMemsetAsync(indeg, 0, sizeof(int32_t) * (size_t)(n + 1), st));
+        ORP_CUDA(cudaMemsetAsync(list_len, 0, sizeof(int32_t) * (size_t)(n + 1), st));
         if (lazy) ORP_CUDA(cudaMemsetAsync(pending, 0, sizeof(int32_t) * (size_t)n, st));
     }
-    // the loop above leaves `edges` as the last buffer obtained from S
-    int2 *edges = static_cast<int2 *>(S.ptrs[S.n - 1]);
     if (zero_rule) {
         nms_zero_pending_kernel<<<G, T, 0, st>>>(zpos, zbetter, n, pending);
         ORP_LAUNCHED();
     }
 
-    ORP_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tb3, indeg, offs, n + 1, st));
+    ORP_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tb3, list_len, offs, n + 1, st));
     count_launches(2);
     int32_t *adj = S.get<int32_t>(cap);
     if (!adj) return fail(ORP_ECUDA, "orp_rnms: adjacency allocation failed");
-    {
-        int grid = kNumSMs * 8;
-        nms_scatter_kernel<<<grid, 256, 0, st>>>(edges, ctr, cap, offs, cursor, adj);
-        ORP_LAUNCHED();
+    nms_scatter_kernel<<<kNumSMs * 8, 256, 0, st>>>(edges, ctr, cap, offs, cursor, adj);
+    ORP_LAUNCHED();
+    if (lazy) {
+        ORP_CUDA(cudaMemsetAsync(status32, 0, sizeof(int32_t) * (size_t)n, st));
+        ORP_CUDA(cudaMemsetAsync(qcount, 0, 6 * sizeof(unsigned int), st));
+        // the candidate buffer is free once scattered into the CSR: it becomes the work queue; after the scatter
+        // `cursor` holds every list's length
+        LazyParams LP{offs, adj, cursor, n, status32, pending, ctr, qcount, worklist, worklist + 2 * (size_t)n, edges,
+                      baabb, v01, v23, area, thr, union_mode, zlist, zpos, zhi, getenv("ORP_NMS_TRACE") ? 1 : 0};
+        void *args[] = {&LP};
+        rc = launch_resolve((const void *)nms_resolve_lazy_kernel, ceil_div(n, 8), args, st);   // a warp per frontier box
+    } else {
+        ORP_CUDA(cudaMemsetAsync(status, 0, (size_t)n, st));
+        ORP_CUDA(cudaMemsetAsync(changed, 0, 2 * sizeof(int), st));
+        // a pointer and its cv-qualified version share one representation: these are the kernel's parameters
+        void *args[] = {&offs, &adj, &n, &status, &changed, &ctr};
+        rc = launch_resolve((const void *)nms_resolve_kernel, ceil_div(n, 256), args, st);
     }
-    {
-        int dev = 0, sms = 0, per_sm = 0;
-        ORP_CUDA(cudaGetDevice(&dev));
-        ORP_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-        if (lazy) {
-            ORP_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, nms_resolve_lazy_kernel, 256, 0));
-            if (per_sm > 4) per_sm = 4;
-            int grid = sms * (per_sm > 0 ? per_sm : 1);
-            int need = ceil_div(n, 8);                       // a warp per frontier box
-            if (grid > need) grid = need;
-            // the candidate buffer is free once scattered into the CSR: it becomes the work queue; after the scatter
-            // `cursor` holds every list's length
-            LazyParams LP{offs, adj, cursor, n, status32, pending, ctr, qcount, worklist, worklist + 2 * (size_t)n, edges,
-                          baabb, v01, v23, area, thr, union_mode, zlist, zero_rule ? zpos : nullptr, zhi,
-                          getenv("ORP_NMS_TRACE") ? 1 : 0};
-            void *args[] = {&LP};
-            ORP_CUDA(cudaLaunchCooperativeKernel((void *)nms_resolve_lazy_kernel, dim3(grid), dim3(256), args, 0, st));
-            ORP_LAUNCHED();
-        } else {
-            ORP_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, nms_resolve_kernel, 256, 0));
-            if (per_sm > 4) per_sm = 4;
-            int grid = sms * (per_sm > 0 ? per_sm : 1);
-            int need = ceil_div(n, 256);
-            if (grid > need) grid = need;
-            const int32_t *a0 = offs, *a1 = adj;
-            int a2 = n;
-            volatile uint8_t *a3 = status;
-            int *a4 = changed;
-            NmsCounters *a5 = ctr;
-            void *args[] = {&a0, &a1, &a2, &a3, &a4, &a5};
-            ORP_CUDA(cudaLaunchCooperativeKernel((void *)nms_resolve_kernel, dim3(grid), dim3(256), args, 0, st));
-            ORP_LAUNCHED();
-        }
-    }
+    if (rc) return rc;
     if (overflow_out) {
         nms_export_overflow_kernel<<<1, 1, 0, st>>>(ctr, overflow_out);
         ORP_LAUNCHED();
     }
-    // EXACT64: status is indexed by original box index; COMPAT32: by rank
-    nms_flags_kernel<<<G, T, 0, st>>>(status, lazy ? status32 : nullptr, order_r, rank, n, flags_out ? ORP_ORDER_INDEX_ASC : order,
-                                      flags_out ? flags_out : flags, vals);
+    // EXACT64: status32 is indexed by original box index; COMPAT32: status by rank
+    nms_flags_kernel<<<G, T, 0, st>>>(status, status32, order_r, rank, n, flags_out ? ORP_ORDER_INDEX_ASC : order, flags, vals);
     ORP_LAUNCHED();
     if (keep_out && num_out) {
         if (flags_out && order != ORP_ORDER_INDEX_ASC) return fail(ORP_EINVAL, "orp_rnms: flags_out needs index order");
-        ORP_CUDA(cub::DeviceSelect::Flagged(tmp, tb4, vals, flags_out ? flags_out : flags, keep_out, num_out, n, st));
+        ORP_CUDA(cub::DeviceSelect::Flagged(tmp, tb4, vals, flags, keep_out, num_out, n, st));
         count_launches(3);
     }
 
     // stash the counters for orp_rnms_last_stats (async copy into pinned memory)
     if (!g_stats_pinned) ORP_CUDA(cudaHostAlloc(&g_stats_pinned, sizeof(NmsCounters), cudaHostAllocDefault));
     ORP_CUDA(cudaMemcpyAsync(g_stats_pinned, ctr, sizeof(NmsCounters), cudaMemcpyDeviceToHost, st));
-    g_last_stats.n = n;
+    g_last_n = n;
     return ORP_OK;
 }
 
@@ -1168,7 +1098,7 @@ extern "C" int orp_rnms_last_stats(orp_nms_stats *out)
     out->suppressing = (int64_t)c.suppressing;
     out->overflow = c.overflow;
     out->rounds = c.rounds;
-    out->n = orp::g_last_stats.n;
+    out->n = orp::g_last_n;
     return ORP_OK;
 }
 
@@ -1193,32 +1123,28 @@ extern "C" int orp_poly_nms_host(int *keep_out, int *num_out, const float *polys
     ORP_CUDA(cudaSetDevice(device_id));
     cudaStream_t st;
     ORP_CUDA(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
-    int rc = ORP_OK;
-    float *d = nullptr;
-    int64_t *k = nullptr;
-    int32_t *cnt = nullptr;
-    do {
-        if (cudaMallocAsync(&d, sizeof(float) * 9 * (size_t)polys_num, st) != cudaSuccess ||
-            cudaMallocAsync(&k, sizeof(int64_t) * (size_t)polys_num, st) != cudaSuccess ||
-            cudaMallocAsync(&cnt, sizeof(int32_t), st) != cudaSuccess) { rc = fail(ORP_ECUDA, "orp_poly_nms_host: alloc"); break; }
-        if (cudaMemcpyAsync(d, polys_host, sizeof(float) * 9 * (size_t)polys_num, cudaMemcpyHostToDevice, st) != cudaSuccess) { rc = fail(ORP_ECUDA, "orp_poly_nms_host: h2d"); break; }
+    const int rc = [&]() -> int {
+        Scratch S(st);
+        float *d = S.get<float>(9 * (size_t)polys_num);
+        int64_t *k = S.get<int64_t>(polys_num);
+        int32_t *cnt = S.get<int32_t>(1);
+        if (!d || !k || !cnt) return fail(ORP_ECUDA, "orp_poly_nms_host: alloc");
+        ORP_CUDA(cudaMemcpyAsync(d, polys_host, sizeof(float) * 9 * (size_t)polys_num, cudaMemcpyHostToDevice, st));
         // the caller sorted by score already (poly_nms.pyx:19-21); our stable descending sort
         // reproduces that order exactly, so SCORE_DESC output == positions in the sorted input
-        rc = run_nms(d, nullptr, polys_num, (double)nms_overlap_thresh, ORP_NMS_EXACT64, ORP_UNION_GUARD,
-                     ORP_ORDER_SCORE_DESC, k, cnt, st, nullptr, false, 1, nullptr);
-        if (rc) break;
+        const int err = run_nms(d, nullptr, polys_num, (double)nms_overlap_thresh, ORP_NMS_EXACT64, ORP_UNION_GUARD,
+                                ORP_ORDER_SCORE_DESC, k, cnt, st, nullptr, false, 1, nullptr);
+        if (err) return err;
         int32_t hc = 0;
-        if (cudaMemcpyAsync(&hc, cnt, sizeof(int32_t), cudaMemcpyDeviceToHost, st) != cudaSuccess ||
-            cudaStreamSynchronize(st) != cudaSuccess) { rc = fail(ORP_ECUDA, "orp_poly_nms_host: d2h"); break; }
-        int64_t *hk = (int64_t *)malloc(sizeof(int64_t) * (size_t)(hc > 0 ? hc : 1));
-        if (cudaMemcpy(hk, k, sizeof(int64_t) * (size_t)hc, cudaMemcpyDeviceToHost) != cudaSuccess) { free(hk); rc = fail(ORP_ECUDA, "orp_poly_nms_host: d2h keep"); break; }
+        ORP_CUDA(cudaMemcpyAsync(&hc, cnt, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+        ORP_CUDA(cudaStreamSynchronize(st));
+        std::vector<int64_t> hk(hc > 0 ? hc : 1);
+        ORP_CUDA(cudaMemcpyAsync(hk.data(), k, sizeof(int64_t) * (size_t)hc, cudaMemcpyDeviceToHost, st));
+        ORP_CUDA(cudaStreamSynchronize(st));
         for (int i = 0; i < hc; ++i) keep_out[i] = (int)hk[i];
-        free(hk);
         *num_out = hc;
-    } while (0);
-    if (d) cudaFreeAsync(d, st);
-    if (k) cudaFreeAsync(k, st);
-    if (cnt) cudaFreeAsync(cnt, st);
+        return ORP_OK;
+    }();
     cudaStreamSynchronize(st);
     cudaStreamDestroy(st);
     cudaSetDevice(prev);
