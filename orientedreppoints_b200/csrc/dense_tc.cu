@@ -43,7 +43,6 @@
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
-#include <cstdlib>
 #include <mutex>
 #include <type_traits>
 
@@ -1245,8 +1244,6 @@ constexpr int kEvPool = 1024;
 thread_local cudaEvent_t g_tc_ev[kEvPool][2];
 thread_local int g_tc_ev_created = 0, g_tc_ev_used = 0;
 thread_local double g_tc_flops = 0.0;
-struct TcTrace { int nprob, N, H, W, Cin, Cout, K, stride, deform, BN, tiles, grid; double flops; };
-thread_local TcTrace g_tc_trace[kEvPool];
 // plan of this thread's most recent launch (orp_tc_last_plan)
 thread_local orp_tc_plan g_tc_plan;
 thread_local bool g_tc_plan_set = false;
@@ -1581,8 +1578,6 @@ int launch_tc(const TcParams &P, int stages, int grid, cudaStream_t st, int extr
             fl += 2.0 * P.prob[i].N * P.prob[i].Ho * P.prob[i].Wo * (double)P.Cout *
                   (P.s2d_stem ? 147.0 : (double)P.KH * P.KW * P.Cin);   // algorithmic K, not the padded one
         g_tc_flops += fl;
-        g_tc_trace[slot] = TcTrace{P.nprob, P.prob[0].N, P.prob[0].H, P.prob[0].W, P.Cin, P.Cout, P.KH, P.stride, DEFORM ? 1 : 0,
-                                   BN, P.num_tiles, grid, fl};
     }
     {
         cudaLaunchConfig_t cfg;
@@ -1786,12 +1781,6 @@ extern "C" int orp_tc_timing_collect(float *total_ms, int *launches, double *flo
         ORP_CUDA(cudaEventSynchronize(g_tc_ev[i][1]));
         ORP_CUDA(cudaEventElapsedTime(&ms, g_tc_ev[i][0], g_tc_ev[i][1]));
         sum += ms;
-        if (getenv("ORP_TC_TRACE")) {
-            const TcTrace &t = g_tc_trace[i];
-            fprintf(stderr, "tc[%3d] np=%d N=%d %4dx%-4d Cin=%4d Cout=%4d k=%d s=%d dcn=%d BN=%3d tiles=%5d grid=%3d  %8.1f us  %7.1f TFLOP/s\n",
-                    i, t.nprob, t.N, t.H, t.W, t.Cin, t.Cout, t.K, t.stride, t.deform, t.BN, t.tiles, t.grid, ms * 1e3,
-                    t.flops / (ms * 1e-3) / 1e12);
-        }
     }
     *total_ms = sum; *launches = g_tc_ev_used; *flops = g_tc_flops;
     g_tc_ev_used = 0; g_tc_flops = 0.0;

@@ -655,15 +655,7 @@ struct LazyParams {
     int union_mode;
     const int32_t *zlist, *zpos, *zhi;         // zero-area lists (NULL: none): a zero-area box j also has the worse zero-area
                                                // boxes zlist[zpos[j] + 1 .. zhi[j]) of its segment as candidates
-    int trace;                                 // ORP_NMS_TRACE=1: block 0 prints per-round frontier sizes and phase times
 };
-
-__device__ __forceinline__ unsigned long long gtime()
-{
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
-    return t;
-}
 
 __global__ void __launch_bounds__(256, 4)
 nms_resolve_lazy_kernel(LazyParams P)
@@ -698,7 +690,6 @@ nms_resolve_lazy_kernel(LazyParams P)
         const int32_t *fk = P.fkept + (size_t)cur * P.n, *fs = P.fsup + (size_t)cur * P.n;
         int32_t *fk_next = P.fkept + (size_t)nxt * P.n, *fs_next = P.fsup + (size_t)nxt * P.n;
         unsigned int *qc = &P.counts[4 + cur];
-        const unsigned long long t0 = P.trace ? gtime() : 0ull;
         // ---- phase 1
         for (unsigned int w = gwarp; w < nk + ns; w += nwarps) {
             const bool kept = w < nk;
@@ -745,7 +736,6 @@ nms_resolve_lazy_kernel(LazyParams P)
         __threadfence();
         grid.sync();
         const unsigned int nq = *(volatile unsigned int *)qc;
-        const unsigned long long t1 = P.trace ? gtime() : 0ull;
         if (tid == 0) { P.counts[cur] = 0; P.counts[2 + cur] = 0; P.counts[4 + nxt] = 0; }
         // ---- phase 2 (the loop bound is warp-uniform: pairs the fp32 clip cannot decide are finished by the whole warp)
         for (unsigned int q0 = (unsigned int)(tid - lane); q0 < nq; q0 += nth) {
@@ -793,9 +783,6 @@ nms_resolve_lazy_kernel(LazyParams P)
         ++round;
         __threadfence();
         grid.sync();
-        if (P.trace && tid == 0)
-            printf("round %d: kept %u sup %u queue %u  phase1 %.1f us  phase2 %.1f us\n", round - 1, nk, ns, nq, (t1 - t0) * 1e-3,
-                   (gtime() - t1) * 1e-3);
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
@@ -880,7 +867,7 @@ int run_nms(const float *dets, const int32_t *segments, int n, double thr, int i
     // 5 344 boxes per (image, class)) do not need them.  Segment ids must fit 15 bits next to the 16-bit strip index.
     const long long per_seg = seg_limit > 0 ? (long long)n / seg_limit : (long long)n;
     // (an unknown segment bound, seg_limit <= 0, keeps the strip-less layout whose key carries 31 segment bits)
-    const int R = (lazy && per_seg >= 16384 && seg_limit > 0 && seg_limit <= 32767 && !getenv("ORP_NMS_NO_STRIPS")) ? 4 : 1;
+    const int R = (lazy && per_seg >= 16384 && seg_limit > 0 && seg_limit <= 32767) ? 4 : 1;
     const int m = n * R;                                          // registration slots
     // sweep keys: R == 1: (segment : xmin), R == 4: (segment(15) : strip(16) : xmin); only the bits in use are sorted -
     // enough of them that the all-ones keys of padding / non-finite boxes still sort after every real key
@@ -1036,7 +1023,7 @@ int run_nms(const float *dets, const int32_t *segments, int n, double thr, int i
         // the candidate buffer is free once scattered into the CSR: it becomes the work queue; after the scatter
         // `cursor` holds every list's length
         LazyParams LP{offs, adj, cursor, n, status32, pending, ctr, qcount, worklist, worklist + 2 * (size_t)n, edges,
-                      baabb, v01, v23, area, thr, union_mode, zlist, zpos, zhi, getenv("ORP_NMS_TRACE") ? 1 : 0};
+                      baabb, v01, v23, area, thr, union_mode, zlist, zpos, zhi};
         void *args[] = {&LP};
         rc = launch_resolve((const void *)nms_resolve_lazy_kernel, ceil_div(n, 8), args, st);   // a warp per frontier box
     } else {

@@ -75,114 +75,15 @@ layernorm_kernel(const typename Act<SPLIT>::T *__restrict__ x, int B, int H, int
     }
 }
 
-// qkv: [B,Hp,Wp,3C] (q | k | v, each heads x 32), out: [B,H,W,C] at the ORIGINAL (unshifted, uncropped-away) positions.
-// block = 64 threads = one (window, head); thread t < 49 owns query token t of the window.
-constexpr int kWin = 7, kTok = 49, kHd = 32;
-
-template <bool SPLIT>
-__global__ void __launch_bounds__(64)
-window_attention_kernel(const typename Act<SPLIT>::T *__restrict__ qkv, int B, int H, int W, int Hp, int Wp, int C, int heads,
-                        int shift, const float *__restrict__ bias_table /* [169, heads] */, float scale,
-                        typename Act<SPLIT>::T *__restrict__ out)
-{
-    // K and V of the window's 49 tokens in shared memory as float4 rows: every thread reads the same key at the same time
-    // (a broadcast, conflict free), 8 LDS.128 per 32 multiply-adds
-    __shared__ __align__(16) float sk[kTok][kHd], sv[kTok][kHd];
-    __shared__ int s_src[kTok], s_reg[kTok];
-    __shared__ float s_bias[169];
-    const int nww = Wp / kWin, nwh = Hp / kWin;
-    const int head = blockIdx.y;
-    const int wid = blockIdx.x % (nwh * nww), b = blockIdx.x / (nwh * nww);
-    const int wy = wid / nww, wx = wid - wy * nww;
-    const int t = threadIdx.x;
-    if (t < kTok) {
-        const int ty = t / kWin, tx = t - ty * kWin;
-        const int ys = wy * kWin + ty, xs = wx * kWin + tx;                 // coordinates in the shifted frame
-        int yo = ys + shift, xo = xs + shift;                                // roll(x, -shift): shifted[y] = x[(y + shift) % Hp]
-        if (yo >= Hp) yo -= Hp;
-        if (xo >= Wp) xo -= Wp;
-        s_src[t] = (b * Hp + yo) * Wp + xo;
-        // BasicLayer mask regions (:376-387): slices (0,-7), (-7,-3), (-3,None) of the shifted frame
-        const int hr = ys < Hp - kWin ? 0 : (ys < Hp - shift ? 1 : 2);
-        const int wr = xs < Wp - kWin ? 0 : (xs < Wp - shift ? 1 : 2);
-        s_reg[t] = shift > 0 ? hr * 3 + wr : 0;
-    }
-    for (int i = t; i < 169; i += 64) s_bias[i] = bias_table[i * heads + head];
-    __syncthreads();
-    for (int e = t; e < kTok * 4; e += 64) {                               // (token, 8-channel chunk)
-        const int j = e >> 2, d8 = (e & 3) * 8;
-        float kk[8], vv[8];
-        Act<SPLIT>::ld8(qkv, s_src[j], 3 * C, C + head * kHd + d8, kk);
-        Act<SPLIT>::ld8(qkv, s_src[j], 3 * C, 2 * C + head * kHd + d8, vv);
-#pragma unroll
-        for (int d = 0; d < 8; ++d) { sk[j][d8 + d] = kk[d]; sv[j][d8 + d] = vv[d]; }
-    }
-    __syncthreads();
-    if (t >= kTok) return;
-    float q[kHd];
-#pragma unroll
-    for (int d8 = 0; d8 < kHd; d8 += 8) {
-        float qq[8];
-        Act<SPLIT>::ld8(qkv, s_src[t], 3 * C, head * kHd + d8, qq);
-#pragma unroll
-        for (int d = 0; d < 8; ++d) q[d8 + d] = qq[d] * scale;               // q = q * self.scale (:138)
-    }
-    const int ty = t / kWin, tx = t - ty * kWin;
-    float sc[kTok];
-    float mx = -3.0e38f;
-#pragma unroll
-    for (int j = 0; j < kTok; ++j) {
-        float a = 0.f;
-        const float4 *kr = reinterpret_cast<const float4 *>(sk[j]);
-#pragma unroll
-        for (int d4 = 0; d4 < kHd / 4; ++d4) {
-            const float4 k4 = kr[d4];
-            a = fmaf(q[4 * d4], k4.x, a); a = fmaf(q[4 * d4 + 1], k4.y, a); a = fmaf(q[4 * d4 + 2], k4.z, a); a = fmaf(q[4 * d4 + 3], k4.w, a);
-        }
-        const int jy = j / kWin, jx = j - jy * kWin;
-        a += s_bias[(ty - jy + kWin - 1) * (2 * kWin - 1) + (tx - jx + kWin - 1)];                       // :107-118, :141-144
-        if (s_reg[t] != s_reg[j]) a += -100.0f;                                                            // :388-389
-        sc[j] = a;
-        mx = fmaxf(mx, a);
-    }
-    float den = 0.f;
-#pragma unroll
-    for (int j = 0; j < kTok; ++j) { sc[j] = expf(sc[j] - mx); den += sc[j]; }
-    const float inv = 1.0f / den;
-    float o[kHd];
-#pragma unroll
-    for (int d = 0; d < kHd; ++d) o[d] = 0.f;
-#pragma unroll
-    for (int j = 0; j < kTok; ++j) {
-        const float pj = sc[j] * inv;
-        const float4 *vr = reinterpret_cast<const float4 *>(sv[j]);
-#pragma unroll
-        for (int d4 = 0; d4 < kHd / 4; ++d4) {
-            const float4 v4 = vr[d4];
-            o[4 * d4] = fmaf(pj, v4.x, o[4 * d4]); o[4 * d4 + 1] = fmaf(pj, v4.y, o[4 * d4 + 1]);
-            o[4 * d4 + 2] = fmaf(pj, v4.z, o[4 * d4 + 2]); o[4 * d4 + 3] = fmaf(pj, v4.w, o[4 * d4 + 3]);
-        }
-    }
-    // window_reverse + roll(+shift) + crop: the token returns to its original position if that is inside H x W
-    const int src = s_src[t];
-    const int xo = src % Wp, yo = (src / Wp) % Hp;
-    if (yo < H && xo < W) {
-        const long long otok = ((long long)b * H + yo) * W + xo;
-#pragma unroll
-        for (int d8 = 0; d8 < kHd; d8 += 8) {
-            const float o8[8] = {o[d8], o[d8 + 1], o[d8 + 2], o[d8 + 3], o[d8 + 4], o[d8 + 5], o[d8 + 6], o[d8 + 7]};
-            Act<SPLIT>::st8(out, otok, C, head * kHd + d8, o8);
-        }
-    }
-}
-
 // ---------------------------------------------------------------------------------------------
 // Window attention on the tensor cores (warp-level mma.sync m16n8k16, fp32 accumulation).  One block of four warps per
 // (window, head); warp w owns query rows 16 w .. 16 w + 15 of the window's 49 (padded to 64).  Q, K, V are staged as the 16-bit
 // planes they are stored in (fp16 hi / lo in split mode, bf16 otherwise) - no conversion; S = Q K^T and O = P V are evaluated
 // with the same three-term products as the convolutions (lo x hi, hi x lo, hi x hi), the probabilities P are split into a
 // (hi, lo) pair in registers (both modes), bias + region mask + softmax run on the accumulator fragments in fp32.
+// qkv: [B,Hp,Wp,3C] (q | k | v, each heads x 32), out: [B,H,W,C] at the ORIGINAL (unshifted, uncropped-away) positions.
 // ---------------------------------------------------------------------------------------------
+constexpr int kWin = 7, kTok = 49, kHd = 32;
 constexpr int kAS = 40;            // shared-memory row pitch in 16-bit elements (80 B: conflict-free ldmatrix rows)
 
 __device__ __forceinline__ void ldsm_x4(uint32_t (&r)[4], const void *p)
@@ -528,13 +429,8 @@ static int window_attention_impl(const void *qkv, int B, int H, int W, int Hp, i
     if (rc) return rc;
     dim3 grid(B * (Hp / kWin) * (Wp / kWin), heads);
     typedef typename Act<SPLIT>::T T;
-    static const bool simt = getenv("ORP_SWIN_ATTN_SIMT") != nullptr;      // experiments: the CUDA-core kernel of round 1
-    if (simt)
-        window_attention_kernel<SPLIT><<<grid, 64, 0, static_cast<cudaStream_t>(stream)>>>(
-            static_cast<const T *>(qkv), B, H, W, Hp, Wp, C, heads, shift, bias_table, scale, static_cast<T *>(out));
-    else
-        window_attention_mma_kernel<SPLIT><<<grid, 128, 0, static_cast<cudaStream_t>(stream)>>>(
-            static_cast<const T *>(qkv), B, H, W, Hp, Wp, C, heads, shift, bias_table, scale, static_cast<T *>(out));
+    window_attention_mma_kernel<SPLIT><<<grid, 128, 0, static_cast<cudaStream_t>(stream)>>>(
+        static_cast<const T *>(qkv), B, H, W, Hp, Wp, C, heads, shift, bias_table, scale, static_cast<T *>(out));
     ORP_LAUNCHED();
     return ORP_OK;
 }

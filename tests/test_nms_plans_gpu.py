@@ -24,7 +24,8 @@ ASC, DESC = 0, 1
 PARITY = {
     (1, 1, 0, 0, KEEPS, DESC, 0): "test_scores_and_ties / test_resolve_chains (bench time_nms: rnms_indices, score order)",
     (1, 1, 0, 0, KEEPS, ASC, 0): "test_zero_area_public_entry_points (rnms)",
-    (1, 1, 0, 0, GUARD, DESC, 0): "test_poly_gpu_nms_strips (n = 16383) / test_zero_area_public_entry_points",
+    (1, 1, 0, 0, GUARD, DESC, 0): "test_poly_gpu_nms_strips (n = 16383; the strip-less runs of every strip test) / "
+                                  "test_zero_area_public_entry_points",
     (1, 4, 0, 0, GUARD, DESC, 0): "test_poly_gpu_nms_strips / test_strip_boundaries / test_zero_height_strips",
     (1, 4, 0, 0, KEEPS, DESC, 0): "test_poly_gpu_nms_strips (rnms_indices without segments: bench time_nms, n >= 16384)",
     (1, 1, 0, 0, SUPP, DESC, 0): "test_zero_area_public_entry_points (py_cpu_nms_poly_fast) / test_degenerate_pair_order_and_hulls",
@@ -63,6 +64,14 @@ def _poly_gpu_nms(d, thr):
     from orientedreppoints_b200.dota.poly_nms_gpu import poly_gpu_nms
     keep = np.asarray(poly_gpu_nms(d, thr), np.int64)
     return keep, _plan()
+
+
+def _strip_less(cuda, d, thr):
+    """the same set through orp_rnms as one segment of unknown bound (seg_limit 0): no strips and 64-bit sweep keys, under
+    poly_gpu_nms's guard and score-descending order"""
+    keep, p, _ = _rnms(cuda, d, thr, segments=np.zeros(d.shape[0], np.int32), union=GUARD)
+    _assert_plan(p, (1, 1, 0, 0, GUARD, DESC, 0), seg_limit=0, sweep_bits=64)
+    return keep
 
 
 def _score_order(d):
@@ -246,7 +255,7 @@ def test_inventory_of_bench_nms_workloads(cuda):
 # ================================================================================================= strips
 @pytest.mark.parametrize("n", [16383, 16384, 20000, 100000, 200000])
 @pytest.mark.parametrize("dense", [False, True])
-def test_poly_gpu_nms_strips(cuda, po, monkeypatch, n, dense):
+def test_poly_gpu_nms_strips(cuda, po, n, dense):
     """poly_gpu_nms - and orp_rnms without segments - cut sets of >= 16384 boxes into y strips; the keep list equals the
     oracle's and the strip-less run's"""
     from orientedreppoints_b200.synth import const_density_extent, gen_rotated_boxes
@@ -255,10 +264,7 @@ def test_poly_gpu_nms_strips(cuda, po, monkeypatch, n, dense):
     R = 4 if n >= 16384 else 1
     _assert_plan(p, (1, R, 0, 0, GUARD, DESC, 0), seg_limit=1, n=n)
     assert p["sweep_bits"] == (48 if R == 4 else 32) + 1
-    monkeypatch.setenv("ORP_NMS_NO_STRIPS", "1")
-    flat, p1 = _poly_gpu_nms(d, 0.1)
-    monkeypatch.delenv("ORP_NMS_NO_STRIPS")
-    assert p1["R"] == 1
+    flat = _strip_less(cuda, d, 0.1)
     assert np.array_equal(got, flat)
     kept, pk, _ = _rnms(cuda, d, 0.1)                # NaN keeps: the same decisions on these non-degenerate boxes
     _assert_plan(pk, (1, R, 0, 0, KEEPS, DESC, 0), seg_limit=1)
@@ -268,19 +274,17 @@ def test_poly_gpu_nms_strips(cuda, po, monkeypatch, n, dense):
 
 
 @pytest.mark.parametrize("h", [4, 16, 64])
-def test_strip_boundaries(cuda, po, monkeypatch, h):
+def test_strip_boundaries(cuda, po, h):
     d = _equal_height_boxes(20000, h, seed=h)
     got, p = _poly_gpu_nms(d, 0.1)
     _assert_plan(p, (1, 4, 0, 0, GUARD, DESC, 0))
-    monkeypatch.setenv("ORP_NMS_NO_STRIPS", "1")
-    flat, _ = _poly_gpu_nms(d, 0.1)
-    monkeypatch.delenv("ORP_NMS_NO_STRIPS")
+    flat = _strip_less(cuda, d, 0.1)
     ref = po.nms_poly_f64(d, 0.1, fast=True)
     assert np.array_equal(flat, ref)
     assert np.array_equal(got, ref)
 
 
-def test_tall_box_and_far_coordinates(cuda, po, monkeypatch):
+def test_tall_box_and_far_coordinates(cuda, po):
     """one 8000 px tall box among small ones (strip height = its height / 3), clusters at -5000 and at +16000.  The tall
     box starts half-way into a strip, so it is registered in four strips, and a shorter box with a better score overlaps
     only its top (IoU 0.11): the pair belongs to the tall box's fourth strip"""
@@ -301,9 +305,7 @@ def test_tall_box_and_far_coordinates(cuda, po, monkeypatch):
     assert int(np.floor((yb - y0) / s)) == int(np.floor((ya + 8000 - y0) / s))
     got, p = _poly_gpu_nms(d, 0.1)
     _assert_plan(p, (1, 4, 0, 0, GUARD, DESC, 0))
-    monkeypatch.setenv("ORP_NMS_NO_STRIPS", "1")
-    flat, _ = _poly_gpu_nms(d, 0.1)
-    monkeypatch.delenv("ORP_NMS_NO_STRIPS")
+    flat = _strip_less(cuda, d, 0.1)
     ref = po.nms_poly_f64(d, 0.1, fast=True)
     assert 7 not in ref.tolist()
     assert np.array_equal(got, ref) and np.array_equal(flat, ref)
