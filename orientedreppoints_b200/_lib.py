@@ -1,4 +1,4 @@
-"""ctypes binding of liborp_b200.so (include/orp_b200.h).
+"""ctypes binding of liborp_b200.so (include/orp_b200.h, orp_b200_dcnv2.h, orp_b200_swin.h).
 
 There is NO fallback: if the shared library is missing or a call fails, an exception is raised.
 The library is built in-tree by `python -m orientedreppoints_b200.build` (nvcc, sm_90a).
@@ -146,6 +146,14 @@ DCNV2_SIGNATURES = {
     "orp_dcnv2_offset_mask": (_i, [_vp, ctypes.c_longlong, _vp, _vp, _vp]),
 }
 
+# name -> (restype, argtypes); every symbol include/orp_b200_swin.h declares
+SWIN_SIGNATURES = {
+    "orp_window_attention12_bf16": (_i, [_vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _f, _vp, _vp]),
+    "orp_window_attention12_f16x3": (_i, [_vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _f, _vp, _vp]),
+    "orp_layernorm_wide_bf16": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _f, _i, _i, _vp, _vp]),
+    "orp_layernorm_wide_f16x3": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _f, _i, _i, _vp, _vp]),
+}
+
 _LIB = None
 
 
@@ -162,7 +170,7 @@ def lib():
                 "liborp_b200.so not found at %s - build it with `python -m orientedreppoints_b200.build` "
                 "(there is no CPU or PyTorch fallback for this path)" % LIB_PATH)
         l = ctypes.CDLL(LIB_PATH)
-        for name, (res, args) in list(SIGNATURES.items()) + list(DCNV2_SIGNATURES.items()):
+        for name, (res, args) in list(SIGNATURES.items()) + list(DCNV2_SIGNATURES.items()) + list(SWIN_SIGNATURES.items()):
             fn = getattr(l, name)   # AttributeError if the symbol is not exported
             fn.restype = res
             fn.argtypes = args

@@ -28,6 +28,7 @@ def _headers():
     hs = [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".cuh", ".h"))]
     hs.append(os.path.join(HERE, "..", "include", "orp_b200.h"))
     hs.append(os.path.join(HERE, "..", "include", "orp_b200_dcnv2.h"))
+    hs.append(os.path.join(HERE, "..", "include", "orp_b200_swin.h"))
     return hs
 
 

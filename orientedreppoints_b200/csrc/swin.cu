@@ -1,7 +1,7 @@
-// swin.cu - the non-GEMM pieces of the Swin-T backbone (SURVEY.md section 8 row a2), NHWC bf16 tokens.
+// swin.cu - the non-GEMM pieces of the Swin backbones (SURVEY.md section 8 row a2; Swin-T/S/B/L, 7x7 or 12x12 windows), NHWC tokens.
 //
 // Reference: mmdet/models/backbones/swin_transformer.py - PatchEmbed :430-446, SwinTransformerBlock :199-256
-// (norm1 -> zero pad to multiples of 7 -> cyclic shift -> 7x7 windows -> WindowAttention :122-154 -> reverse ->
+// (norm1 -> zero pad to multiples of the window -> cyclic shift -> windows -> WindowAttention :122-154 -> reverse ->
 // crop -> residual; norm2 -> MLP), PatchMerging :272-299, BasicLayer mask :371-390.  All Linear layers run on the
 // tensor-core convolution kernel (dense_tc.cu) as 1x1 convolutions; here are LayerNorm (optionally scattering into
 // the zero-padded window grid), the window attention itself (shift, relative-position bias and the -100 region mask
@@ -13,6 +13,7 @@
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
+#include "../../include/orp_b200_swin.h"
 #include "act.cuh"
 #include "common.cuh"
 
@@ -32,7 +33,7 @@ layernorm_kernel(const typename Act<SPLIT>::T *__restrict__ x, int B, int H, int
     const long long tok = ((long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)) * tpw + lane / G;
     const long long ntok = (long long)B * H * W;
     const bool live = tok < ntok;
-    float v[kLnChunks][8];                         // 3 chunks per lane up to C = 768 (every block norm of Swin-T: few registers, high occupancy), 6 for the 1536-wide PatchMerging norm
+    float v[kLnChunks][8];                         // 3 chunks per lane up to C = 768 (every block norm of Swin-T: few registers, high occupancy), 6 up to the 1536-wide PatchMerging norm, 12 up to 3072 (Swin-B / L)
     const int chunks = C >> 3;
     float s = 0.f;
 #pragma unroll
@@ -76,15 +77,30 @@ layernorm_kernel(const typename Act<SPLIT>::T *__restrict__ x, int B, int H, int
 }
 
 // ---------------------------------------------------------------------------------------------
-// Window attention on the tensor cores (warp-level mma.sync m16n8k16, fp32 accumulation).  One block of four warps per
-// (window, head); warp w owns query rows 16 w .. 16 w + 15 of the window's 49 (padded to 64).  Q, K, V are staged as the 16-bit
-// planes they are stored in (fp16 hi / lo in split mode, bf16 otherwise) - no conversion; S = Q K^T and O = P V are evaluated
-// with the same three-term products as the convolutions (lo x hi, hi x lo, hi x hi), the probabilities P are split into a
-// (hi, lo) pair in registers (both modes), bias + region mask + softmax run on the accumulator fragments in fp32.
+// Window attention on the tensor cores (warp-level mma.sync m16n8k16, fp32 accumulation), one template over the window side
+// WIN (7: orp_window_attention_*, 12: orp_window_attention12_*).  One block per (window, head), one warp per 16 query rows:
+// the window's WIN^2 tokens are staged as kRows = 16 * ceil(WIN^2 / 16) rows (49 -> 64 in four warps; 144 = 9 x 16 in nine warps,
+// no padded rows).  Q, K, V are staged as the 16-bit planes they are stored in (fp16 hi / lo in split mode, bf16 otherwise) - no
+// conversion; S = Q K^T and O = P V are evaluated with the same three-term products as the convolutions (lo x hi, hi x lo, hi x hi),
+// the probabilities P are split into a (hi, lo) pair in registers (both modes), bias + region mask + softmax run on the
+// accumulator fragments in fp32.
 // qkv: [B,Hp,Wp,3C] (q | k | v, each heads x 32), out: [B,H,W,C] at the ORIGINAL (unshifted, uncropped-away) positions.
 // ---------------------------------------------------------------------------------------------
-constexpr int kWin = 7, kTok = 49, kHd = 32;
+constexpr int kHd = 32;
 constexpr int kAS = 40;            // shared-memory row pitch in 16-bit elements (80 B: conflict-free ldmatrix rows)
+
+template <int WIN>
+struct WinShape {
+    static constexpr int kTok = WIN * WIN;                 // tokens per window
+    static constexpr int kKSteps = (kTok + 15) / 16;       // 16-key steps of O = P V; also the warps (one 16-row query tile each)
+    static constexpr int kRows = 16 * kKSteps;             // staged rows of q, k and v; rows kTok.. are zero
+    static constexpr int kThreads = 32 * kKSteps;
+    static constexpr int kKeyTiles = (kTok + 7) / 8;       // 8-key tiles of S = Q K^T that hold a key (7 of 8 / 18 of 18)
+    static constexpr int kSpan = 2 * WIN - 1;              // relative offsets per axis
+    static constexpr int kBias = kSpan * kSpan;            // rows of the relative-position bias table (169 / 529)
+    // q, k, v, each [planes][kRows][kAS] 16-bit: 30 KiB for w7 in split mode, 67.5 KiB for w12 (dynamic, opted in beyond 48 KiB)
+    static constexpr int smem_bytes(bool split) { return 3 * (split ? 2 : 1) * kRows * kAS * 2; }
+};
 
 __device__ __forceinline__ void ldsm_x4(uint32_t (&r)[4], const void *p)
 {
@@ -123,55 +139,60 @@ __device__ __forceinline__ void split_pair(float x, float y, uint32_t &hi, uint3
     }
 }
 
-template <bool SPLIT>
-__global__ void __launch_bounds__(128)
+template <bool SPLIT, int WIN>
+__global__ void __launch_bounds__(WinShape<WIN>::kThreads)
 window_attention_mma_kernel(const typename Act<SPLIT>::T *__restrict__ qkv, int B, int H, int W, int Hp, int Wp, int C, int heads,
-                            int shift, const float *__restrict__ bias_table /* [169, heads] */, float scale,
+                            int shift, const float *__restrict__ bias_table /* [(2 WIN - 1)^2, heads] */, float scale,
                             typename Act<SPLIT>::T *__restrict__ out)
 {
+    typedef WinShape<WIN> WS;
+    constexpr int kTok = WS::kTok, kRows = WS::kRows, kThreads = WS::kThreads, kSpan = WS::kSpan;
     constexpr int NP = SPLIT ? 2 : 1;                      // 16-bit planes per value
-    __shared__ __align__(16) uint16_t sq[NP][64][kAS], sk[NP][64][kAS], sv[NP][64][kAS];
-    __shared__ int s_src[64], s_reg[64], s_col[64];
-    __shared__ float s_bias[169];
-    const int nww = Wp / kWin, nwh = Hp / kWin;
+    extern __shared__ uint4 s_attn_qkv[];                  // q | k | v, each [NP][kRows][kAS]
+    typedef uint16_t Tile[kRows][kAS];
+    Tile *sq = reinterpret_cast<Tile *>(s_attn_qkv), *sk = sq + NP, *sv = sk + NP;
+    __shared__ int s_src[kRows], s_reg[kRows], s_col[kRows];
+    __shared__ float s_bias[WS::kBias];
+    const int nww = Wp / WIN, nwh = Hp / WIN;
     const int head = blockIdx.y;
     const int wid = blockIdx.x % (nwh * nww), b = blockIdx.x / (nwh * nww);
     const int wy = wid / nww, wx = wid - wy * nww;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    if (tid < 64) {
+    if (tid < kRows) {
         int src = 0, reg = 0;
-        // relative position index (:107-118) = (ty - jy + 6) * 13 + (tx - jx + 6) = [ty * 13 + tx + 84] - [jy * 13 + jx]: one table entry
-        // per token, the softmax loop subtracts
+        // relative position index (:107-118) = (ty - jy + WIN - 1) * kSpan + (tx - jx + WIN - 1) = [ty * kSpan + tx + (WIN - 1) (kSpan + 1)]
+        // - [jy * kSpan + jx]: one table entry per token, the softmax loop subtracts
         const int tq = tid < kTok ? tid : kTok - 1;
-        s_col[tid] = (tq / kWin) * (2 * kWin - 1) + (tq % kWin);
+        s_col[tid] = (tq / WIN) * kSpan + (tq % WIN);
         if (tid < kTok) {
-            const int ty = tid / kWin, tx = tid - ty * kWin;
-            const int ys = wy * kWin + ty, xs = wx * kWin + tx;                 // coordinates in the shifted frame
+            const int ty = tid / WIN, tx = tid - ty * WIN;
+            const int ys = wy * WIN + ty, xs = wx * WIN + tx;                   // coordinates in the shifted frame
             int yo = ys + shift, xo = xs + shift;                                // roll(x, -shift): shifted[y] = x[(y + shift) % Hp]
             if (yo >= Hp) yo -= Hp;
             if (xo >= Wp) xo -= Wp;
             src = (b * Hp + yo) * Wp + xo;
-            // BasicLayer mask regions (:376-387): slices (0,-7), (-7,-3), (-3,None) of the shifted frame
-            const int hr = ys < Hp - kWin ? 0 : (ys < Hp - shift ? 1 : 2);
-            const int wr = xs < Wp - kWin ? 0 : (xs < Wp - shift ? 1 : 2);
+            // BasicLayer mask regions (:376-387): slices (0,-WIN), (-WIN,-shift), (-shift,None) of the shifted frame
+            const int hr = ys < Hp - WIN ? 0 : (ys < Hp - shift ? 1 : 2);
+            const int wr = xs < Wp - WIN ? 0 : (xs < Wp - shift ? 1 : 2);
             reg = shift > 0 ? hr * 3 + wr : 0;
         }
         s_src[tid] = src;
         s_reg[tid] = reg;
     }
-    for (int i = tid; i < 169; i += 128) s_bias[i] = bias_table[i * heads + head];
+    for (int i = tid; i < WS::kBias; i += kThreads) s_bias[i] = bias_table[i * heads + head];
     __syncthreads();
-    // stage the 16-byte chunks of q | k | v (both planes); rows 49..63 are zero
+    // stage the 16-byte chunks of q | k | v (both planes); rows kTok..kRows-1 are zero
     {
-        // thread -> (16-byte chunk c4, plane pl) fixed, rows j = jb + kRows * i, tensor q | k | v: simple addressing, all loads in
+        // thread -> (16-byte chunk c4, plane pl) fixed, rows j = jb + kPass * i, tensor q | k | v: simple addressing, all loads in
         // flight before the first store
-        constexpr int kRows = 128 / (4 * NP);                // rows covered by one pass of the block
-        constexpr int kRowIt = 64 / kRows;
+        constexpr int kPass = kThreads / (4 * NP);           // rows covered by one pass of the block
+        constexpr int kRowIt = kRows / kPass;
+        static_assert(kRowIt * kPass == kRows, "staging passes must tile the rows");
         const int c4 = tid & 3, pl = (tid >> 2) % NP, jb = tid / (4 * NP);
         uint4 val[kRowIt][3];
 #pragma unroll
         for (int i = 0; i < kRowIt; ++i) {
-            const int j = jb + kRows * i;
+            const int j = jb + kPass * i;
             const uint16_t *src = reinterpret_cast<const uint16_t *>(qkv) + ((size_t)s_src[j] * NP + pl) * (size_t)(3 * C) + head * kHd + c4 * 8;
 #pragma unroll
             for (int ten = 0; ten < 3; ++ten)
@@ -179,14 +200,14 @@ window_attention_mma_kernel(const typename Act<SPLIT>::T *__restrict__ qkv, int 
         }
 #pragma unroll
         for (int i = 0; i < kRowIt; ++i) {
-            const int j = jb + kRows * i;
+            const int j = jb + kPass * i;
             *reinterpret_cast<uint4 *>(&sq[pl][j][c4 * 8]) = val[i][0];
             *reinterpret_cast<uint4 *>(&sk[pl][j][c4 * 8]) = val[i][1];
             *reinterpret_cast<uint4 *>(&sv[pl][j][c4 * 8]) = val[i][2];
         }
     }
     __syncthreads();
-    if (warp * 16 >= kTok) return;                         // (never: 4 warps cover rows 0..63, row 48 lives in warp 3)
+    if (warp * 16 >= kTok) return;                         // (never: the warps cover rows 0..kRows-1, the last one holds token kTok-1)
     const int g = lane >> 2, t4 = lane & 3, m0 = warp * 16;
 
     // ---- S = Q K^T (accumulator fragment: [0],[1] = row g, cols 2 t4, +1; [2],[3] = row g + 8)
@@ -195,9 +216,9 @@ window_attention_mma_kernel(const typename Act<SPLIT>::T *__restrict__ qkv, int 
     for (int pl = 0; pl < NP; ++pl)
 #pragma unroll
         for (int ks = 0; ks < 2; ++ks) ldsm_x4(aq[pl][ks], &sq[pl][m0 + (lane & 15)][ks * 16 + (lane >> 4) * 8]);
-    float sc[8][4];
+    float sc[2 * WS::kKSteps][4];
 #pragma unroll
-    for (int j = 0; j < 7; ++j) {
+    for (int j = 0; j < WS::kKeyTiles; ++j) {
         sc[j][0] = sc[j][1] = sc[j][2] = sc[j][3] = 0.f;
         uint32_t bk[NP][4];
 #pragma unroll
@@ -208,14 +229,14 @@ window_attention_mma_kernel(const typename Act<SPLIT>::T *__restrict__ qkv, int 
         }
         mma16816<SPLIT>(sc[j], aq[0][0], bk[0][0], bk[0][1]); mma16816<SPLIT>(sc[j], aq[0][1], bk[0][2], bk[0][3]);
     }
-    // ---- q * scale (:138), + relative position bias (:107-118, :141-144), + region mask (:388-389), softmax over the 49 keys
+    // ---- q * scale (:138), + relative position bias (:107-118, :141-144), + region mask (:388-389), softmax over the kTok keys
     const int r0 = m0 + g, r1 = r0 + 8;
     const int q0 = r0 < kTok ? r0 : kTok - 1, q1 = r1 < kTok ? r1 : kTok - 1;     // padded rows compute on a clamped query, never stored
-    const int rp0 = s_col[q0] + (kWin - 1) * (2 * kWin - 1) + (kWin - 1), rp1 = s_col[q1] + (kWin - 1) * (2 * kWin - 1) + (kWin - 1);
+    const int rp0 = s_col[q0] + (WIN - 1) * kSpan + (WIN - 1), rp1 = s_col[q1] + (WIN - 1) * kSpan + (WIN - 1);
     const int rg0 = s_reg[q0], rg1 = s_reg[q1];
     float mx0 = -3.0e38f, mx1 = -3.0e38f;
 #pragma unroll
-    for (int j = 0; j < 7; ++j) {
+    for (int j = 0; j < WS::kKeyTiles; ++j) {
 #pragma unroll
         for (int u = 0; u < 2; ++u) {
             const int c = 8 * j + 2 * t4 + u;
@@ -236,7 +257,7 @@ window_attention_mma_kernel(const typename Act<SPLIT>::T *__restrict__ qkv, int 
     mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1)); mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
     float den0 = 0.f, den1 = 0.f;
 #pragma unroll
-    for (int j = 0; j < 7; ++j)
+    for (int j = 0; j < WS::kKeyTiles; ++j)
 #pragma unroll
         for (int u = 0; u < 2; ++u) {
             const bool in = (8 * j + 2 * t4 + u) < kTok;
@@ -247,14 +268,16 @@ window_attention_mma_kernel(const typename Act<SPLIT>::T *__restrict__ qkv, int 
     den0 += __shfl_xor_sync(0xffffffffu, den0, 1); den0 += __shfl_xor_sync(0xffffffffu, den0, 2);
     den1 += __shfl_xor_sync(0xffffffffu, den1, 1); den1 += __shfl_xor_sync(0xffffffffu, den1, 2);
     const float inv0 = 1.0f / den0, inv1 = 1.0f / den1;
-    sc[7][0] = sc[7][1] = sc[7][2] = sc[7][3] = 0.f;       // keys 56..63 do not exist
+#pragma unroll
+    for (int j = WS::kKeyTiles; j < 2 * WS::kKSteps; ++j)   // key tiles past the window (w7: keys 56..63) do not exist
+        sc[j][0] = sc[j][1] = sc[j][2] = sc[j][3] = 0.f;
 
     // ---- O = P V: the accumulator fragments of two neighbouring key tiles are the A fragment of one 16-key step
     float o[4][4];
 #pragma unroll
     for (int jn = 0; jn < 4; ++jn) o[jn][0] = o[jn][1] = o[jn][2] = o[jn][3] = 0.f;
 #pragma unroll
-    for (int kk = 0; kk < 4; ++kk) {
+    for (int kk = 0; kk < WS::kKSteps; ++kk) {
         uint32_t ph[4], pl_[4];
         split_pair<SPLIT>(sc[2 * kk][0] * inv0, sc[2 * kk][1] * inv0, ph[0], pl_[0]);
         split_pair<SPLIT>(sc[2 * kk][2] * inv1, sc[2 * kk][3] * inv1, ph[1], pl_[1]);
@@ -383,23 +406,32 @@ subsample2_kernel(const uint16_t *__restrict__ x, int B, int H, int W, int C /* 
 
 using namespace orp;
 
-template <bool SPLIT>
+// WIDE: the 1536 < C <= 3072 PatchMerging norms of Swin-B / Swin-L (orp_layernorm_wide_*), 12 chunks per lane at G = 32
+template <bool SPLIT, bool WIDE>
 static int layernorm_impl(const void *x, int B, int H, int W, int C, const float *gamma, const float *beta, float eps, int Hp, int Wp,
                           void *y, void *stream)
 {
-    if (!x || !y || !gamma || !beta || C < 8 || C > 1536 || (C & 7) || Hp < H || Wp < W) return fail(ORP_EINVAL, "layernorm: C must be a multiple of 8, <= 1536");
+    if (WIDE) {
+        if (!x || !y || !gamma || !beta || C <= 1536 || C > 3072 || (C & 7) || Hp < H || Wp < W)
+            return fail(ORP_EINVAL, "layernorm_wide: C must be a multiple of 8, 1536 < C <= 3072");
+    } else if (!x || !y || !gamma || !beta || C < 8 || C > 1536 || (C & 7) || Hp < H || Wp < W) {
+        return fail(ORP_EINVAL, "layernorm: C must be a multiple of 8, <= 1536");
+    }
     int rc = ensure_device();
     if (rc) return rc;
     const long long ntok = (long long)B * H * W;
     typedef typename Act<SPLIT>::T T;
     // lanes per token: the smallest power of two whose lanes hold the token in at most kLnChunks 16-byte chunks each - for Swin-T's
     // widths (96 / 192 / 384 / 768 -> 4 / 8 / 16 / 32 lanes x 3 chunks) no lane idles
-    const int kLnChunks = C <= 768 ? 3 : 6;
+    const int kLnChunks = WIDE ? 12 : (C <= 768 ? 3 : 6);
     int G = 1;
     while (G < 32 && G * kLnChunks < (C >> 3)) G <<= 1;
     const long long tok_per_block = 8LL * (32 / G);
     const unsigned nblk = (unsigned)((ntok + tok_per_block - 1) / tok_per_block);
-    if (kLnChunks == 3)
+    if (WIDE)
+        layernorm_kernel<SPLIT, 12><<<nblk, 256, 0, static_cast<cudaStream_t>(stream)>>>(static_cast<const T *>(x), B, H, W, C, gamma, beta, eps,
+                                                                                         Hp, Wp, G, static_cast<T *>(y));
+    else if (kLnChunks == 3)
         layernorm_kernel<SPLIT, 3><<<nblk, 256, 0, static_cast<cudaStream_t>(stream)>>>(static_cast<const T *>(x), B, H, W, C, gamma, beta, eps,
                                                                                         Hp, Wp, G, static_cast<T *>(y));
     else
@@ -411,25 +443,48 @@ static int layernorm_impl(const void *x, int B, int H, int W, int C, const float
 extern "C" int orp_layernorm_bf16(const void *x, int B, int H, int W, int C, const float *gamma, const float *beta, float eps,
                                   int Hp, int Wp, void *y, void *stream)
 {
-    return layernorm_impl<false>(x, B, H, W, C, gamma, beta, eps, Hp, Wp, y, stream);
+    return layernorm_impl<false, false>(x, B, H, W, C, gamma, beta, eps, Hp, Wp, y, stream);
 }
 extern "C" int orp_layernorm_f16x3(const void *x, int B, int H, int W, int C, const float *gamma, const float *beta, float eps,
                                    int Hp, int Wp, void *y, void *stream)
 {
-    return layernorm_impl<true>(x, B, H, W, C, gamma, beta, eps, Hp, Wp, y, stream);
+    return layernorm_impl<true, false>(x, B, H, W, C, gamma, beta, eps, Hp, Wp, y, stream);
+}
+extern "C" int orp_layernorm_wide_bf16(const void *x, int B, int H, int W, int C, const float *gamma, const float *beta, float eps,
+                                       int Hp, int Wp, void *y, void *stream)
+{
+    return layernorm_impl<false, true>(x, B, H, W, C, gamma, beta, eps, Hp, Wp, y, stream);
+}
+extern "C" int orp_layernorm_wide_f16x3(const void *x, int B, int H, int W, int C, const float *gamma, const float *beta, float eps,
+                                        int Hp, int Wp, void *y, void *stream)
+{
+    return layernorm_impl<true, true>(x, B, H, W, C, gamma, beta, eps, Hp, Wp, y, stream);
 }
 
-template <bool SPLIT>
+template <bool SPLIT, int WIN>
 static int window_attention_impl(const void *qkv, int B, int H, int W, int Hp, int Wp, int C, int heads, int shift,
                                  const float *bias_table, float scale, void *out, void *stream)
 {
-    if (!qkv || !out || !bias_table || heads * kHd != C || Hp % kWin || Wp % kWin || shift < 0 || shift >= kWin)
-        return fail(ORP_EINVAL, "window_attention: needs 7x7 windows, head_dim 32, padded grid");
+    if (!qkv || !out || !bias_table || heads * kHd != C || Hp % WIN || Wp % WIN || shift < 0 || shift >= WIN)
+        return fail(ORP_EINVAL, WIN == 7 ? "window_attention: needs 7x7 windows, head_dim 32, padded grid"
+                                         : "window_attention12: needs 12x12 windows, head_dim 32, padded grid");
     int rc = ensure_device();
     if (rc) return rc;
-    dim3 grid(B * (Hp / kWin) * (Wp / kWin), heads);
+    typedef WinShape<WIN> WS;
+    constexpr int smem = WS::smem_bytes(SPLIT);
+    auto kern = window_attention_mma_kernel<SPLIT, WIN>;
+    if (smem > 48 * 1024) {                      // opt in to more than 48 KiB of dynamic shared memory, once per device
+        static int opted[64];
+        int dev = 0;
+        ORP_CUDA(cudaGetDevice(&dev));
+        if (dev >= 64 || !__atomic_load_n(&opted[dev], __ATOMIC_ACQUIRE)) {
+            ORP_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+            if (dev < 64) __atomic_store_n(&opted[dev], 1, __ATOMIC_RELEASE);
+        }
+    }
+    dim3 grid(B * (Hp / WIN) * (Wp / WIN), heads);
     typedef typename Act<SPLIT>::T T;
-    window_attention_mma_kernel<SPLIT><<<grid, 128, 0, static_cast<cudaStream_t>(stream)>>>(
+    kern<<<grid, WS::kThreads, smem, static_cast<cudaStream_t>(stream)>>>(
         static_cast<const T *>(qkv), B, H, W, Hp, Wp, C, heads, shift, bias_table, scale, static_cast<T *>(out));
     ORP_LAUNCHED();
     return ORP_OK;
@@ -437,12 +492,22 @@ static int window_attention_impl(const void *qkv, int B, int H, int W, int Hp, i
 extern "C" int orp_window_attention_bf16(const void *qkv, int B, int H, int W, int Hp, int Wp, int C, int heads, int shift,
                                          const float *bias_table, float scale, void *out, void *stream)
 {
-    return window_attention_impl<false>(qkv, B, H, W, Hp, Wp, C, heads, shift, bias_table, scale, out, stream);
+    return window_attention_impl<false, 7>(qkv, B, H, W, Hp, Wp, C, heads, shift, bias_table, scale, out, stream);
 }
 extern "C" int orp_window_attention_f16x3(const void *qkv, int B, int H, int W, int Hp, int Wp, int C, int heads, int shift,
                                           const float *bias_table, float scale, void *out, void *stream)
 {
-    return window_attention_impl<true>(qkv, B, H, W, Hp, Wp, C, heads, shift, bias_table, scale, out, stream);
+    return window_attention_impl<true, 7>(qkv, B, H, W, Hp, Wp, C, heads, shift, bias_table, scale, out, stream);
+}
+extern "C" int orp_window_attention12_bf16(const void *qkv, int B, int H, int W, int Hp, int Wp, int C, int heads, int shift,
+                                           const float *bias_table, float scale, void *out, void *stream)
+{
+    return window_attention_impl<false, 12>(qkv, B, H, W, Hp, Wp, C, heads, shift, bias_table, scale, out, stream);
+}
+extern "C" int orp_window_attention12_f16x3(const void *qkv, int B, int H, int W, int Hp, int Wp, int C, int heads, int shift,
+                                            const float *bias_table, float scale, void *out, void *stream)
+{
+    return window_attention_impl<true, 12>(qkv, B, H, W, Hp, Wp, C, heads, shift, bias_table, scale, out, stream);
 }
 
 template <bool SPLIT>

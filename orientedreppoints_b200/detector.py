@@ -118,15 +118,19 @@ class EngineF32:
 
 
 class OrientedRepPointsDetector:
-    """R-50 / R-101 + FPN(GN) + OrientedRepPointsHead, inference only."""
+    """R-50 / R-101 or Swin-T/S/B/L + FPN(GN) + OrientedRepPointsHead, inference only."""
 
     def __init__(self, state_dict, depth=50, device="cuda", precision="fp32", test_cfg=None, dcn=None):
-        """dcn: the ResNet's deformable conv2 layers per stage and block, None / 'DCN' / 'DCNv2' (models.ResNet.dcn_layout,
+        """depth: 50 / 101 (ResNet), or a Swin backbone - "swin_tiny" (Swin-T, window 7), any key of swin.ARCHS
+        ("swin_small", "swin_base_w12", ...) or a swin.SwinArch.
+        dcn: the ResNet's deformable conv2 layers per stage and block, None / 'DCN' / 'DCNv2' (models.ResNet.dcn_layout,
         weights.dcn_layout); None: every conv2 is a plain convolution"""
+        from .swin import arch_of
         self.device = torch.device(device)
         if self.device.type == "cuda" and self.device.index is None:      # 'cuda' -> the current device, with its index
             self.device = torch.device("cuda", torch.cuda.current_device())
         self.depth = depth
+        self.swin_arch = arch_of(depth)                    # None for a ResNet
         self.dcn = dcn
         self.test_cfg = dict(nms_pre=2000, min_bbox_size=0, score_thr=0.05, nms=dict(type='rnms', iou_thr=0.4),
                              max_per_img=2000)                         # configs/dota/orientedrepoints_r50_demo.py:62-67
@@ -154,9 +158,9 @@ class OrientedRepPointsDetector:
     # ------------------------------------------------------------------ weights
     def _load(self, sd):
         d = self.device
-        if self.depth == "swin_tiny":
+        if self.swin_arch is not None:
             if self.dcn is not None:
-                raise ValueError("dcn describes the deformable layers of a ResNet backbone; the Swin-T backbone has none")
+                raise ValueError("dcn describes the deformable layers of a ResNet backbone; the Swin backbone has none")
             return self._load_swin(sd)
 
         def folded(conv, bn, stride, pad, pad_cin_to=None):
@@ -238,12 +242,12 @@ class OrientedRepPointsDetector:
         self.ref_out = ConvLayer(sd[r + "pts_refine_out.weight"].float(), sd[r + "pts_refine_out.bias"].float(), 1, 0, d)
 
     def _load_swin(self, sd):
-        """Swin-T + FPN(in [192,384,768], start_level 0, no extra convs: P6/P7 = stride-2 subsampling, fpn.py:163-165)"""
-        from .swin import SwinTiny
+        """Swin + FPN(in [2E,4E,8E], start_level 0, no extra convs: P6/P7 = stride-2 subsampling, fpn.py:163-165)"""
+        from .swin import Swin
         d = self.device
         if self.eng.name not in ("bf16", "f16x3"):
-            raise ValueError("the Swin-T backbone runs on the tensor-core engines ('f16x3' or 'bf16')")
-        self.swin = SwinTiny(sd, d, self.eng)
+            raise ValueError("the Swin backbones run on the tensor-core engines ('f16x3' or 'bf16')")
+        self.swin = Swin(sd, d, self.eng, self.swin_arch)
         self.lat = [(ConvLayer(sd["neck.lateral_convs.%d.conv.weight" % i].float(), None, 1, 0, d),
                      Norm(sd, "neck.lateral_convs.%d.gn" % i, d)) for i in range(3)]
         self.fpn = [(ConvLayer(sd["neck.fpn_convs.%d.conv.weight" % i].float(), None, 1, 1, d),
@@ -279,7 +283,7 @@ class OrientedRepPointsDetector:
     def extract_feat(self, img, valid_hw=None):
         """valid_hw: optional device int32 [N,2] extents of uint8 images padded by the test pipeline"""
         e = self.eng
-        if self.depth == "swin_tiny":
+        if self.swin_arch is not None:
             # decoded uint8 tiles: Normalize + ImageToTensor (+ the zero padding outside valid_hw) are fused into the patch gather
             c3, c4, c5 = self.swin.forward(img, self.img_norm_cfg, valid_hw)
             l2 = e.conv_gn(c5, *self.lat[2])

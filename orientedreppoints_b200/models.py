@@ -126,16 +126,25 @@ class ResNet(_EngineOnly):
 
 @BACKBONES.register_module()
 class SwinTransformer(_EngineOnly):
-    """parameter tree of swin_transformer.py:449-631 for the configuration of configs/dota/orientedrepoints_swin_tiny_demo.py"""
+    """parameter tree of swin_transformer.py:449-631 for every architecture the engine builds (swin.check_arch: four stages,
+    head dimension 32, embed_dim a multiple of 32 up to 192, window 7 or 12 - Swin-T/S/B/L), the other arguments as
+    configs/dota/orientedrepoints_swin_tiny_demo.py has them"""
 
     def __init__(self, embed_dim=96, depths=(2, 2, 6, 2), num_heads=(3, 6, 12, 24), window_size=7, mlp_ratio=4., qkv_bias=True,
                  qk_scale=None, drop_rate=0., attn_drop_rate=0., drop_path_rate=0.2, ape=False, patch_norm=True,
                  out_indices=(0, 1, 2, 3), frozen_stages=-1, use_checkpoint=False, pretrain_img_size=224, patch_size=4, in_chans=3):
         super().__init__()
-        if (embed_dim, tuple(depths), tuple(num_heads), window_size, float(mlp_ratio), bool(qkv_bias), bool(ape), bool(patch_norm),
-                tuple(out_indices), patch_size) != (96, (2, 2, 6, 2), (3, 6, 12, 24), 7, 4.0, True, False, True, (1, 2, 3), 4):
-            raise NotImplementedError("liborp_b200 builds Swin-Tiny as configured in configs/dota/orientedrepoints_swin_tiny_demo.py")
+        from .swin import check_arch
+        self.arch = check_arch(embed_dim, depths, num_heads, window_size, qk_scale)
+        for name, value, built in (("mlp_ratio", float(mlp_ratio), 4.0), ("qkv_bias", bool(qkv_bias), True), ("ape", bool(ape), False),
+                                   ("patch_norm", bool(patch_norm), True), ("out_indices", tuple(out_indices), (1, 2, 3)),
+                                   ("patch_size", patch_size, 4), ("in_chans", in_chans, 3)):
+            if value != built:
+                raise NotImplementedError("liborp_b200 builds Swin backbones with %s=%r (configs/dota/orientedrepoints_swin_tiny_demo.py), "
+                                          "not %s=%r" % (name, built, name, value))
         self.out_indices = tuple(out_indices)
+        self.embed_dim, self.depths, self.num_heads = self.arch.embed, self.arch.depths, self.arch.heads
+        self.window_size, self.qk_scale = self.arch.window, self.arch.qk_scale
 
         def block(c, heads):
             m = nn.Module()
@@ -243,7 +252,7 @@ class OrientedRepPointsDetector(nn.Module):
                                    dcn=self.backbone.dcn_cfg, stage_with_dcn=self.backbone.stage_with_dcn)
         else:
             from .swin import random_swin_state_dict
-            sd = random_swin_state_dict(0, num_classes=self.bbox_head.num_classes)
+            sd = random_swin_state_dict(0, num_classes=self.bbox_head.num_classes, arch=self.backbone.arch)
         self.load_state_dict(sd, strict=True)
         if isinstance(pretrained, str) and os.path.isfile(pretrained):
             ck = torch.load(pretrained, map_location='cpu')
@@ -261,7 +270,7 @@ class OrientedRepPointsDetector(nn.Module):
             if dev.type != 'cuda':
                 raise NotImplementedError("OrientedRepPointsDetector inference needs a CUDA (sm_90a) device: there is no CPU path")
             resnet = isinstance(self.backbone, ResNet)
-            depth = self.backbone.depth if resnet else "swin_tiny"
+            depth = self.backbone.depth if resnet else self.backbone.arch
             self._engine = Engine({k: v.detach() for k, v in self.state_dict().items()}, depth, dev, self.precision,
                                   test_cfg=dict(self.test_cfg) if self.test_cfg else None,
                                   dcn=self.backbone.dcn_layout() if resnet else None)
