@@ -1,4 +1,4 @@
-"""ctypes binding of liborp_b200.so (include/orp_b200.h, orp_b200_dcnv2.h, orp_b200_swin.h).
+"""ctypes binding of liborp_b200.so (include/orp_b200.h, orp_b200_dcnv2.h, orp_b200_swin.h, orp_b200_group.h).
 
 There is NO fallback: if the shared library is missing or a call fails, an exception is raised.
 The library is built in-tree by `python -m orientedreppoints_b200.build` (nvcc, sm_90a).
@@ -154,6 +154,14 @@ SWIN_SIGNATURES = {
     "orp_layernorm_wide_f16x3": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _f, _i, _i, _vp, _vp]),
 }
 
+# name -> (restype, argtypes); every symbol include/orp_b200_group.h declares
+GROUP_SIGNATURES = {
+    "orp_group_conv2d_bf16": (_i, [ctypes.POINTER(TcProblem), _vp, _i, _i, _i, _vp, _i, _vp]),
+    "orp_group_conv2d_f16x3": (_i, [ctypes.POINTER(TcProblem), _vp, _i, _i, _i, _vp, _i, _i, _vp]),
+    "orp_group_conv2d_f32": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _i, _vp, _i, _vp, _vp]),
+    "orp_tc_plan_group_conv": (_i, [_i, ctypes.POINTER(TcProblem), _vp, _i, _i, _i, _vp, _i, _i, _i, _i, ctypes.POINTER(TcPlan)]),
+}
+
 _LIB = None
 
 
@@ -170,7 +178,8 @@ def lib():
                 "liborp_b200.so not found at %s - build it with `python -m orientedreppoints_b200.build` "
                 "(there is no CPU or PyTorch fallback for this path)" % LIB_PATH)
         l = ctypes.CDLL(LIB_PATH)
-        for name, (res, args) in list(SIGNATURES.items()) + list(DCNV2_SIGNATURES.items()) + list(SWIN_SIGNATURES.items()):
+        for name, (res, args) in list(SIGNATURES.items()) + list(DCNV2_SIGNATURES.items()) + list(SWIN_SIGNATURES.items()) + \
+                list(GROUP_SIGNATURES.items()):
             fn = getattr(l, name)   # AttributeError if the symbol is not exported
             fn.restype = res
             fn.argtypes = args
@@ -246,6 +255,23 @@ def tc_plan_for(problems, cout, cout_p, kh, kw, cin, stride, pad, *, bias=False,
     check(lib().orp_tc_plan_conv(len(problems), arr, ph, cout, cout_p, kh, kw, cin, stride, pad, ph if bias else None, 0,
                                  int(relu), int(out_f32), int(deform), int(split), stem, ksplit, sms, ctypes.byref(p)),
           "orp_tc_plan_conv")
+    return p.as_dict()
+
+
+def tc_plan_group_for(problems, width, groups, stride, *, split=False, bias=True, relu=1, out_f32=False, residual=0, gn=False,
+                      sms=132):
+    """the plan orp_tc_plan_group_conv reports for a grouped 3x3 launch over problems [(N, H, W), ...] (placeholder pointers,
+    no device needed); residual / gn / out_f32 / several problems are there to be refused"""
+    ph = 256
+    arr = (TcProblem * len(problems))()
+    for q, (n, h, w) in zip(arr, problems):
+        q.x, q.N, q.H, q.W, q.out = ph, n, h, w, ph
+        q.residual_bf16 = ph if residual == 1 else None
+        q.residual_f32 = ph if residual == 2 else None
+        q.gn_stats = ph if gn else None
+    p = TcPlan()
+    check(lib().orp_tc_plan_group_conv(len(problems), arr, ph, width, groups, stride, ph if bias else None, int(relu), int(out_f32),
+                                       int(split), sms, ctypes.byref(p)), "orp_tc_plan_group_conv")
     return p.as_dict()
 
 

@@ -29,6 +29,7 @@ def _headers():
     hs.append(os.path.join(HERE, "..", "include", "orp_b200.h"))
     hs.append(os.path.join(HERE, "..", "include", "orp_b200_dcnv2.h"))
     hs.append(os.path.join(HERE, "..", "include", "orp_b200_swin.h"))
+    hs.append(os.path.join(HERE, "..", "include", "orp_b200_group.h"))
     return hs
 
 

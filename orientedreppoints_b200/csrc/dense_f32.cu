@@ -15,6 +15,7 @@
 // Epilogue fuses bias, residual add, ReLU and the per-(image, group) sum / sum-of-squares that
 // GroupNorm needs (fp32 partials per thread and per CTA, added across CTAs with double atomics).
 #include "common.cuh"
+#include "../../include/orp_b200_group.h"
 
 namespace orp {
 namespace {
@@ -205,6 +206,51 @@ conv_f32_kernel(ConvP p)
     }
 }
 
+// Grouped 3x3 convolution, pad 1 (ResNeXt conv2, resnext.py:44-54): one thread per output pixel and 4 consecutive output
+// channels, which share a group (gw % 4 == 0).  Each sums the 9 gw products of its group in the implicit GEMM's order (taps,
+// then input channels), float4 reads of x and of the weights [C][3][3][gw].
+__global__ void __launch_bounds__(256)
+group_conv3x3_f32_kernel(const float *__restrict__ x, int N, int H, int W, int C, int gw, const float *__restrict__ w, int stride,
+                         int Ho, int Wo, const float *__restrict__ bias, int relu, float *__restrict__ y)
+{
+    const int c4n = C / 4;
+    const size_t total = (size_t)N * Ho * Wo * c4n;
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+        const size_t pix = i / c4n;
+        const int co = (int)(i - pix * c4n) * 4;
+        const int ow = (int)(pix % Wo), oh = (int)((pix / Wo) % Ho), n = (int)(pix / ((size_t)Wo * Ho));
+        const int ci0 = co - co % gw;                             // first input channel of the group
+        float acc[4] = {0.f, 0.f, 0.f, 0.f};
+        for (int kh = 0; kh < 3; ++kh) {
+            const int ih = oh * stride - 1 + kh;
+            if (ih < 0 || ih >= H) continue;
+            for (int kw = 0; kw < 3; ++kw) {
+                const int iw = ow * stride - 1 + kw;
+                if (iw < 0 || iw >= W) continue;
+                const float *xp = x + (((size_t)n * H + ih) * W + iw) * C + ci0;
+                const float *wp = w + ((size_t)co * 9 + kh * 3 + kw) * gw;
+                for (int c = 0; c < gw; c += 4) {
+                    const float4 xv = *reinterpret_cast<const float4 *>(xp + c);
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) {
+                        const float4 wv = *reinterpret_cast<const float4 *>(wp + (size_t)j * 9 * gw + c);
+                        acc[j] = fmaf(xv.x, wv.x, acc[j]);
+                        acc[j] = fmaf(xv.y, wv.y, acc[j]);
+                        acc[j] = fmaf(xv.z, wv.z, acc[j]);
+                        acc[j] = fmaf(xv.w, wv.w, acc[j]);
+                    }
+                }
+            }
+        }
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            if (bias) acc[j] += bias[co + j];
+            if (relu) acc[j] = max_nan(acc[j], 0.f);
+        }
+        *reinterpret_cast<float4 *>(y + pix * C + co) = make_float4(acc[0], acc[1], acc[2], acc[3]);
+    }
+}
+
 // GroupNorm apply (+ optional ReLU, + optional nearest-2x upsampled addend: the FPN top-down step
 // laterals[i-1] += interpolate(laterals[i]) of fpn.py:150-154 fused into the lateral's GN)
 __global__ void __launch_bounds__(256)
@@ -323,6 +369,26 @@ extern "C" int orp_deform_conv2d_f32(const float *x, int N, int H, int W, int Ci
     if (!offset) return fail(ORP_EINVAL, "deform_conv2d_f32: offset is NULL");
     return conv_common("deform_conv2d_f32", x, N, H, W, Cin, w, Cout, KH, KW, stride, pad, dilation, bias, nullptr, relu, y,
                        nullptr, 0, offset, mask, static_cast<cudaStream_t>(stream));
+}
+
+/* see include/orp_b200_group.h */
+extern "C" int orp_group_conv2d_f32(const float *x, int N, int H, int W, int width, int groups, const float *w, int stride,
+                                    const float *bias, int relu, float *y, void *stream)
+{
+    if (!x || !w || !y) return fail(ORP_EINVAL, "group_conv2d_f32: x, w and y must not be NULL");
+    if (N < 1 || H < 1 || W < 1 || width < 1 || stride < 1) return fail(ORP_EINVAL, "group_conv2d_f32: N, H, W, width and stride must be >= 1");
+    if (groups < 1 || width % groups || (width / groups) % 4)
+        return fail(ORP_EINVAL, "group_conv2d_f32: width must divide into groups of a multiple of 4 channels");
+    int rc = ensure_device();
+    if (rc) return rc;
+    const int Ho = conv_out_extent(H, 3, stride, 1, 1), Wo = conv_out_extent(W, 3, stride, 1, 1);
+    const size_t total = (size_t)N * Ho * Wo * (width / 4);
+    int grid = (int)((total + 255) / 256);
+    if (grid > kNumSMs * 16) grid = kNumSMs * 16;
+    group_conv3x3_f32_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(x, N, H, W, width, width / groups, w, stride, Ho, Wo,
+                                                                                  bias, relu, y);
+    ORP_LAUNCHED();
+    return ORP_OK;
 }
 
 extern "C" int orp_gn_apply_f32(const float *x, int N, int H, int W, int C, const double *stats, int groups,

@@ -47,6 +47,7 @@
 #include <type_traits>
 
 #include "common.cuh"
+#include "../../include/orp_b200_group.h"
 #include "wgmma.cuh"
 
 namespace orp {
@@ -113,6 +114,7 @@ struct alignas(64) TcParams {
     int KH, KW, Cin, cin_blocks, stride, pad, Cout, relu;
     int s2d_stem;                             // conv1 in space-to-depth form (host bookkeeping: 147 useful K of 256)
     const float *bias;
+    int gw;                                   // grouped walk: channels per group (host bookkeeping: useful K = 9 gw); 0 otherwise
 };
 
 // ----------------------------------------------------------------------------------------------- PTX
@@ -390,6 +392,14 @@ constexpr int kWalkK = 0;        // one stage per K block and term: bf16, or f16
 constexpr int kWalkNcat = 1;     // f16x3, terms concatenated along N: BN <= 128, TMA epilogue, no residual
 constexpr int kWalkDcat = 2;     // deformable f16x3: one stage carries x_hi | x_lo | w_hi | w_lo of a K block
 constexpr int kWalkKRes = 3;     // kWalkK, then the residual K blocks (res_mma: residual tile x identity into the accumulator)
+// Grouped 3x3 convolution (ResNeXt conv2), BN = 64: output channels [64 j, 64 j + 64) read only input channels
+// [64 j, 64 j + 64), so N tile j walks the 9 taps of channel block j alone (kWalkK's walk with one channel block at channel
+// offset 64 j), and of each 64 x 64 weight tile only the diagonal blocks of width DW = max(16, group width) are multiplied.
+// One walk per DW: the weights carry the zeros of groups narrower than 16 inside the 16 x 16 diagonal blocks.
+constexpr int kWalkG16 = 4;
+constexpr int kWalkG32 = 5;
+constexpr int kWalkG64 = 6;
+__host__ __device__ constexpr int group_dw(int walk) { return walk == kWalkG16 ? 16 : walk == kWalkG32 ? 32 : walk == kWalkG64 ? 64 : 0; }
 
 // accumulator columns [64 G, 64 G + 64) += A * B[rows 64 G ..]^T for G = 0 .. NG - 1: one width-64 MMA per column group
 // (the B rows of group G start 64 rows = 8 KiB further, 512 in the descriptor's address field)
@@ -398,6 +408,20 @@ __device__ __forceinline__ void wgmma_cols64(float (&acc)[R], uint64_t da, uint6
 {
     wgmma_n<64, BF16>(acc_view<32 * G, 32>(acc), da, db + (uint64_t)(G * 512), accumulate);
     if constexpr (G + 1 < NG) wgmma_cols64<NG, BF16, R, G + 1>(acc, da, db, accumulate);
+}
+
+// The MMAs of one grouped K block (64 channels of one tap): k16 slice k of A (32 B further in the swizzled rows, 2 in the
+// descriptor's address field) meets the diagonal block s = 16 k / DW of the weight tile: B rows [DW s, DW s + DW), DW s * 128
+// bytes further (a multiple of 1024: the swizzle pattern is unchanged), DW s * 8 in the address field.  The m64nDW fragment of
+// columns [DW s, DW s + DW) is registers [DW s / 2, DW s / 2 + DW / 2) of the m64n64 fragment the epilogue reads (wgmma.cuh).
+// Every register sees MMAs of the one width DW only.
+template <int DW, bool BF16, int K = 0>
+__device__ __forceinline__ void wgmma_diag(float (&acc)[32], uint64_t da, uint64_t db, int kb)
+{
+    constexpr int S = 16 * K / DW;
+    wgmma_n<DW, BF16>(acc_view<DW / 2 * S, DW / 2>(acc), da + (uint64_t)(K * 2), db + (uint64_t)(DW * S * 8 + K * 2),
+                      (kb | (K % (DW / 16))) ? 1u : 0u);
+    if constexpr (K + 1 < kBK / 16) wgmma_diag<DW, BF16, K + 1>(acc, da, db, kb);
 }
 
 // accumulator (+)= A * B^T over BN columns (dcat walk): one MMA, or at BN = 256 two of 128 columns each - an m64n256 MMA
@@ -437,6 +461,8 @@ conv_tc_kernel(const __grid_constant__ TcParams P, int stages)
     static_assert(!DEFORM || (WALK == kWalkDcat) == SPLIT, "deformable: dcat exactly in f16x3");
     static_assert(DEFORM || WALK != kWalkDcat, "dcat is the deformable walk");
     static_assert(WALK != kWalkKRes || (!DEFORM && !OUT_F32 && BN >= 64), "residual K blocks: TMA-epilogue layers");
+    constexpr int kGroupDW = group_dw(WALK);
+    static_assert(kGroupDW == 0 || (BN == 64 && !DEFORM && !OUT_F32), "grouped walk: one 64-channel block per N tile, 16-bit output");
     constexpr bool kBF16 = !SPLIT;                     // operand type of every MMA
     constexpr int kWTerms = SPLIT ? 2 : 1;             // weight K blocks per (tap, channel block): hi, lo
     constexpr bool kCat = WALK == kWalkNcat || WALK == kWalkDcat;             // a stage holds both halves of both operands
@@ -582,9 +608,10 @@ conv_tc_kernel(const __grid_constant__ TcParams P, int stages)
                     for (int k = 0; k < kBK / 16; ++k) {
                         if constexpr (WALK == kWalkKRes)     // the shape of the residual blocks' MMAs (see there)
                             wgmma_cols64<BN / 64, kBF16>(acc, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (kb | k) ? 1u : 0u);
-                        else
+                        else if constexpr (kGroupDW == 0)
                             wgmma_n<BN, kBF16>(acc, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (kb | k) ? 1u : 0u);
                     }
+                    if constexpr (kGroupDW > 0) wgmma_diag<kGroupDW, kBF16>(acc, da, db, kb);
                 }
                 wgmma_commit();
                 wgmma_wait<1>();
@@ -1009,8 +1036,10 @@ conv_tc_kernel(const __grid_constant__ TcParams P, int stages)
                             tma_load_2d(sa + 2 * kABytes + kBBytes, &P.tmB, &full[r.stage], wblk + kBK, nt * BN);
                         }
                     } else {
+                        // grouped walk: channel block nt, the one the N tile's output channels read
+                        const int a_c = kGroupDW ? nt * kBK : it.cb * kBK;
                         mbar_expect_tx(&full[r.stage], P.b_resident ? kABytes : kABytes + kBBytes);
-                        tma_load_5d(sa, &P.tmA[pi], &full[r.stage], it.cb * kBK, it.term == 1 ? 1 : 0, w0 + kw, h0 + kh, i0);
+                        tma_load_5d(sa, &P.tmA[pi], &full[r.stage], a_c, it.term == 1 ? 1 : 0, w0 + kw, h0 + kh, i0);
                         if (!P.b_resident)
                             tma_load_2d(sa + kABytes, &P.tmB, &full[r.stage], wblk + (it.term == 2 ? kBK : 0), nt * BN);
                     }
@@ -1266,6 +1295,7 @@ struct ConvDesc {
     int wscale_log2;                          // f16x3: power-of-two weight scale
     int stem;                                 // 0, or 2 for conv1 in space-to-depth form (the value orp_tc_plan.stem reports)
     int ksplit;                               // split-K factor, >= 1
+    int gw;                                   // grouped 3x3 convolution (Cin == Cout, groups of gw channels); 0: dense
 };
 
 // how it runs: the plan orp_tc_last_plan reports, plus the tile geometry of every problem (Problem without its pointers)
@@ -1296,6 +1326,17 @@ int check_conv(const ConvDesc &d)
     if (d.ksplit > 1 && (d.nprob != 1 || d.deform || d.stem || !d.out_f32 || (d.KH * d.KW) % d.ksplit || q0.residual_bf16 ||
                          q0.residual_f32 || d.bias || d.relu))
         return fail(ORP_EINVAL, "conv2d_tc: split-K serves one plain problem with an fp32 partial-sum output and taps % ksplit == 0");
+    if (d.gw) {
+        // the grouped walk serves ResNeXt's conv2 only: one problem, 3x3 / pad 1, bias + ReLU, 16-bit output
+        if (d.gw != 4 && d.gw != 8 && d.gw != 16 && d.gw != 32 && d.gw != 64)
+            return fail(ORP_EINVAL, "group_conv2d: group width (width / groups) must be 4, 8, 16, 32 or 64");
+        if (d.Cout % kBK || d.Cin != d.Cout || d.Cout_padded != d.Cout)
+            return fail(ORP_EINVAL, "group_conv2d: width must be a multiple of 64");
+        if (d.nprob != 1 || d.out_f32 || d.deform || d.stem || d.ksplit != 1 || d.relu == 2 || d.KH != 3 || d.KW != 3 || d.pad != 1 ||
+            q0.residual_bf16 || q0.residual_f32 || q0.offset || q0.mask || q0.gn_stats)
+            return fail(ORP_EINVAL, "group_conv2d: one 3x3 / pad 1 problem with a 16-bit output; no residual, fp32 output, GroupNorm "
+                                    "statistics, deformation or split-K");
+    }
     return ORP_OK;
 }
 
@@ -1311,6 +1352,7 @@ int plan_conv(const ConvDesc &d, int sms, ConvPlan &pl)
 
     int BN = 256;
     if (d.Cout_padded % 256) BN = (d.Cout_padded % 128 == 0) ? 128 : (d.Cout_padded % 64 == 0) ? 64 : 32;
+    if (d.gw) BN = 64;                        // grouped walk: one 64-channel block per N tile
     {
         // narrower accumulators when the 128 x BN tiling would leave SMs idle
         long long mtiles = 0;
@@ -1324,7 +1366,7 @@ int plan_conv(const ConvDesc &d, int sms, ConvPlan &pl)
     // fits beside the staged epilogue, a 64 x 256 one does not
     if (d.deform && BN > 128) BN = 128;
     // a partial last channel block is zero-filled by TMA (A operand) and by the weight layout (B operand)
-    const int cin_blocks = (d.Cin + kBK - 1) / kBK;
+    const int cin_blocks = d.gw ? 1 : (d.Cin + kBK - 1) / kBK;     // grouped: the K walk of a tile is its own channel block
     const int n_tiles_n = d.Cout_padded / BN;
     // N-tile pairs: in f16x3 with 16-bit outputs and no GELU (the detector's head) a deformable launch computes two adjacent
     // 128-wide N tiles of an M tile in one CTA, on ONE sampled A operand - every sample is gathered once per M tile instead
@@ -1371,13 +1413,14 @@ int plan_conv(const ConvDesc &d, int sms, ConvPlan &pl)
         if (pl.prob[i].BW * pl.prob[i].BH < 32) gn_ok = false;
     }
     const int gn_fused = (want_gn && gn_ok) ? 1 : 0;
-    const bool mem_bound = any_res || (d.KH * d.KW * (d.Cin / kBK) <= 8);
+    // (grouped: 9 gw products per output - memory-bound at every group width)
+    const bool mem_bound = any_res || d.gw || (d.KH * d.KW * (d.Cin / kBK) <= 8);
     int epi_bufs = mem_bound ? 2 : 1;          // a second staging tile costs compute-bound layers a main-loop stage
     const int epi_merge = (d.split && tma_epi && !frag_epi && (mem_bound || d.stem == 2)) ? 1 : 0;
     // terms concatenated along N for narrow layers (kernel header); the residual / deformable / fp32-output variants keep
     // the K-concatenated walk
     const int dcat = (d.split && d.deform) ? 1 : 0;
-    const int ncat = (d.split && tma_epi && BN <= 128 && !d.deform && !any_res) ? 1 : 0;
+    const int ncat = (d.split && tma_epi && BN <= 128 && !d.deform && !any_res && !d.gw) ? 1 : 0;
     // residual through the tensor core (TMA epilogue only; the staged epilogue adds it itself)
     const int res_mma = (tma_epi && any_res) ? 1 : 0;
     if (res_mma) {
@@ -1432,7 +1475,8 @@ int plan_conv(const ConvDesc &d, int sms, ConvPlan &pl)
 int make_params(const ConvDesc &d, const ConvPlan &pl, TcParams &P)
 {
     memset(&P, 0, sizeof(P));
-    P.nprob = d.nprob; P.KH = d.KH; P.KW = d.KW; P.Cin = d.Cin; P.cin_blocks = (d.Cin + kBK - 1) / kBK;
+    P.nprob = d.nprob; P.KH = d.KH; P.KW = d.KW; P.Cin = d.Cin; P.cin_blocks = d.gw ? 1 : (d.Cin + kBK - 1) / kBK;
+    P.gw = d.gw;
     P.stride = d.stride; P.pad = d.pad;
     P.Cout = d.Cout; P.relu = d.relu; P.bias = d.bias; P.s2d_stem = (d.stem == 2) ? 1 : 0;
     P.split = d.split ? 1 : 0;
@@ -1576,7 +1620,7 @@ int launch_tc(const TcParams &P, int stages, int grid, cudaStream_t st, int extr
         double fl = 0;
         for (int i = 0; i < P.nprob; ++i)
             fl += 2.0 * P.prob[i].N * P.prob[i].Ho * P.prob[i].Wo * (double)P.Cout *
-                  (P.s2d_stem ? 147.0 : (double)P.KH * P.KW * P.Cin);   // algorithmic K, not the padded one
+                  (P.s2d_stem ? 147.0 : (double)P.KH * P.KW * (P.gw ? P.gw : P.Cin));   // algorithmic K, not the padded one
         g_tc_flops += fl;
     }
     {
@@ -1614,6 +1658,20 @@ int launch_plan(const TcParams &P, int stages, int grid, cudaStream_t st, int ex
                            : launch_tc<BN, OUT_F32, true, false, kWalkK>(P, stages, grid, st, extra_bytes);
         }
     } else {
+        if (P.gw) {
+            if constexpr (BN == 64 && !OUT_F32) {
+                if (P.ncat || P.res_mma) return fail(ORP_EINVAL, "group_conv2d: grouped plan with ncat or a residual");
+                if (P.gw <= 16)
+                    return P.split ? launch_tc<64, false, false, true, kWalkG16>(P, stages, grid, st, extra_bytes)
+                                   : launch_tc<64, false, false, false, kWalkG16>(P, stages, grid, st, extra_bytes);
+                if (P.gw == 32)
+                    return P.split ? launch_tc<64, false, false, true, kWalkG32>(P, stages, grid, st, extra_bytes)
+                                   : launch_tc<64, false, false, false, kWalkG32>(P, stages, grid, st, extra_bytes);
+                return P.split ? launch_tc<64, false, false, true, kWalkG64>(P, stages, grid, st, extra_bytes)
+                               : launch_tc<64, false, false, false, kWalkG64>(P, stages, grid, st, extra_bytes);
+            }
+            return fail(ORP_EINVAL, "group_conv2d: grouped plan outside BN 64 with a 16-bit output");
+        }
         if (P.ncat && P.res_mma) return fail(ORP_EINVAL, "conv2d_tc: ncat plan with a residual");
         if (P.ncat) {
             if constexpr (!OUT_F32 && BN >= 64 && BN <= 128) {
@@ -1842,6 +1900,42 @@ extern "C" int orp_conv2d_f16x3(int nprob, const orp_tc_problem *probs, const vo
     return conv2d_tc(ConvDesc{nprob, probs, w_split, Cout, Cout_padded, KH, KW, Cin, stride, pad, bias, relu, out_f32, deform, 1,
                               wscale_log2, 0, 1},
                      stream);
+}
+
+// ResNeXt conv2 (grouped 3x3, pad 1) as the descriptor of the grouped walk; groups < 1 or not dividing width: gw 0 -> refused
+// by check_conv through the group-width test
+ConvDesc group_desc(const orp_tc_problem *probs, int nprob, const void *w, int width, int groups, int stride, const float *bias,
+                    int relu, int out_f32, int split, int wscale_log2)
+{
+    const int gw = (groups >= 1 && width % groups == 0) ? width / groups : -1;
+    return ConvDesc{nprob, probs, w, width, width, 3, 3, width, stride, 1, bias, relu, out_f32, 0, split, split ? wscale_log2 : 0, 0,
+                    1, gw};
+}
+
+/* see include/orp_b200_group.h */
+extern "C" int orp_group_conv2d_bf16(const orp_tc_problem *prob, const void *w, int width, int groups, int stride, const float *bias,
+                                     int relu, void *stream)
+{
+    return conv2d_tc(group_desc(prob, 1, w, width, groups, stride, bias, relu, 0, 0, 0), stream);
+}
+
+/* see include/orp_b200_group.h */
+extern "C" int orp_group_conv2d_f16x3(const orp_tc_problem *prob, const void *w_split, int width, int groups, int stride,
+                                      const float *bias, int wscale_log2, int relu, void *stream)
+{
+    return conv2d_tc(group_desc(prob, 1, w_split, width, groups, stride, bias, relu, 0, 1, wscale_log2), stream);
+}
+
+/* see include/orp_b200_group.h */
+extern "C" int orp_tc_plan_group_conv(int nprob, const orp_tc_problem *probs, const void *w, int width, int groups, int stride,
+                                      const float *bias, int relu, int out_f32, int split, int sms, orp_tc_plan *out)
+{
+    if (!out || sms < 1) return fail(ORP_EINVAL, "orp_tc_plan_group_conv: bad arguments");
+    ConvPlan pl;
+    const int rc = plan_conv(group_desc(probs, nprob, w, width, groups, stride, bias, relu, out_f32, split ? 1 : 0, 0), sms, pl);
+    if (rc) return rc;
+    *out = pl.rep;
+    return ORP_OK;
 }
 
 extern "C" int orp_stem_conv_s2d_f16x3(const void *x_s2d, int N, int H, int W, const void *w_split, const float *bias,

@@ -9,6 +9,23 @@
 namespace orp {
 
 template <bool BF16>
+__device__ __forceinline__ void wgmma_n16(float (&d)[8], uint64_t da, uint64_t db, uint32_t accumulate)
+{
+    if constexpr (BF16)
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+            : "l"(da), "l"(db), "r"(accumulate));
+    else
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+            : "l"(da), "l"(db), "r"(accumulate));
+}
+
+template <bool BF16>
 __device__ __forceinline__ void wgmma_n32(float (&d)[16], uint64_t da, uint64_t db, uint32_t accumulate)
 {
     if constexpr (BF16)
@@ -79,8 +96,9 @@ __device__ __forceinline__ void wgmma_n256(float (&d)[128], uint64_t da, uint64_
 template <int N, bool BF16>
 __device__ __forceinline__ void wgmma_n(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t accumulate)
 {
-    static_assert(N == 32 || N == 64 || N == 128 || N == 256, "wgmma_n: unsupported width");
-    if constexpr (N == 32) wgmma_n32<BF16>(d, da, db, accumulate);
+    static_assert(N == 16 || N == 32 || N == 64 || N == 128 || N == 256, "wgmma_n: unsupported width");
+    if constexpr (N == 16) wgmma_n16<BF16>(d, da, db, accumulate);
+    else if constexpr (N == 32) wgmma_n32<BF16>(d, da, db, accumulate);
     else if constexpr (N == 64) wgmma_n64<BF16>(d, da, db, accumulate);
     else if constexpr (N == 128) wgmma_n128<BF16>(d, da, db, accumulate);
     else wgmma_n256<BF16>(d, da, db, accumulate);

@@ -16,7 +16,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .weights import STAGE_BLOCKS, fold_bn
+from .weights import STAGE_BLOCKS, block_width, check_groups, fold_bn
 
 STRIDES = (8, 16, 32, 64, 128)
 
@@ -106,6 +106,15 @@ class EngineF32:
         _lib.check(rc, "orp_maxpool3x3s2_f32")
         return y
 
+    def group_conv(self, x, L, groups, relu=False):
+        """ResNeXt's grouped 3x3 conv2 (L.w: [width, 3, 3, width / groups]) + folded bn2 + ReLU"""
+        n, h, w, width = x.shape
+        ho, wo = (h + 2 - 3) // L.stride + 1, (w + 2 - 3) // L.stride + 1
+        y = torch.empty((n, ho, wo, width), dtype=torch.float32, device=self.device)
+        _lib.check(self.lib.orp_group_conv2d_f32(_lib.ptr(x), n, h, w, width, groups, _lib.ptr(L.w), L.stride, _lib.ptr(L.bias),
+                                                 int(relu), _lib.ptr(y), _lib.current_stream_ptr()), "orp_group_conv2d_f32")
+        return y
+
     def deform_conv(self, x, offset, L, relu=False, mask=None):
         n, h, w, cin = x.shape
         ho, wo = (h + 2 * L.pad - L.kh) // L.stride + 1, (w + 2 * L.pad - L.kw) // L.stride + 1
@@ -118,10 +127,10 @@ class EngineF32:
 
 
 class OrientedRepPointsDetector:
-    """R-50 / R-101 or Swin-T/S/B/L + FPN(GN) + OrientedRepPointsHead, inference only."""
+    """R-50 / R-101 / R-152, ResNeXt of those depths, or Swin-T/S/B/L + FPN(GN) + OrientedRepPointsHead, inference only."""
 
     def __init__(self, state_dict, depth=50, device="cuda", precision="fp32", test_cfg=None, dcn=None):
-        """depth: 50 / 101 (ResNet), or a Swin backbone - "swin_tiny" (Swin-T, window 7), any key of swin.ARCHS
+        """depth: 50 / 101 / 152 (ResNet or ResNeXt: the groups of every conv2 come from the state dict's shapes), or a Swin backbone - "swin_tiny" (Swin-T, window 7), any key of swin.ARCHS
         ("swin_small", "swin_base_w12", ...) or a swin.SwinArch.
         dcn: the ResNet's deformable conv2 layers per stage and block, None / 'DCN' / 'DCNv2' (models.ResNet.dcn_layout,
         weights.dcn_layout); None: every conv2 is a plain convolution"""
@@ -168,10 +177,16 @@ class OrientedRepPointsDetector:
                            sd[bn + ".running_mean"].float(), sd[bn + ".running_var"].float())
             return ConvLayer(w, b, stride, pad, d, pad_cin_to)
 
+        if self.depth not in STAGE_BLOCKS:
+            raise ValueError("depth must be one of %s for a ResNet / ResNeXt backbone" % sorted(STAGE_BLOCKS))
         layout = self.dcn if self.dcn is not None else tuple((None,) * n for n in STAGE_BLOCKS[self.depth])
         if tuple(len(s) for s in layout) != STAGE_BLOCKS[self.depth] or \
                 any(k not in (None, 'DCN', 'DCNv2') for s in layout for k in s):
             raise ValueError("dcn must give None, 'DCN' or 'DCNv2' for each of the %s blocks of R-%d" % (STAGE_BLOCKS[self.depth], self.depth))
+        self.groups = self._groups_of(sd)
+        if self.groups > 1 and any(k is not None for s in layout for k in s):
+            raise NotImplementedError("dcn on a ResNeXt with groups=%d would be a grouped deformable convolution: not built"
+                                      % self.groups)
         self.stem = folded("backbone.conv1", "backbone.bn1", 2, 3, pad_cin_to=4)
         self.blocks = []
         for li, nblk in enumerate(STAGE_BLOCKS[self.depth]):
@@ -191,6 +206,40 @@ class OrientedRepPointsDetector:
         self.fpn = [(ConvLayer(sd["neck.fpn_convs.%d.conv.weight" % i].float(), None, 2 if i >= 3 else 1, 1, d),
                      Norm(sd, "neck.fpn_convs.%d.gn" % i, d)) for i in range(5)]
         self._load_head(sd)
+
+    def _groups_of(self, sd):
+        """the backbone's conv2 groups, from the shapes: conv2 [width, gw, 3, 3] has width / gw groups.  1 for a ResNet.  A
+        ResNeXt (resnext.py:20-23) has the same groups in every block and width = floor(planes * base_width / 64) * groups, so
+        gw is constant within a stage and doubles from stage to stage; conv1 / conv3 must be `width` wide.  ValueError when the
+        shapes contradict that, NotImplementedError for a group width the kernels are not built for (weights.check_groups)"""
+        found = set()
+        gw0 = None
+        for li, nblk in enumerate(STAGE_BLOCKS[self.depth]):
+            planes = 64 << li
+            for b in range(nblk):
+                p = "backbone.layer%d.%d" % (li + 1, b)
+                w2 = tuple(sd[p + ".conv2.weight"].shape)
+                width = tuple(sd[p + ".conv1.weight"].shape)[0]
+                if len(w2) != 4 or w2[0] != width or w2[2:] != (3, 3) or w2[1] < 1 or width % w2[1] or \
+                        tuple(sd[p + ".conv3.weight"].shape)[:2] != (planes * 4, width):
+                    raise ValueError("%s: conv1 [%d, ...], conv2 %s and conv3 %s do not form a bottleneck of width %d"
+                                     % (p, width, w2, tuple(sd[p + ".conv3.weight"].shape), width))
+                gw = w2[1]
+                groups = width // gw
+                if gw0 is None:
+                    gw0 = gw
+                found.add(groups)
+                if len(found) > 1:
+                    raise ValueError("%s: conv2 has %d groups where earlier blocks have %s: a ResNeXt has the same groups in "
+                                     "every block" % (p, groups, sorted(found - {groups})))
+                want = block_width(planes, groups, gw0) if groups > 1 else planes
+                if width != want or (groups > 1 and gw != gw0 << li):
+                    raise ValueError("%s: conv2 %s does not follow width = floor(planes * base_width / 64) * groups with "
+                                     "planes %d, groups %d, base_width %d (group width %d in stage 1)"
+                                     % (p, w2, planes, groups, gw0, gw0))
+        groups = found.pop()
+        check_groups(groups, gw0)
+        return groups
 
     def _offset_conv(self, sd, conv2, kind, planes, stride):
         """the conv_offset of a deformable conv2 (deform_conv.py:258-323, 377-446): a plain 3x3 convolution with bias into
@@ -214,6 +263,8 @@ class OrientedRepPointsDetector:
         [N,Ho,Wo,18|27]; for DCNv2 one kernel splits that into the offsets (channels 0..17) and the sigmoid mask (18..26),
         ModulatedDeformConvPack.forward; the deformable convolution then samples x with them"""
         e = self.eng
+        if self.groups > 1:
+            return e.group_conv(x, blk["c2"], self.groups, relu=True)
         if blk["dcn"] is None:
             return e.conv(x, blk["c2"], relu=True)
         om = e.conv(x, blk["off"], out_f32=True)

@@ -85,6 +85,25 @@ class EngineTC:
         """the weight-scale argument of the f16x3 entry points (none in bf16)"""
         return ()
 
+    @staticmethod
+    def _group_weights(L):
+        """a grouped conv2's weights (L.w_raw [width, 3, 3, gw]) in the layout of orp_b200_group.h: fp32 [width, 9, 64], the row
+        of output channel co holding the gw weights of its group at that group's place inside co's 64-channel block, zeros
+        elsewhere"""
+        width, kh, kw, gw = L.w_raw.shape
+        wp = torch.zeros((width, kh * kw, 64), dtype=torch.float32)
+        c0 = (torch.arange(width) % 64) // gw * gw                  # first input channel of co's group inside its block
+        rows = torch.arange(width)
+        w = L.w_raw.reshape(width, kh * kw, gw)
+        for k in range(gw):
+            wp[rows, :, c0 + k] = w[:, :, k]
+        return wp
+
+    def _group_tc(self, L):
+        if L.tc is None:
+            L.tc = dict(w=self._group_weights(L).to(self.device, torch.bfloat16).contiguous())
+        return L.tc
+
     # ------------------------------------------------------------------ layers
     def prepare_input(self, img_nchw):
         img = img_nchw.to(self.device, torch.float32).contiguous()
@@ -257,6 +276,18 @@ class EngineTC:
         weights inside the tensor-core kernel's A-operand producers"""
         return self.deform_conv_multi([x], [offset], L, relu, masks=None if mask is None else [mask])[0]
 
+    def group_conv(self, x, L, groups, relu=False):
+        """ResNeXt's grouped 3x3 conv2 (L.w_raw: [width, 3, 3, width / groups]) + folded bn2 + ReLU, orp_group_conv2d_*"""
+        tc = self._group_tc(L)
+        n, h, w, width = self.dims(x)
+        assert x.dtype == self.act_dtype and width == L.cout
+        y = self.alloc(n, (h + 2 - 3) // L.stride + 1, (w + 2 - 3) // L.stride + 1, width)
+        q = _lib.TcProblem()
+        q.x, q.N, q.H, q.W, q.out = x.data_ptr(), n, h, w, y.data_ptr()
+        self._call("orp_group_conv2d_%s", ctypes.byref(q), _lib.ptr(tc["w"]), width, groups, L.stride, _lib.ptr(L.bias),
+                   *self._wscale(tc), int(relu), _lib.current_stream_ptr())
+        return y
+
     def to_float(self, x):
         """activation tensor of this engine -> fp32 NHWC"""
         return x.float()
@@ -324,6 +355,12 @@ class EngineTCSplit(EngineTC):
             cbn = cin_p // 64                                        # [cout_p, taps, channel block, (hi, lo), 64]: the two halves
             wp = torch.stack([hi.reshape(cout_p, kh * kw, cbn, 64), lo.reshape(cout_p, kh * kw, cbn, 64)], dim=3)   # of a block are adjacent
             L.tc3 = dict(w=wp.reshape(cout_p, -1).to(self.device).contiguous(), cout_p=cout_p, s=s)
+        return L.tc3
+
+    def _group_tc(self, L):
+        if getattr(L, "tc3", None) is None:
+            hi, lo, s = self._split_weights(self._group_weights(L))    # [width, 9 taps, (hi, lo), 64]
+            L.tc3 = dict(w=torch.stack([hi, lo], dim=2).reshape(L.cout, -1).to(self.device).contiguous(), s=s)
         return L.tc3
 
     def _stem_s2d_tc(self, L):

@@ -1,5 +1,5 @@
 """Module-structure layer of the drop-in boundary (SURVEY.md 8(b), last row): the registries and the nn.Module parameter
-containers the reference's configs name - ResNet (mmdet/models/backbones/resnet.py:345-515), SwinTransformer
+containers the reference's configs name - ResNet (mmdet/models/backbones/resnet.py:345-515), ResNeXt (resnext.py), SwinTransformer
 (backbones/swin_transformer.py:449-631), FPN (necks/fpn.py:50-136), OrientedRepPointsHead
 (anchor_heads/orientedreppoints_head.py:18-146), OrientedRepPointsDetector (detectors/orientedreppoints_detector.py,
 single_stage.py) - with the reference's attribute names, so `build_detector(cfg.model, test_cfg=cfg.test_cfg)` builds from
@@ -16,6 +16,7 @@ from .ops.conv_module import ConvModule
 from .ops.dcn import DeformConv, DeformConvPack, ModulatedDeformConvPack
 from .ops.norm import build_norm_layer
 from .utils.registry import Registry, build_from_cfg
+from .weights import STAGE_BLOCKS, block_width, check_groups
 
 BACKBONES = Registry('backbone')
 NECKS = Registry('neck')
@@ -59,28 +60,30 @@ class _EngineOnly(nn.Module):
 class Bottleneck(_EngineOnly):
     """resnet.py:84-239 (style 'pytorch': the stride sits on the 3x3).  dcn: the conv2 config of resnet.py:146-168 - a
     DCN / DCNv2 layer (DeformConvPack / ModulatedDeformConvPack) unless `fallback_on_stride`, which is popped from the dict
-    itself: ResNet hands every block the same dict, so only the first block built from it sees the value"""
+    itself: ResNet hands every block the same dict, so only the first block built from it sees the value.
+    groups / base_width: the ResNeXt block (resnext.py:11-70): conv1 / conv2 are block_width() wide, conv2 has `groups` groups"""
     expansion = 4
 
-    def __init__(self, inplanes, planes, stride, downsample, norm_cfg, conv_cfg=None, dcn=None):
+    def __init__(self, inplanes, planes, stride, downsample, norm_cfg, conv_cfg=None, dcn=None, groups=1, base_width=4):
         super().__init__()
-        self.conv1 = nn.Conv2d(inplanes, planes, 1, bias=False)
-        self.add_module('bn1', build_norm_layer(norm_cfg, planes, 1)[1])
+        width = block_width(planes, groups, base_width)
+        self.conv1 = nn.Conv2d(inplanes, width, 1, bias=False)
+        self.add_module('bn1', build_norm_layer(norm_cfg, width, 1)[1])
         fallback_on_stride = dcn.pop('fallback_on_stride', False) if dcn is not None else False
         if dcn is None or fallback_on_stride:
-            self.conv2 = nn.Conv2d(planes, planes, 3, stride, 1, bias=False)
+            self.conv2 = nn.Conv2d(width, width, 3, stride, 1, groups=groups, bias=False)
         else:
             assert conv_cfg is None, 'conv_cfg cannot be None for DCN'
-            self.conv2 = build_conv_layer(dcn, planes, planes, kernel_size=3, stride=stride, padding=1, dilation=1, bias=False)
-        self.add_module('bn2', build_norm_layer(norm_cfg, planes, 2)[1])
-        self.conv3 = nn.Conv2d(planes, planes * 4, 1, bias=False)
+            self.conv2 = build_conv_layer(dcn, width, width, kernel_size=3, stride=stride, padding=1, dilation=1, bias=False)
+        self.add_module('bn2', build_norm_layer(norm_cfg, width, 2)[1])
+        self.conv3 = nn.Conv2d(width, planes * 4, 1, bias=False)
         self.add_module('bn3', build_norm_layer(norm_cfg, planes * 4, 3)[1])
         self.downsample = downsample
 
 
 @BACKBONES.register_module
 class ResNet(_EngineOnly):
-    arch_settings = {50: (3, 4, 6, 3), 101: (3, 4, 23, 3)}
+    arch_settings = STAGE_BLOCKS                                      # depth -> blocks per stage, shared with weights / the engine
 
     def __init__(self, depth, in_channels=3, num_stages=4, strides=(1, 2, 2, 2), dilations=(1, 1, 1, 1), out_indices=(0, 1, 2, 3),
                  style='pytorch', frozen_stages=-1, conv_cfg=None, norm_cfg=dict(type='BN', requires_grad=True), norm_eval=True,
@@ -113,15 +116,37 @@ class ResNet(_EngineOnly):
                 ds = None
                 if b == 0:
                     ds = nn.Sequential(nn.Conv2d(inplanes, planes * 4, 1, stride, bias=False), build_norm_layer(norm_cfg, planes * 4)[1])
-                blocks.append(Bottleneck(inplanes, planes, stride, ds, norm_cfg, conv_cfg, stage_dcn))
+                blocks.append(Bottleneck(inplanes, planes, stride, ds, norm_cfg, conv_cfg, stage_dcn, **self._block_args()))
                 inplanes = planes * 4
             self.add_module('layer%d' % (i + 1), nn.Sequential(*blocks))
+
+    def _block_args(self):
+        """extra Bottleneck arguments of this backbone (ResNeXt: groups, base_width)"""
+        return {}
 
     def dcn_layout(self):
         """per stage, per block: None for a plain conv2, else 'DCN' or 'DCNv2' - what the engine builds for that conv2"""
         kinds = {ModulatedDeformConvPack: 'DCNv2', DeformConvPack: 'DCN', nn.Conv2d: None}
         return tuple(tuple(kinds[type(blk.conv2)] for blk in getattr(self, 'layer%d' % (i + 1)))
                      for i in range(len(self.arch_settings[self.depth])))
+
+
+@BACKBONES.register_module
+class ResNeXt(ResNet):
+    """resnext.py:128-206: a ResNet whose bottlenecks are block_width() wide with a grouped conv2.  The engine runs the group
+    widths of the published models (32x4d, 64x4d, 32x8d); other (groups, base_width) and DCN on a grouped conv2 raise
+    NotImplementedError.  groups=1 is the ResNet, DCN included."""
+
+    def __init__(self, groups=1, base_width=4, **kwargs):
+        check_groups(groups, base_width)
+        if groups > 1 and kwargs.get('dcn') is not None and any(kwargs.get('stage_with_dcn', ())):
+            raise NotImplementedError("dcn with groups=%d would be a grouped deformable convolution (resnext.py:56-66): "
+                                      "liborp_b200 does not build it" % groups)
+        self.groups, self.base_width = groups, base_width            # read by _block_args while ResNet.__init__ builds
+        super().__init__(**kwargs)
+
+    def _block_args(self):
+        return dict(groups=self.groups, base_width=self.base_width)
 
 
 @BACKBONES.register_module()
@@ -249,7 +274,8 @@ class OrientedRepPointsDetector(nn.Module):
         if isinstance(self.backbone, ResNet):
             from .weights import random_state_dict
             sd = random_state_dict(self.backbone.depth, seed=0, reference_init=True, num_classes=self.bbox_head.num_classes,
-                                   dcn=self.backbone.dcn_cfg, stage_with_dcn=self.backbone.stage_with_dcn)
+                                   dcn=self.backbone.dcn_cfg, stage_with_dcn=self.backbone.stage_with_dcn,
+                                   **self.backbone._block_args())
         else:
             from .swin import random_swin_state_dict
             sd = random_swin_state_dict(0, num_classes=self.bbox_head.num_classes, arch=self.backbone.arch)

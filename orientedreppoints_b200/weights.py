@@ -1,8 +1,9 @@
-"""State-dict layout and random initialisation of OrientedRepPointsDetector (R-50 / R-101 + FPN + head).
+"""State-dict layout and random initialisation of OrientedRepPointsDetector (R-50 / R-101 / R-152 or ResNeXt + FPN + head).
 
 Key names follow the reference modules so published checkpoints load unchanged (SURVEY.md section 5):
   backbone.conv1.weight, backbone.bn1.*, backbone.layer{1..4}.{i}.conv{1,2,3}.weight / bn{1,2,3}.* /
-  downsample.{0,1}.*            (mmdet/models/backbones/resnet.py:84-239, 345-515)
+  downsample.{0,1}.*            (mmdet/models/backbones/resnet.py:84-239, 345-515; ResNeXt: resnext.py:11-70, the same
+                                 keys with conv1 / conv2 / bn1 / bn2 `width` wide and conv2 grouped)
   neck.lateral_convs.{i}.{conv,gn}.*, neck.fpn_convs.{i}.{conv,gn}.*   (necks/fpn.py:88-128)
   bbox_head.{cls,reg}_convs.{i}.{conv,gn}.*, bbox_head.reppoints_*     (orientedreppoints_head.py:91-132)
 Tensors are in the reference's layouts (conv weights [Cout, Cin, KH, KW]).
@@ -11,7 +12,31 @@ import math
 
 import torch
 
-STAGE_BLOCKS = {50: (3, 4, 6, 3), 101: (3, 4, 23, 3)}
+STAGE_BLOCKS = {50: (3, 4, 6, 3), 101: (3, 4, 23, 3), 152: (3, 8, 36, 3)}
+# group widths (channels per group of conv2) the grouped kernels are built for: those of ResNeXt 32x4d, 64x4d and 32x8d
+GROUP_WIDTHS = (4, 8, 16, 32, 64)
+
+
+def block_width(planes, groups=1, base_width=4):
+    """the bottleneck width of resnext.py:20-23: planes for groups == 1, else floor(planes * base_width / 64) * groups"""
+    return planes if groups == 1 else math.floor(planes * (base_width / 64)) * groups
+
+
+def check_groups(groups, base_width):
+    """NotImplementedError unless every stage's conv2 is one the grouped kernels run: width a multiple of 64 and a group width
+    in GROUP_WIDTHS (groups == 1 is a ResNet and always passes)"""
+    if groups == 1:
+        return
+    if not isinstance(groups, int) or groups < 1:
+        raise NotImplementedError("groups=%r: ResNeXt needs a positive integer number of groups" % (groups,))
+    for planes in (64, 128, 256, 512):
+        width = block_width(planes, groups, base_width)
+        if width % 64:
+            raise NotImplementedError("groups=%d, base_width=%r give a conv2 width of %d at planes=%d: liborp_b200 runs grouped "
+                                      "convolutions whose width is a multiple of 64" % (groups, base_width, width, planes))
+        if width // groups not in GROUP_WIDTHS:
+            raise NotImplementedError("groups=%d, base_width=%r give %d channels per group at planes=%d: liborp_b200 runs group "
+                                      "widths %s" % (groups, base_width, width // groups, planes, GROUP_WIDTHS))
 
 
 def _kaiming_fan_out(w, gen):
@@ -47,7 +72,7 @@ def dcn_layout(depth, dcn=None, stage_with_dcn=(False, False, False, False)):
 
 
 def random_state_dict(depth=50, seed=0, reference_init=True, num_classes=16, feat=256, residual_gain=1.0, dcn=None,
-                      stage_with_dcn=(False, False, False, False), dcn_offset_scale=0.0):
+                      stage_with_dcn=(False, False, False, False), dcn_offset_scale=0.0, groups=1, base_width=4):
     """reference_init=True reproduces the reference's init_weights (incl. zero_init_residual and all-ones
     norm scales); False randomises norm parameters / running statistics so that every branch of the graph
     carries signal (used by the parity tests); residual_gain scales the randomised scale of every block's last norm
@@ -57,13 +82,18 @@ def random_state_dict(depth=50, seed=0, reference_init=True, num_classes=16, fea
     that is not an nn.Conv2d; with reference_init=False the kaiming draw of a plain conv2 instead) and an all-zero
     conv_offset.  dcn_offset_scale > 0 (tests only) draws conv_offset from N(0, scale^2 / fan_in) with N(0, scale^2) biases
     instead, so that the samples leave the grid by about `scale` pixels per unit of input and the DCNv2 mask logits vary;
-    with zero offsets a deformable layer is a plain convolution."""
+    with zero offsets a deformable layer is a plain convolution.
+    groups / base_width: a ResNeXt (resnext.py): conv1 / conv2 / bn1 / bn2 are block_width() wide and conv2 has `groups` groups,
+    its kaiming fan_out width * 9 as for any nn.Conv2d.  groups=1 draws exactly the ResNet's tensors."""
+    check_groups(groups, base_width)
+    if groups > 1 and dcn is not None and any(stage_with_dcn):
+        raise NotImplementedError("dcn with groups=%d would be a grouped deformable convolution (resnext.py:56-66): not built" % groups)
     g = torch.Generator().manual_seed(seed)
     sd = {}
     layout = dcn_layout(depth, dcn, stage_with_dcn)
 
     def conv(name, cout, cin, k, init, bias=False, std=0.01):
-        w = torch.empty(cout, cin, k, k)
+        w = torch.empty(cout, cin, k, k)                              # (grouped conv2: cin = channels per group)
         if init == "kaiming":
             _kaiming_fan_out(w, g)
         elif init == "xavier":
@@ -95,11 +125,12 @@ def random_state_dict(depth=50, seed=0, reference_init=True, num_classes=16, fea
     for li, (nblk, planes) in enumerate(zip(STAGE_BLOCKS[depth], (64, 128, 256, 512))):
         for b in range(nblk):
             p = "backbone.layer%d.%d" % (li + 1, b)
-            conv(p + ".conv1", planes, inplanes, 1, "kaiming")
-            norm(p + ".bn1", planes, True)
+            width = block_width(planes, groups, base_width)
+            conv(p + ".conv1", width, inplanes, 1, "kaiming")
+            norm(p + ".bn1", width, True)
             kind = layout[li][b]
             if kind is None:
-                conv(p + ".conv2", planes, planes, 3, "kaiming")
+                conv(p + ".conv2", width, width // groups, 3, "kaiming")
             else:
                 if reference_init:
                     bound = 1.0 / math.sqrt(9 * planes)
@@ -112,8 +143,8 @@ def random_state_dict(depth=50, seed=0, reference_init=True, num_classes=16, fea
                     w.normal_(0, dcn_offset_scale / math.sqrt(9 * planes), generator=g)
                     bias.normal_(0, dcn_offset_scale, generator=g)
                 sd[p + ".conv2.conv_offset.weight"], sd[p + ".conv2.conv_offset.bias"] = w, bias
-            norm(p + ".bn2", planes, True)
-            conv(p + ".conv3", planes * 4, planes, 1, "kaiming")
+            norm(p + ".bn2", width, True)
+            conv(p + ".conv3", planes * 4, width, 1, "kaiming")
             norm(p + ".bn3", planes * 4, True, zero_gamma=True)           # zero_init_residual, resnet.py:486-491
             if b == 0:
                 conv(p + ".downsample.0", planes * 4, inplanes, 1, "kaiming")
