@@ -1,4 +1,5 @@
-"""ctypes binding of liborp_b200.so (include/orp_b200.h, orp_b200_dcnv2.h, orp_b200_swin.h, orp_b200_group.h).
+"""ctypes binding of liborp_b200.so (include/orp_b200.h, orp_b200_dcnv2.h, orp_b200_swin.h, orp_b200_group.h,
+orp_b200_hrnet.h).
 
 There is NO fallback: if the shared library is missing or a call fails, an exception is raised.
 The library is built in-tree by `python -m orientedreppoints_b200.build` (nvcc, sm_90a).
@@ -162,6 +163,20 @@ GROUP_SIGNATURES = {
     "orp_tc_plan_group_conv": (_i, [_i, ctypes.POINTER(TcProblem), _vp, _i, _i, _i, _vp, _i, _i, _i, _i, ctypes.POINTER(TcPlan)]),
 }
 
+# name -> (restype, argtypes); every symbol include/orp_b200_hrnet.h declares (the pointer arrays are host arrays of device
+# pointers: ctypes (c_void_p * n))
+HRNET_SIGNATURES = {
+    "orp_hr_fuse_bf16": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
+    "orp_hr_fuse_f16x3": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
+    "orp_hr_fuse_f32": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
+    "orp_hrfpn_reduce_bf16": (_i, [_i, _vp, _i, _i, _i, _i, _vp, _vp]),
+    "orp_hrfpn_reduce_f16x3": (_i, [_i, _vp, _i, _i, _i, _i, _vp, _vp]),
+    "orp_hrfpn_reduce_f32": (_i, [_i, _vp, _i, _i, _i, _i, _vp, _vp]),
+    "orp_hrfpn_pool_bf16": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp]),
+    "orp_hrfpn_pool_f16x3": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp]),
+    "orp_hrfpn_pool_f32": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp]),
+}
+
 _LIB = None
 
 
@@ -179,7 +194,7 @@ def lib():
                 "(there is no CPU or PyTorch fallback for this path)" % LIB_PATH)
         l = ctypes.CDLL(LIB_PATH)
         for name, (res, args) in list(SIGNATURES.items()) + list(DCNV2_SIGNATURES.items()) + list(SWIN_SIGNATURES.items()) + \
-                list(GROUP_SIGNATURES.items()):
+                list(GROUP_SIGNATURES.items()) + list(HRNET_SIGNATURES.items()):
             fn = getattr(l, name)   # AttributeError if the symbol is not exported
             fn.restype = res
             fn.argtypes = args
@@ -273,6 +288,11 @@ def tc_plan_group_for(problems, width, groups, stride, *, split=False, bias=True
     check(lib().orp_tc_plan_group_conv(len(problems), arr, ph, width, groups, stride, ph if bias else None, int(relu), int(out_f32),
                                        int(split), sms, ctypes.byref(p)), "orp_tc_plan_group_conv")
     return p.as_dict()
+
+
+def ptr_array(ts):
+    """host array of the device pointers of tensors ts (None -> NULL), for the pointer-array arguments"""
+    return (ctypes.c_void_p * len(ts))(*[None if t is None else t.data_ptr() for t in ts])
 
 
 def current_stream_ptr():

@@ -30,6 +30,7 @@ def _headers():
     hs.append(os.path.join(HERE, "..", "include", "orp_b200_dcnv2.h"))
     hs.append(os.path.join(HERE, "..", "include", "orp_b200_swin.h"))
     hs.append(os.path.join(HERE, "..", "include", "orp_b200_group.h"))
+    hs.append(os.path.join(HERE, "..", "include", "orp_b200_hrnet.h"))
     return hs
 
 

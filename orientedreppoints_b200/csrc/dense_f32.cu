@@ -16,6 +16,8 @@
 // GroupNorm needs (fp32 partials per thread and per CTA, added across CTAs with double atomics).
 #include "common.cuh"
 #include "../../include/orp_b200_group.h"
+#include "../../include/orp_b200_hrnet.h"
+#include "hrnet.cuh"
 
 namespace orp {
 namespace {
@@ -424,4 +426,20 @@ extern "C" int orp_maxpool3x3s2_f32(const float *x, int N, int H, int W, int C, 
     maxpool3x3s2_f32_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(x, N, H, W, C, Ho, Wo, y);
     ORP_LAUNCHED();
     return ORP_OK;
+}
+
+/* see include/orp_b200_hrnet.h */
+extern "C" int orp_hr_fuse_f32(const float *base, int N, int H, int W, int C, int nsrc, const float *const *src, float *y, void *stream)
+{
+    return orp::hr_fuse<orp::ActF32>(base, N, H, W, C, nsrc, reinterpret_cast<const void *const *>(src), y, stream, "hr_fuse_f32");
+}
+
+extern "C" int orp_hrfpn_reduce_f32(int nparts, const float *const *part, int N, int H, int W, int C, float *y, void *stream)
+{
+    return orp::hrfpn_reduce<orp::ActF32>(nparts, part, N, H, W, C, y, stream, "hrfpn_reduce_f32");
+}
+
+extern "C" int orp_hrfpn_pool_f32(const float *x, int N, int H, int W, int C, int max_pool, float *const *out, void *stream)
+{
+    return orp::hrfpn_pool<orp::ActF32>(x, N, H, W, C, max_pool, reinterpret_cast<void *const *>(out), stream, "hrfpn_pool_f32");
 }

@@ -1963,6 +1963,14 @@ __global__ void overflow_take_kernel(unsigned int *dst, int reset)
     *dst = reset ? atomicExch(&g_f16_overflow, 0u) : atomicAdd(&g_f16_overflow, 0u);
 }
 
+namespace orp {
+unsigned int *f16x3_overflow_counter()
+{
+    void *p = nullptr;
+    return cudaGetSymbolAddress(&p, g_f16_overflow) == cudaSuccess ? static_cast<unsigned int *>(p) : nullptr;
+}
+}  // namespace orp
+
 /* see include/orp_b200.h */
 extern "C" int orp_f16x3_overflow_count(unsigned int *count, int reset, void *stream)
 {

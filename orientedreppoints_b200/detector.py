@@ -115,6 +115,27 @@ class EngineF32:
                                                  int(relu), _lib.ptr(y), _lib.current_stream_ptr()), "orp_group_conv2d_f32")
         return y
 
+    def hr_fuse(self, base, srcs):
+        n, h, w, c = base.shape
+        y = torch.empty_like(base)
+        _lib.check(self.lib.orp_hr_fuse_f32(_lib.ptr(base), n, h, w, c, len(srcs), _lib.ptr_array(srcs), _lib.ptr(y),
+                                            _lib.current_stream_ptr()), "orp_hr_fuse_f32")
+        return y
+
+    def hrfpn_reduce(self, parts):
+        n, h, w, c = parts[0].shape
+        y = torch.empty((n, h, w, c), dtype=torch.float32, device=self.device)
+        _lib.check(self.lib.orp_hrfpn_reduce_f32(len(parts), _lib.ptr_array(parts), n, h, w, c, _lib.ptr(y),
+                                                 _lib.current_stream_ptr()), "orp_hrfpn_reduce_f32")
+        return y
+
+    def hrfpn_pool(self, x, max_pool):
+        n, h, w, c = x.shape
+        outs = [torch.empty((n, h >> l, w >> l, c), dtype=torch.float32, device=self.device) for l in range(1, 5)]
+        _lib.check(self.lib.orp_hrfpn_pool_f32(_lib.ptr(x), n, h, w, c, int(bool(max_pool)), _lib.ptr_array(outs),
+                                               _lib.current_stream_ptr()), "orp_hrfpn_pool_f32")
+        return outs
+
     def deform_conv(self, x, offset, L, relu=False, mask=None):
         n, h, w, cin = x.shape
         ho, wo = (h + 2 * L.pad - L.kh) // L.stride + 1, (w + 2 * L.pad - L.kw) // L.stride + 1
@@ -127,19 +148,27 @@ class EngineF32:
 
 
 class OrientedRepPointsDetector:
-    """R-50 / R-101 / R-152, ResNeXt of those depths, or Swin-T/S/B/L + FPN(GN) + OrientedRepPointsHead, inference only."""
+    """R-50 / R-101 / R-152, ResNeXt of those depths, or Swin-T/S/B/L + FPN(GN), or HRNet + HRFPN, + OrientedRepPointsHead,
+    inference only."""
 
-    def __init__(self, state_dict, depth=50, device="cuda", precision="fp32", test_cfg=None, dcn=None):
+    def __init__(self, state_dict, depth=50, device="cuda", precision="fp32", test_cfg=None, dcn=None, pooling_type='AVG'):
         """depth: 50 / 101 / 152 (ResNet or ResNeXt: the groups of every conv2 come from the state dict's shapes), or a Swin backbone - "swin_tiny" (Swin-T, window 7), any key of swin.ARCHS
-        ("swin_small", "swin_base_w12", ...) or a swin.SwinArch.
+        ("swin_small", "swin_base_w12", ...) or a swin.SwinArch, or an HRNet backbone with the HRFPN neck (stride 2, five
+        outputs) - a key of hrnet.ARCHS ("hrnetv2p_w18", ...) or an hrnet.HRNetArch.
         dcn: the ResNet's deformable conv2 layers per stage and block, None / 'DCN' / 'DCNv2' (models.ResNet.dcn_layout,
-        weights.dcn_layout); None: every conv2 is a plain convolution"""
+        weights.dcn_layout); None: every conv2 is a plain convolution.
+        pooling_type: HRFPN's pooling, 'AVG' or 'MAX' (HRNet only)"""
+        from . import hrnet
         from .swin import arch_of
         self.device = torch.device(device)
         if self.device.type == "cuda" and self.device.index is None:      # 'cuda' -> the current device, with its index
             self.device = torch.device("cuda", torch.cuda.current_device())
         self.depth = depth
-        self.swin_arch = arch_of(depth)                    # None for a ResNet
+        self.hr_arch = hrnet.arch_of(depth)                # None for a ResNet or Swin
+        self.swin_arch = None if self.hr_arch is not None else arch_of(depth)     # None for a ResNet or HRNet
+        if pooling_type not in ('AVG', 'MAX'):
+            raise ValueError("pooling_type must be 'AVG' or 'MAX', not %r" % (pooling_type,))
+        self.pooling_type = pooling_type
         self.dcn = dcn
         self.test_cfg = dict(nms_pre=2000, min_bbox_size=0, score_thr=0.05, nms=dict(type='rnms', iou_thr=0.4),
                              max_per_img=2000)                         # configs/dota/orientedrepoints_r50_demo.py:62-67
@@ -171,6 +200,10 @@ class OrientedRepPointsDetector:
             if self.dcn is not None:
                 raise ValueError("dcn describes the deformable layers of a ResNet backbone; the Swin backbone has none")
             return self._load_swin(sd)
+        if self.hr_arch is not None:
+            if self.dcn is not None:
+                raise ValueError("dcn describes the deformable layers of a ResNet backbone; the HRNet backbone has none")
+            return self._load_hrnet(sd)
 
         def folded(conv, bn, stride, pad, pad_cin_to=None):
             w, b = fold_bn(sd[conv + ".weight"].float(), sd[bn + ".weight"].float(), sd[bn + ".bias"].float(),
@@ -305,6 +338,18 @@ class OrientedRepPointsDetector:
                      Norm(sd, "neck.fpn_convs.%d.gn" % i, d)) for i in range(3)]
         self._load_head(sd)
 
+    def _load_hrnet(self, sd):
+        """HRNet + HRFPN (hrnet.HRNetGraph); conv1 (3x3 / s2 / pad 1) + bn1 + ReLU runs on the stem kernels"""
+        from .hrnet import HRNetGraph
+        w = sd["backbone.conv1.weight"]
+        if tuple(w.shape) != (64, 3, 3, 3):
+            raise ValueError("backbone.conv1.weight has shape %s where HRNet needs (64, 3, 3, 3)" % (tuple(w.shape),))
+        wf, b = fold_bn(w.float(), sd["backbone.bn1.weight"].float(), sd["backbone.bn1.bias"].float(),
+                        sd["backbone.bn1.running_mean"].float(), sd["backbone.bn1.running_var"].float())
+        self.stem = ConvLayer(wf, b, 2, 1, self.device, pad_cin_to=4)
+        self.hrnet = HRNetGraph(sd, self.device, self.eng, self.hr_arch, self.pooling_type)
+        self._load_head(sd)
+
     # ------------------------------------------------------------------ dense graph
     def normalize(self, img, valid_hw=None):
         """decoded uint8 HWC tiles [N,H,W,3] -> the pipeline's Normalize + ImageToTensor on the device
@@ -331,6 +376,13 @@ class OrientedRepPointsDetector:
             x = torch.where(inside.unsqueeze(-1), x, torch.zeros((), dtype=x.dtype, device=self.device))
         return x.permute(0, 3, 1, 2).contiguous()
 
+    def _stem(self, img, valid_hw):
+        """conv1 + folded bn1 + ReLU of a ResNet or HRNet backbone"""
+        e = self.eng
+        if img.dtype == torch.uint8 and hasattr(e, "stem_u8") and img.shape[1] % 2 == 0 and img.shape[2] % 2 == 0:
+            return e.stem_u8(img, self.stem, self.img_norm_cfg, valid_hw)     # Normalize (+ Pad) fused into the stem input
+        return e.stem(e.prepare_input(self.normalize(img, valid_hw)), self.stem)
+
     def extract_feat(self, img, valid_hw=None):
         """valid_hw: optional device int32 [N,2] extents of uint8 images padded by the test pipeline"""
         e = self.eng
@@ -344,11 +396,13 @@ class OrientedRepPointsDetector:
             outs.append(self.swin.subsample2(outs[-1]))
             outs.append(self.swin.subsample2(outs[-1]))
             return outs
-        if img.dtype == torch.uint8 and hasattr(e, "stem_u8") and img.shape[1] % 2 == 0 and img.shape[2] % 2 == 0:
-            x = e.maxpool(e.stem_u8(img, self.stem, self.img_norm_cfg, valid_hw))   # Normalize (+ Pad) fused into the stem input
-        else:
-            x = e.prepare_input(self.normalize(img, valid_hw))
-            x = e.maxpool(e.stem(x, self.stem))
+        if self.hr_arch is not None:
+            h, w = img.shape[1:3] if img.dtype == torch.uint8 else img.shape[2:4]
+            if h % 32 or w % 32 or h < 64 or w < 64:
+                raise ValueError("an HRNet backbone needs input H and W that are multiples of 32 and at least 64 (the configs' "
+                                 "Pad(size_divisor=32)), not %dx%d: its fuse adds and HRFPN's 16x16 pooling need them" % (h, w))
+            return self.hrnet.neck(self.hrnet.backbone(self._stem(img, valid_hw)))
+        x = e.maxpool(self._stem(img, valid_hw))
         feats = []
         for stage in self.blocks:
             for blk in stage:

@@ -31,7 +31,7 @@ class EngineTC:
         _lib.check(getattr(self.lib, fn)(*args), fn)
 
     # ------------------------------------------------------------------ weights
-    def _tc(self, L):
+    def _tc(self, L, out16=False):
         if L.tc is None:
             w = L.w_raw                                              # [Cout, KH, KW, Cin] fp32 (unpadded Cin)
             cout, kh, kw, cin = w.shape
@@ -53,19 +53,24 @@ class EngineTC:
 
     @staticmethod
     def _s2d_weights(L):
-        """conv1 weights for the space-to-depth form, fp32 [64][kh' 0..3][kw' 0..3][16] with ky = 2kh'+dy-1,
-        kx = 2kw'+dx-1, channel (dy*2+dx)*3+c (zero where ky/kx fall outside 0..6, channels 12-15 zero)"""
-        w = L.w_raw                                                  # [64, 7, 7, 3]
+        """conv1 weights for the space-to-depth form, fp32 [64][kh' 0..3][kw' 0..3][16] with ky = 2kh'+dy-o,
+        kx = 2kw'+dx-o, channel (dy*2+dx)*3+c (zero where ky/kx fall outside the kernel, channels 12-15 zero).  o = 1 for
+        ResNet's 7x7 / s2 / pad 3 conv1, o = 3 for HRNet's 3x3 / s2 / pad 1 conv1: both read image row 2(oy+kh'-2)+dy, so
+        one 4x4 stride-1 convolution of the same space-to-depth input computes either, with the same output extent"""
+        w = L.w_raw                                                  # [64, k, k, 3], k = 7 or 3
+        k = w.shape[1]
+        assert tuple(w.shape) in ((64, 7, 7, 3), (64, 3, 3, 3)), tuple(w.shape)
+        o = 4 - k // 2
         wp = torch.zeros((64, 4, 4, 16), dtype=torch.float32)
         for khp in range(4):
             for dy in range(2):
-                ky = 2 * khp + dy - 1
-                if not 0 <= ky <= 6:
+                ky = 2 * khp + dy - o
+                if not 0 <= ky < k:
                     continue
                 for kwp in range(4):
                     for dx in range(2):
-                        kx = 2 * kwp + dx - 1
-                        if not 0 <= kx <= 6:
+                        kx = 2 * kwp + dx - o
+                        if not 0 <= kx < k:
                             continue
                         ch = (dy * 2 + dx) * 3
                         wp[:, khp, kwp, ch:ch + 3] = w[:, ky, kx, :]
@@ -198,7 +203,7 @@ class EngineTC:
     def conv_multi(self, xs, L, relu=False, residual=None, out_f32=False, residual_f32=None, stats=None):
         """relu: False/True, or 2 for the exact-GELU epilogue (Swin MLP); stats: per-problem double [N,32,2] tensors
         (zeroed) that receive the GroupNorm statistics of the outputs"""
-        tc = self._tc(L)
+        tc = self._tc(L, out16=not out_f32)
         ys = []
         for x in xs:
             n, h, w, cin = self.dims(x)
@@ -288,6 +293,29 @@ class EngineTC:
                    *self._wscale(tc), int(relu), _lib.current_stream_ptr())
         return y
 
+    def hr_fuse(self, base, srcs):
+        """relu(base + sum_k nearest_up(srcs[k-1], 2^k)), orp_hr_fuse_*: one HRModule output branch (hrnet.py:182-190)"""
+        n, h, w, c = self.dims(base)
+        y = self.alloc(n, h, w, c)
+        self._call("orp_hr_fuse_%s", _lib.ptr(base), n, h, w, c, len(srcs), _lib.ptr_array(srcs), _lib.ptr(y),
+                   _lib.current_stream_ptr())
+        return y
+
+    def hrfpn_reduce(self, parts):
+        """sum_i bilinear_up(parts[i], 2^i) of fp32 NHWC parts into this engine's format, orp_hrfpn_reduce_*"""
+        n, h, w, c = parts[0].shape
+        y = self.alloc(n, h, w, c)
+        self._call("orp_hrfpn_reduce_%s", len(parts), _lib.ptr_array(parts), n, h, w, c, _lib.ptr(y), _lib.current_stream_ptr())
+        return y
+
+    def hrfpn_pool(self, x, max_pool):
+        """avg / max pools of kernel = stride 2, 4, 8, 16 of x in one pass, orp_hrfpn_pool_*"""
+        n, h, w, c = self.dims(x)
+        outs = [self.alloc(n, h >> l, w >> l, c) for l in range(1, 5)]
+        self._call("orp_hrfpn_pool_%s", _lib.ptr(x), n, h, w, c, int(bool(max_pool)), _lib.ptr_array(outs),
+                   _lib.current_stream_ptr())
+        return outs
+
     def to_float(self, x):
         """activation tensor of this engine -> fp32 NHWC"""
         return x.float()
@@ -343,11 +371,13 @@ class EngineTCSplit(EngineTC):
             return 256
         return ((cout + 63) // 64) * 64
 
-    def _tc(self, L):
+    def _tc(self, L, out16=False):
+        """out16: the layer writes 16-bit outputs, whose TMA epilogue needs at least one 64-column tile (HRNet's 24- and
+        32-channel branches); the 32-row padding serves the narrow fp32 outputs only"""
         if getattr(L, "tc3", None) is None:
             w = L.w_raw                                              # [Cout, KH, KW, Cin] fp32 (unpadded Cin)
             cout, kh, kw, cin = w.shape
-            cout_p = self._pad_cout(cout)
+            cout_p = 64 if out16 and cout <= 32 else self._pad_cout(cout)
             cin_p = ((cin + 63) // 64) * 64
             wp4 = torch.zeros((cout_p, kh * kw, cin_p), dtype=torch.float32)
             wp4[:cout, :, :cin] = w.reshape(cout, kh * kw, cin)

@@ -1,7 +1,7 @@
 """Module-structure layer of the drop-in boundary (SURVEY.md 8(b), last row): the registries and the nn.Module parameter
 containers the reference's configs name - ResNet (mmdet/models/backbones/resnet.py:345-515), ResNeXt (resnext.py), SwinTransformer
 (backbones/swin_transformer.py:449-631), FPN (necks/fpn.py:50-136), OrientedRepPointsHead
-(anchor_heads/orientedreppoints_head.py:18-146), OrientedRepPointsDetector (detectors/orientedreppoints_detector.py,
+(anchor_heads/orientedreppoints_head.py:18-146), HRNet (backbones/hrnet.py) with HRFPN (necks/hrfpn.py), OrientedRepPointsDetector (detectors/orientedreppoints_detector.py,
 single_stage.py) - with the reference's attribute names, so `build_detector(cfg.model, test_cfg=cfg.test_cfg)` builds from
 the reference's config dicts and `state_dict()` / `load_state_dict()` use the reference's keys (published checkpoints load).
 
@@ -198,6 +198,133 @@ class SwinTransformer(_EngineOnly):
             self.add_module('norm%d' % i, nn.LayerNorm(embed_dim << i))
 
 
+class BasicBlock(_EngineOnly):
+    """resnet.py:13-83: conv1 3x3 (stride) + bn1 + ReLU, conv2 3x3 + bn2, + identity or downsample, ReLU"""
+    expansion = 1
+
+    def __init__(self, inplanes, planes, stride=1, downsample=None, norm_cfg=dict(type='BN')):
+        super().__init__()
+        self.conv1 = nn.Conv2d(inplanes, planes, 3, stride, 1, bias=False)
+        self.add_module('bn1', build_norm_layer(norm_cfg, planes, 1)[1])
+        self.conv2 = nn.Conv2d(planes, planes, 3, 1, 1, bias=False)
+        self.add_module('bn2', build_norm_layer(norm_cfg, planes, 2)[1])
+        self.downsample = downsample
+
+
+def _conv_bn(cin, cout, k, stride, norm_cfg, relu=False, upsample=None):
+    layers = [nn.Conv2d(cin, cout, k, stride, k // 2, bias=False), build_norm_layer(norm_cfg, cout)[1]]
+    if relu:
+        layers.append(nn.ReLU(inplace=False))
+    if upsample:
+        layers.append(nn.Upsample(scale_factor=upsample, mode='nearest'))
+    return nn.Sequential(*layers)
+
+
+class HRModule(_EngineOnly):
+    """hrnet.py:12-191: branches.{b} (BasicBlocks), fuse_layers.{i}.{j} (1x1 + BN + upsample for j > i, a chain of 3x3 / s2
+    convs for j < i, None for j == i)"""
+
+    def __init__(self, num_branches, num_blocks, in_channels, num_channels, norm_cfg):
+        super().__init__()
+        from .hrnet import fuse_convs
+        self.num_branches = num_branches
+        branches = []
+        for b in range(num_branches):
+            ds = None
+            if in_channels[b] != num_channels[b]:
+                ds = nn.Sequential(nn.Conv2d(in_channels[b], num_channels[b], 1, bias=False), build_norm_layer(norm_cfg, num_channels[b])[1])
+            blocks = [BasicBlock(in_channels[b], num_channels[b], 1, ds, norm_cfg)]
+            blocks += [BasicBlock(num_channels[b], num_channels[b], norm_cfg=norm_cfg) for _ in range(1, num_blocks[b])]
+            branches.append(nn.Sequential(*blocks))
+        self.branches = nn.ModuleList(branches)
+        self.fuse_layers = None
+        if num_branches > 1:
+            rows = []
+            for i, row in enumerate(fuse_convs(tuple(num_channels))):
+                mods = []
+                for j, path in enumerate(row):
+                    if path is None:
+                        mods.append(None)
+                    elif j > i:
+                        mods.append(_conv_bn(num_channels[j], num_channels[i], 1, 1, norm_cfg, upsample=2 ** (j - i)))
+                    else:
+                        mods.append(nn.Sequential(*[_conv_bn(cin, cout, 3, 2, norm_cfg, relu=k < len(path) - 1)
+                                                    for k, (_, _, cout, cin, _, _) in enumerate(path)]))
+                rows.append(nn.ModuleList(mods))
+            self.fuse_layers = nn.ModuleList(rows)
+
+
+@BACKBONES.register_module
+class HRNet(_EngineOnly):
+    """hrnet.py:194-525 for every architecture hrnet.HRNetArch.from_extra accepts (stages 1-4 of 1, 2, 3, 4 branches, stage 1
+    BOTTLENECK or BASIC, stages 2-4 BASIC, any widths and module / block counts); `arch` is that description"""
+
+    def __init__(self, extra, in_channels=3, conv_cfg=None, norm_cfg=dict(type='BN'), norm_eval=True, with_cp=False,
+                 zero_init_residual=False):
+        super().__init__()
+        from .hrnet import HRNetArch, transition_convs
+        if in_channels != 3:
+            raise NotImplementedError("HRNet with in_channels=%r: liborp_b200 builds 3-channel (RGB) inputs" % (in_channels,))
+        if conv_cfg is not None:
+            raise NotImplementedError("HRNet with conv_cfg=%r: liborp_b200 builds plain convolutions" % (conv_cfg,))
+        if norm_cfg is None or norm_cfg.get('type') != 'BN':
+            raise NotImplementedError("HRNet with norm_cfg=%r: liborp_b200 builds BN norms (folded into the convolutions)" % (norm_cfg,))
+        self.arch = HRNetArch.from_extra(extra)
+        self.extra, self.norm_cfg, self.norm_eval, self.with_cp = extra, norm_cfg, norm_eval, with_cp
+        self.zero_init_residual = zero_init_residual
+        self.conv1 = nn.Conv2d(3, 64, 3, 2, 1, bias=False)
+        self.add_module('bn1', build_norm_layer(norm_cfg, 64, 1)[1])
+        self.conv2 = nn.Conv2d(64, 64, 3, 2, 1, bias=False)
+        self.add_module('bn2', build_norm_layer(norm_cfg, 64, 2)[1])
+        s1 = self.arch.stages[0]
+        ch, out1 = s1.num_channels[0], s1.widths[0]
+        ds = None if out1 == 64 else nn.Sequential(nn.Conv2d(64, out1, 1, bias=False), build_norm_layer(norm_cfg, out1)[1])
+        if s1.block == 'BOTTLENECK':
+            blocks = [Bottleneck(64, ch, 1, ds, norm_cfg)] + [Bottleneck(out1, ch, 1, None, norm_cfg) for _ in range(1, s1.num_blocks[0])]
+        else:
+            blocks = [BasicBlock(64, ch, 1, ds, norm_cfg)] + [BasicBlock(out1, ch, norm_cfg=norm_cfg) for _ in range(1, s1.num_blocks[0])]
+        self.layer1 = nn.Sequential(*blocks)
+        pre = s1.widths
+        for s in range(1, 4):
+            st = self.arch.stages[s]
+            trans = []
+            for t in transition_convs(pre, st.widths):
+                if t is None:
+                    trans.append(None)
+                elif len(t) == 1 and t[0][4] == 1:
+                    trans.append(_conv_bn(t[0][3], t[0][2], 3, 1, norm_cfg, relu=True))
+                else:
+                    trans.append(nn.Sequential(*[_conv_bn(cin, cout, 3, 2, norm_cfg, relu=True) for _, _, cout, cin, _ in t]))
+            self.add_module('transition%d' % s, nn.ModuleList(trans))
+            self.add_module('stage%d' % (s + 1), nn.Sequential(*[HRModule(st.num_branches, st.num_blocks, list(st.widths),
+                                                                           list(st.widths), norm_cfg)
+                                                                  for _ in range(st.num_modules)]))
+            pre = st.widths
+
+
+@NECKS.register_module
+class HRFPN(_EngineOnly):
+    """hrfpn.py:11-100: reduction_conv and fpn_convs.{i} are ConvModules with a bias and NO norm, whatever norm_cfg says
+    (hrfpn.py:49-66 never passes it on).  Built: num_outs=5 with stride=2 (the head's strides 8..128), pooling 'MAX' or
+    anything else for average, as the reference reads it"""
+
+    def __init__(self, in_channels, out_channels, num_outs=5, pooling_type='AVG', conv_cfg=None, norm_cfg=None, with_cp=False,
+                 stride=1):
+        super().__init__()
+        assert isinstance(in_channels, list)
+        if num_outs != 5 or stride != 2:
+            raise NotImplementedError("HRFPN with num_outs=%r, stride=%r: liborp_b200 builds num_outs=5 with stride=2, whose "
+                                      "five levels have the head's strides 8..128" % (num_outs, stride))
+        if conv_cfg is not None:
+            raise NotImplementedError("HRFPN with conv_cfg=%r: liborp_b200 builds plain convolutions" % (conv_cfg,))
+        self.in_channels, self.out_channels, self.num_ins, self.num_outs = in_channels, out_channels, len(in_channels), num_outs
+        self.with_cp, self.conv_cfg, self.norm_cfg, self.stride = with_cp, conv_cfg, norm_cfg, stride
+        self.pooling_type = 'MAX' if pooling_type == 'MAX' else 'AVG'
+        self.reduction_conv = ConvModule(sum(in_channels), out_channels, 1, conv_cfg=conv_cfg, act_cfg=None)
+        self.fpn_convs = nn.ModuleList([ConvModule(out_channels, out_channels, 3, padding=1, stride=stride, conv_cfg=conv_cfg,
+                                                   act_cfg=None) for _ in range(num_outs)])
+
+
 @NECKS.register_module
 class FPN(_EngineOnly):
     def __init__(self, in_channels, out_channels, num_outs, start_level=0, end_level=-1, add_extra_convs=False,
@@ -261,6 +388,16 @@ class OrientedRepPointsDetector(nn.Module):
         self.backbone = build_backbone(backbone)
         self.neck = build_neck(neck) if neck is not None else None
         self.bbox_head = build_head(bbox_head)
+        if isinstance(self.backbone, HRNet) != isinstance(self.neck, HRFPN):
+            raise NotImplementedError("%s with %s: liborp_b200 builds HRNet with the HRFPN neck, and the ResNet / Swin backbones "
+                                      "with FPN" % (type(self.backbone).__name__, type(self.neck).__name__))
+        if isinstance(self.neck, HRFPN):
+            if list(self.neck.in_channels) != list(self.backbone.arch.out_widths):
+                raise ValueError("HRFPN in_channels %s are not the HRNet's stage-4 widths %s"
+                                 % (list(self.neck.in_channels), list(self.backbone.arch.out_widths)))
+            if self.neck.out_channels != self.bbox_head.in_channels:
+                raise ValueError("HRFPN out_channels %d are not the head's in_channels %d"
+                                 % (self.neck.out_channels, self.bbox_head.in_channels))
         self.train_cfg, self.test_cfg, self.precision = train_cfg, test_cfg, precision
         self._engine = None
         self.init_weights(pretrained)
@@ -276,6 +413,10 @@ class OrientedRepPointsDetector(nn.Module):
             sd = random_state_dict(self.backbone.depth, seed=0, reference_init=True, num_classes=self.bbox_head.num_classes,
                                    dcn=self.backbone.dcn_cfg, stage_with_dcn=self.backbone.stage_with_dcn,
                                    **self.backbone._block_args())
+        elif isinstance(self.backbone, HRNet):
+            from .weights import random_hrnet_state_dict
+            sd = random_hrnet_state_dict(self.backbone.arch, seed=0, reference_init=True, num_classes=self.bbox_head.num_classes,
+                                         feat=self.neck.out_channels, zero_init_residual=self.backbone.zero_init_residual)
         else:
             from .swin import random_swin_state_dict
             sd = random_swin_state_dict(0, num_classes=self.bbox_head.num_classes, arch=self.backbone.arch)
@@ -297,9 +438,11 @@ class OrientedRepPointsDetector(nn.Module):
                 raise NotImplementedError("OrientedRepPointsDetector inference needs a CUDA (sm_90a) device: there is no CPU path")
             resnet = isinstance(self.backbone, ResNet)
             depth = self.backbone.depth if resnet else self.backbone.arch
+            hr = isinstance(self.neck, HRFPN)
             self._engine = Engine({k: v.detach() for k, v in self.state_dict().items()}, depth, dev, self.precision,
                                   test_cfg=dict(self.test_cfg) if self.test_cfg else None,
-                                  dcn=self.backbone.dcn_layout() if resnet else None)
+                                  dcn=self.backbone.dcn_layout() if resnet else None,
+                                  pooling_type=self.neck.pooling_type if hr else 'AVG')
         return self._engine
 
     def extract_feat(self, img):

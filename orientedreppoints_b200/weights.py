@@ -1,4 +1,5 @@
-"""State-dict layout and random initialisation of OrientedRepPointsDetector (R-50 / R-101 / R-152 or ResNeXt + FPN + head).
+"""State-dict layout and random initialisation of OrientedRepPointsDetector (R-50 / R-101 / R-152 or ResNeXt + FPN + head;
+HRNet + HRFPN + head in random_hrnet_state_dict, keys as mmdet/models/backbones/hrnet.py and necks/hrfpn.py name them).
 
 Key names follow the reference modules so published checkpoints load unchanged (SURVEY.md section 5):
   backbone.conv1.weight, backbone.bn1.*, backbone.layer{1..4}.{i}.conv{1,2,3}.weight / bn{1,2,3}.* /
@@ -71,6 +72,68 @@ def dcn_layout(depth, dcn=None, stage_with_dcn=(False, False, False, False)):
     return tuple(layout)
 
 
+def _drawers(sd, g, reference_init, residual_gain):
+    """the (conv, norm) draws of the random state dicts into sd from generator g"""
+
+    def conv(name, cout, cin, k, init, bias=False, std=0.01):
+        w = torch.empty(cout, cin, k, k)                              # (grouped conv2: cin = channels per group)
+        if init == "kaiming":
+            _kaiming_fan_out(w, g)
+        elif init == "xavier":
+            _xavier_uniform(w, g)
+        elif init == "fan_in":
+            w.normal_(0, math.sqrt(1.0 / (cin * k * k)), generator=g)
+        elif init == "caffe2_xavier":
+            # mmcv caffe2_xavier_init = kaiming_init(a=1, mode='fan_in', nonlinearity='leaky_relu', distribution='uniform')
+            bound = math.sqrt(3.0 / (cin * k * k))
+            w.uniform_(-bound, bound, generator=g)
+        else:
+            w.normal_(0, std, generator=g)
+        sd[name + ".weight"] = w
+        if bias:
+            sd[name + ".bias"] = torch.zeros(cout)
+
+    def norm(name, c, running, zero_gamma=False):
+        if reference_init:
+            sd[name + ".weight"] = torch.zeros(c) if zero_gamma else torch.ones(c)
+            sd[name + ".bias"] = torch.zeros(c)
+            if running:
+                sd[name + ".running_mean"] = torch.zeros(c)
+                sd[name + ".running_var"] = torch.ones(c)
+        else:
+            sd[name + ".weight"] = torch.empty(c).uniform_(0.5, 1.5, generator=g) * (residual_gain if zero_gamma else 1.0)
+            sd[name + ".bias"] = torch.empty(c).normal_(0, 0.1, generator=g)
+            if running:
+                sd[name + ".running_mean"] = torch.empty(c).normal_(0, 0.1, generator=g)
+                sd[name + ".running_var"] = torch.empty(c).uniform_(0.5, 1.5, generator=g)
+
+    return conv, norm
+
+
+def _draw_head(sd, g, conv, norm, reference_init, num_classes, feat):
+    """OrientedRepPointsHead (orientedreppoints_head.py:134-146)"""
+    std = 0.01 if reference_init else 0.03
+    for i in range(3):
+        conv("bbox_head.cls_convs.%d.conv" % i, feat, feat, 3, "normal", std=std)
+        norm("bbox_head.cls_convs.%d.gn" % i, feat, False)
+        conv("bbox_head.reg_convs.%d.conv" % i, feat, feat, 3, "normal", std=std)
+        norm("bbox_head.reg_convs.%d.gn" % i, feat, False)
+    conv("bbox_head.reppoints_cls_conv", feat, feat, 3, "normal", std=std)                 # DeformConv, no bias
+    conv("bbox_head.reppoints_cls_out", num_classes - 1, feat, 1, "normal", bias=True, std=std)
+    sd["bbox_head.reppoints_cls_out.bias"].fill_(-math.log((1 - 0.01) / 0.01))            # bias_init_with_prob(0.01)
+    conv("bbox_head.reppoints_pts_init_conv", feat, feat, 3, "normal", bias=True, std=std)
+    conv("bbox_head.reppoints_pts_init_out", 18, feat, 1, "normal", bias=True, std=std)
+    conv("bbox_head.reppoints_pts_refine_conv", feat, feat, 3, "normal", std=std)          # DeformConv, no bias
+    conv("bbox_head.reppoints_pts_refine_out", 18, feat, 1, "normal", bias=True, std=std)
+    if not reference_init:
+        for k in list(sd):
+            if k.endswith("_out.bias") or k.endswith("init_conv.bias"):
+                sd[k] = sd[k] + torch.empty_like(sd[k]).normal_(0, 0.1, generator=g)
+        # spread the predicted points so that the deformable sampling actually leaves the 3x3 grid
+        sd["bbox_head.reppoints_pts_init_out.bias"] += torch.empty(18).uniform_(-1.5, 1.5, generator=g)
+
+
+
 def random_state_dict(depth=50, seed=0, reference_init=True, num_classes=16, feat=256, residual_gain=1.0, dcn=None,
                       stage_with_dcn=(False, False, False, False), dcn_offset_scale=0.0, groups=1, base_width=4):
     """reference_init=True reproduces the reference's init_weights (incl. zero_init_residual and all-ones
@@ -91,32 +154,7 @@ def random_state_dict(depth=50, seed=0, reference_init=True, num_classes=16, fea
     g = torch.Generator().manual_seed(seed)
     sd = {}
     layout = dcn_layout(depth, dcn, stage_with_dcn)
-
-    def conv(name, cout, cin, k, init, bias=False, std=0.01):
-        w = torch.empty(cout, cin, k, k)                              # (grouped conv2: cin = channels per group)
-        if init == "kaiming":
-            _kaiming_fan_out(w, g)
-        elif init == "xavier":
-            _xavier_uniform(w, g)
-        else:
-            w.normal_(0, std, generator=g)
-        sd[name + ".weight"] = w
-        if bias:
-            sd[name + ".bias"] = torch.zeros(cout)
-
-    def norm(name, c, running, zero_gamma=False):
-        if reference_init:
-            sd[name + ".weight"] = torch.zeros(c) if zero_gamma else torch.ones(c)
-            sd[name + ".bias"] = torch.zeros(c)
-            if running:
-                sd[name + ".running_mean"] = torch.zeros(c)
-                sd[name + ".running_var"] = torch.ones(c)
-        else:
-            sd[name + ".weight"] = torch.empty(c).uniform_(0.5, 1.5, generator=g) * (residual_gain if zero_gamma else 1.0)
-            sd[name + ".bias"] = torch.empty(c).normal_(0, 0.1, generator=g)
-            if running:
-                sd[name + ".running_mean"] = torch.empty(c).normal_(0, 0.1, generator=g)
-                sd[name + ".running_var"] = torch.empty(c).uniform_(0.5, 1.5, generator=g)
+    conv, norm = _drawers(sd, g, reference_init, residual_gain)
 
     # ---------------------------------------------------------------- backbone (resnet.py)
     conv("backbone.conv1", 64, 3, 7, "kaiming")
@@ -160,26 +198,7 @@ def random_state_dict(depth=50, seed=0, reference_init=True, num_classes=16, fea
     norm("neck.fpn_convs.3.gn", feat, False)
     conv("neck.fpn_convs.4.conv", feat, feat, 3, "xavier")
     norm("neck.fpn_convs.4.gn", feat, False)
-    # ---------------------------------------------------------------- head (orientedreppoints_head.py:134-146)
-    std = 0.01 if reference_init else 0.03
-    for i in range(3):
-        conv("bbox_head.cls_convs.%d.conv" % i, feat, feat, 3, "normal", std=std)
-        norm("bbox_head.cls_convs.%d.gn" % i, feat, False)
-        conv("bbox_head.reg_convs.%d.conv" % i, feat, feat, 3, "normal", std=std)
-        norm("bbox_head.reg_convs.%d.gn" % i, feat, False)
-    conv("bbox_head.reppoints_cls_conv", feat, feat, 3, "normal", std=std)                 # DeformConv, no bias
-    conv("bbox_head.reppoints_cls_out", num_classes - 1, feat, 1, "normal", bias=True, std=std)
-    sd["bbox_head.reppoints_cls_out.bias"].fill_(-math.log((1 - 0.01) / 0.01))            # bias_init_with_prob(0.01)
-    conv("bbox_head.reppoints_pts_init_conv", feat, feat, 3, "normal", bias=True, std=std)
-    conv("bbox_head.reppoints_pts_init_out", 18, feat, 1, "normal", bias=True, std=std)
-    conv("bbox_head.reppoints_pts_refine_conv", feat, feat, 3, "normal", std=std)          # DeformConv, no bias
-    conv("bbox_head.reppoints_pts_refine_out", 18, feat, 1, "normal", bias=True, std=std)
-    if not reference_init:
-        for k in list(sd):
-            if k.endswith("_out.bias") or k.endswith("init_conv.bias"):
-                sd[k] = sd[k] + torch.empty_like(sd[k]).normal_(0, 0.1, generator=g)
-        # spread the predicted points so that the deformable sampling actually leaves the 3x3 grid
-        sd["bbox_head.reppoints_pts_init_out.bias"] += torch.empty(18).uniform_(-1.5, 1.5, generator=g)
+    _draw_head(sd, g, conv, norm, reference_init, num_classes, feat)
     return sd
 
 
@@ -188,3 +207,34 @@ def fold_bn(w, bn_w, bn_b, mean, var, eps=1e-5):
     tools/fuse_conv_bn.py:10-24.  Returns (w', b')."""
     factor = bn_w / torch.sqrt(var + eps)
     return w * factor.reshape(-1, 1, 1, 1), bn_b - mean * factor
+
+
+def random_hrnet_state_dict(arch="hrnetv2p_w32", seed=0, reference_init=True, num_classes=16, residual_gain=1.0, feat=256,
+                            zero_init_residual=False):
+    """state dict of HRNet(arch) + HRFPN(arch.out_widths, feat) + the head, with the reference's keys.
+    arch: a key of hrnet.ARCHS or an hrnet.HRNetArch.  reference_init=True reproduces the reference's init_weights: kaiming
+    (fan_out, normal) on every backbone conv and constant-1 norms (hrnet.py:462-478; with zero_init_residual, each residual
+    block's last norm constant 0),
+    caffe2_xavier_init with zero biases on HRFPN (hrfpn.py:73-76), the head's own init.  False randomises the norms as
+    random_state_dict does, draws the backbone convs from N(0, 1 / fan_in) (kaiming's fan_out would amplify the 1x1 fuse
+    convs, 8 * w channels into w, 16-fold in variance) and HRFPN's biases from N(0, 0.1^2), so every branch and fuse path
+    carries signal at a bounded scale;
+    residual_gain scales the randomised scale of each residual block's last norm (BasicBlock bn2, Bottleneck bn3)"""
+    from .hrnet import ARCHS, backbone_convs
+    arch = ARCHS[arch] if isinstance(arch, str) else arch
+    g = torch.Generator().manual_seed(seed)
+    sd = {}
+    conv, norm = _drawers(sd, g, reference_init, residual_gain)
+    for ck, bk, cout, cin, k, last in backbone_convs(arch):
+        conv("backbone." + ck, cout, cin, k, "kaiming" if reference_init else "fan_in")
+        norm("backbone." + bk, cout, True, zero_gamma=last and (zero_init_residual or not reference_init))
+    conv("neck.reduction_conv.conv", feat, sum(arch.out_widths), 1, "caffe2_xavier", bias=True)
+    for i in range(5):
+        conv("neck.fpn_convs.%d.conv" % i, feat, feat, 3, "caffe2_xavier", bias=True)
+    if not reference_init:
+        for k in list(sd):
+            if k.startswith("neck."):
+                if k.endswith(".bias"):
+                    sd[k] = torch.empty_like(sd[k]).normal_(0, 0.1, generator=g)
+    _draw_head(sd, g, conv, norm, reference_init, num_classes, feat)
+    return sd
