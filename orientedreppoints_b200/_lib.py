@@ -1,5 +1,5 @@
 """ctypes binding of liborp_b200.so (include/orp_b200.h, orp_b200_dcnv2.h, orp_b200_swin.h, orp_b200_group.h,
-orp_b200_hrnet.h).
+orp_b200_hrnet.h, orp_b200_attention.h).
 
 There is NO fallback: if the shared library is missing or a call fails, an exception is raised.
 The library is built in-tree by `python -m orientedreppoints_b200.build` (nvcc, sm_90a).
@@ -177,6 +177,32 @@ HRNET_SIGNATURES = {
     "orp_hrfpn_pool_f32": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp]),
 }
 
+
+
+class GenAttentionArgs(ctypes.Structure):
+    _fields_ = [(k, _vp) for k in ("q_c", "q_p", "k", "v", "pos_x", "pos_y", "out")] + \
+              [(k, _i) for k in ("N", "H", "W", "Hk", "Wk", "kv_stride", "C", "heads", "ld_q", "ld_kv")]
+
+
+class GenAttentionPlan(ctypes.Structure):
+    _fields_ = [(k, _i) for k in ("head_dim", "queries_per_cta", "threads", "grid_x", "grid_y", "grid_z", "smem_bytes", "rx", "ry",
+                                  "content", "position")]
+
+    def as_dict(self):
+        return {k: int(getattr(self, k)) for k, _ in self._fields_}
+
+
+# name -> (restype, argtypes); every symbol include/orp_b200_attention.h declares
+ATTENTION_SIGNATURES = {
+    "orp_gen_attention_bf16": (_i, [ctypes.POINTER(GenAttentionArgs), _vp]),
+    "orp_gen_attention_f16x3": (_i, [ctypes.POINTER(GenAttentionArgs), _vp]),
+    "orp_gen_attention_f32": (_i, [ctypes.POINTER(GenAttentionArgs), _vp]),
+    "orp_gen_attention_make_plan": (_i, [ctypes.POINTER(GenAttentionArgs), _i, ctypes.POINTER(GenAttentionPlan)]),
+    "orp_gen_attention_bcast_add_bf16": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp]),
+    "orp_gen_attention_bcast_add_f16x3": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp]),
+    "orp_gen_attention_bcast_add_f32": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp]),
+}
+
 _LIB = None
 
 
@@ -194,7 +220,7 @@ def lib():
                 "(there is no CPU or PyTorch fallback for this path)" % LIB_PATH)
         l = ctypes.CDLL(LIB_PATH)
         for name, (res, args) in list(SIGNATURES.items()) + list(DCNV2_SIGNATURES.items()) + list(SWIN_SIGNATURES.items()) + \
-                list(GROUP_SIGNATURES.items()) + list(HRNET_SIGNATURES.items()):
+                list(GROUP_SIGNATURES.items()) + list(HRNET_SIGNATURES.items()) + list(ATTENTION_SIGNATURES.items()):
             fn = getattr(l, name)   # AttributeError if the symbol is not exported
             fn.restype = res
             fn.argtypes = args
@@ -287,6 +313,28 @@ def tc_plan_group_for(problems, width, groups, stride, *, split=False, bias=True
     p = TcPlan()
     check(lib().orp_tc_plan_group_conv(len(problems), arr, ph, width, groups, stride, ph if bias else None, int(relu), int(out_f32),
                                        int(split), sms, ctypes.byref(p)), "orp_tc_plan_group_conv")
+    return p.as_dict()
+
+
+GEN_ATTENTION_FORMATS = {"bf16": 0, "f16x3": 1, "fp32": 2}
+
+
+def gen_attention_plan_for(fmt, N, H, W, C, heads, kv_stride, *, content=True, position=True, Hk=None, Wk=None, ld_q=None,
+                           ld_kv=None):
+    """the plan orp_gen_attention_make_plan reports for one attention launch in format fmt ('bf16' / 'f16x3' / 'fp32'), with
+    placeholder pointers (never read, no device needed); Hk / Wk default to ceil(H / kv_stride), ceil(W / kv_stride)"""
+    ph = 256
+    a = GenAttentionArgs()
+    a.q_c, a.k = (ph, ph) if content else (None, None)
+    a.q_p, a.pos_x, a.pos_y = (ph, ph, ph) if position else (None, None, None)
+    a.v, a.out = ph, 512
+    a.N, a.H, a.W, a.C, a.heads, a.kv_stride = N, H, W, C, heads, kv_stride
+    a.Hk = -(-H // kv_stride) if Hk is None else Hk
+    a.Wk = -(-W // kv_stride) if Wk is None else Wk
+    a.ld_q = 2 * C if ld_q is None else ld_q
+    a.ld_kv = 2 * C if ld_kv is None else ld_kv
+    p = GenAttentionPlan()
+    check(lib().orp_gen_attention_make_plan(ctypes.byref(a), GEN_ATTENTION_FORMATS[fmt], ctypes.byref(p)), "orp_gen_attention_make_plan")
     return p.as_dict()
 
 

@@ -31,6 +31,7 @@ def _headers():
     hs.append(os.path.join(HERE, "..", "include", "orp_b200_swin.h"))
     hs.append(os.path.join(HERE, "..", "include", "orp_b200_group.h"))
     hs.append(os.path.join(HERE, "..", "include", "orp_b200_hrnet.h"))
+    hs.append(os.path.join(HERE, "..", "include", "orp_b200_attention.h"))
     return hs
 
 

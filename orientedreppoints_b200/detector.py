@@ -151,7 +151,8 @@ class OrientedRepPointsDetector:
     """R-50 / R-101 / R-152, ResNeXt of those depths, or Swin-T/S/B/L + FPN(GN), or HRNet + HRFPN, + OrientedRepPointsHead,
     inference only."""
 
-    def __init__(self, state_dict, depth=50, device="cuda", precision="fp32", test_cfg=None, dcn=None, pooling_type='AVG'):
+    def __init__(self, state_dict, depth=50, device="cuda", precision="fp32", test_cfg=None, dcn=None, pooling_type='AVG',
+                 gen_attention=None):
         """depth: 50 / 101 / 152 (ResNet or ResNeXt: the groups of every conv2 come from the state dict's shapes), or a Swin backbone - "swin_tiny" (Swin-T, window 7), any key of swin.ARCHS
         ("swin_small", "swin_base_w12", ...) or a swin.SwinArch, or an HRNet backbone with the HRFPN neck (stride 2, five
         outputs) - a key of hrnet.ARCHS ("hrnetv2p_w18", ...) or an hrnet.HRNetArch.
@@ -170,6 +171,7 @@ class OrientedRepPointsDetector:
             raise ValueError("pooling_type must be 'AVG' or 'MAX', not %r" % (pooling_type,))
         self.pooling_type = pooling_type
         self.dcn = dcn
+        self.gen_attention = gen_attention
         self.test_cfg = dict(nms_pre=2000, min_bbox_size=0, score_thr=0.05, nms=dict(type='rnms', iou_thr=0.4),
                              max_per_img=2000)                         # configs/dota/orientedrepoints_r50_demo.py:62-67
         if test_cfg:
@@ -196,6 +198,9 @@ class OrientedRepPointsDetector:
     # ------------------------------------------------------------------ weights
     def _load(self, sd):
         d = self.device
+        if self.gen_attention is not None and (self.swin_arch is not None or self.hr_arch is not None):
+            raise ValueError("gen_attention describes the attention blocks of a ResNet backbone; %s has none"
+                             % ("the Swin backbone" if self.swin_arch is not None else "the HRNet backbone"))
         if self.swin_arch is not None:
             if self.dcn is not None:
                 raise ValueError("dcn describes the deformable layers of a ResNet backbone; the Swin backbone has none")
@@ -220,6 +225,14 @@ class OrientedRepPointsDetector:
         if self.groups > 1 and any(k is not None for s in layout for k in s):
             raise NotImplementedError("dcn on a ResNeXt with groups=%d would be a grouped deformable convolution: not built"
                                       % self.groups)
+        ga = self.gen_attention if self.gen_attention is not None else tuple((None,) * n for n in STAGE_BLOCKS[self.depth])
+        if tuple(len(s) for s in ga) != STAGE_BLOCKS[self.depth] or \
+                any(sp is not None and not isinstance(sp, dict) for s in ga for sp in s):
+            raise ValueError("gen_attention must give None or a gen_attention_spec for each of the %s blocks of R-%d"
+                             % (STAGE_BLOCKS[self.depth], self.depth))
+        if self.groups > 1 and any(sp is not None for s in ga for sp in s):
+            raise NotImplementedError("gen_attention on a ResNeXt: the reference's ResNeXt builds no attention blocks "
+                                      "(resnext.py:196-216)")
         self.stem = folded("backbone.conv1", "backbone.bn1", 2, 3, pad_cin_to=4)
         self.blocks = []
         for li, nblk in enumerate(STAGE_BLOCKS[self.depth]):
@@ -232,6 +245,7 @@ class OrientedRepPointsDetector:
                            ds=folded(p + ".downsample.0", p + ".downsample.1", s, 0) if b == 0 else None)
                 blk["dcn"] = layout[li][b]
                 blk["off"] = self._offset_conv(sd, p + ".conv2", blk["dcn"], 64 << li, s)
+                blk["att"] = self._gen_attention_block(sd, p, ga[li][b], 64 << li)
                 stage.append(blk)
             self.blocks.append(stage)
         self.lat = [(ConvLayer(sd["neck.lateral_convs.%d.conv.weight" % i].float(), None, 1, 0, d),
@@ -290,6 +304,18 @@ class OrientedRepPointsDetector:
                              % (conv2, kind, planes, planes, co, planes, co))
         return ConvLayer(sd[conv2 + ".conv_offset.weight"].float(), sd[conv2 + ".conv_offset.bias"].float(), stride, 1,
                          self.device)
+
+    def _gen_attention_block(self, sd, prefix, spec, planes):
+        """the engine form of a block's gen_attention_block (gen_attention.GenAttentionBlock), None without one; ValueError when
+        the state dict contradicts the layout"""
+        from .gen_attention import GenAttentionBlock, check_block
+        if spec is None:
+            check_block(sd, prefix, None)
+            return None
+        if spec.get('channels') != planes:
+            raise ValueError("%s: the gen_attention spec is for %r channels where the block's conv2 has %d"
+                             % (prefix, spec.get('channels'), planes))
+        return GenAttentionBlock(sd, prefix, spec, self.device)
 
     def _conv2(self, x, blk):
         """a block's 3x3 convolution + folded bn2 + ReLU.  Deformable (DCN / DCNv2): the offset convolution writes fp32 NHWC
@@ -409,6 +435,8 @@ class OrientedRepPointsDetector:
                 idt = x if blk["ds"] is None else e.conv(x, blk["ds"])
                 o = e.conv(x, blk["c1"], relu=True)
                 o = self._conv2(o, blk)
+                if blk["att"] is not None:                              # resnet.py:216-217, between relu(bn2) and conv3
+                    o = blk["att"](e, o)
                 x = e.conv(o, blk["c3"], relu=True, residual=idt)
             feats.append(x)
         c3, c4, c5 = feats[1], feats[2], feats[3]

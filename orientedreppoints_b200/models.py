@@ -16,7 +16,7 @@ from .ops.conv_module import ConvModule
 from .ops.dcn import DeformConv, DeformConvPack, ModulatedDeformConvPack
 from .ops.norm import build_norm_layer
 from .utils.registry import Registry, build_from_cfg
-from .weights import STAGE_BLOCKS, block_width, check_groups
+from .weights import STAGE_BLOCKS, block_width, check_groups, gen_attention_spec
 
 BACKBONES = Registry('backbone')
 NECKS = Registry('neck')
@@ -57,6 +57,31 @@ class _EngineOnly(nn.Module):
                                   "on the liborp_b200 engine" % type(self).__name__)
 
 
+class GeneralizedAttention(_EngineOnly):
+    """the parameter tree of generalized_attention.py:34-150 for a spec of weights.gen_attention_spec: only the layers that
+    attention_type uses exist (query_conv for t0 / t1, key_conv for t0 / t2, appr_geom_fc_{x,y} for t1 / t3, appr_bias for t2,
+    geom_bias for t3); value_conv, proj_conv (with bias) and gamma always"""
+
+    def __init__(self, in_dim, spec):
+        super().__init__()
+        t, c, e = spec['attention_type'], in_dim, spec['position_embedding_dim']
+        self.spec = spec
+        if t[0] or t[1]:
+            self.query_conv = nn.Conv2d(c, c, 1, bias=False)
+        if t[0] or t[2]:
+            self.key_conv = nn.Conv2d(c, c, 1, bias=False)
+        self.value_conv = nn.Conv2d(c, c, 1, bias=False)
+        if t[1] or t[3]:
+            self.appr_geom_fc_x = nn.Linear(e // 2, c, bias=False)
+            self.appr_geom_fc_y = nn.Linear(e // 2, c, bias=False)
+        if t[2]:
+            self.appr_bias = nn.Parameter(torch.zeros(c))
+        if t[3]:
+            self.geom_bias = nn.Parameter(torch.zeros(c))
+        self.proj_conv = nn.Conv2d(c, c, 1, bias=True)
+        self.gamma = nn.Parameter(torch.zeros(1))
+
+
 class Bottleneck(_EngineOnly):
     """resnet.py:84-239 (style 'pytorch': the stride sits on the 3x3).  dcn: the conv2 config of resnet.py:146-168 - a
     DCN / DCNv2 layer (DeformConvPack / ModulatedDeformConvPack) unless `fallback_on_stride`, which is popped from the dict
@@ -64,7 +89,8 @@ class Bottleneck(_EngineOnly):
     groups / base_width: the ResNeXt block (resnext.py:11-70): conv1 / conv2 are block_width() wide, conv2 has `groups` groups"""
     expansion = 4
 
-    def __init__(self, inplanes, planes, stride, downsample, norm_cfg, conv_cfg=None, dcn=None, groups=1, base_width=4):
+    def __init__(self, inplanes, planes, stride, downsample, norm_cfg, conv_cfg=None, dcn=None, groups=1, base_width=4,
+                 gen_attention=None):
         super().__init__()
         width = block_width(planes, groups, base_width)
         self.conv1 = nn.Conv2d(inplanes, width, 1, bias=False)
@@ -79,6 +105,8 @@ class Bottleneck(_EngineOnly):
         self.conv3 = nn.Conv2d(width, planes * 4, 1, bias=False)
         self.add_module('bn3', build_norm_layer(norm_cfg, planes * 4, 3)[1])
         self.downsample = downsample
+        if gen_attention is not None:                                 # resnet.py:186-189, applied after relu(bn2(conv2))
+            self.gen_attention_block = GeneralizedAttention(planes, gen_attention_spec(gen_attention, planes))
 
 
 @BACKBONES.register_module
@@ -93,9 +121,9 @@ class ResNet(_EngineOnly):
         if depth not in self.arch_settings:
             raise KeyError('invalid depth {} for resnet'.format(depth))
         if style != 'pytorch' or num_stages != 4 or tuple(strides) != (1, 2, 2, 2) or tuple(dilations) != (1, 1, 1, 1) \
-                or gcb is not None or gen_attention is not None:
+                or gcb is not None:
             raise NotImplementedError("liborp_b200 builds the configuration of configs/dota/*.py: 4 stages, style 'pytorch', "
-                                      "strides (1,2,2,2), no dilation / GCB / attention in the backbone")
+                                      "strides (1,2,2,2), no dilation / GCB in the backbone")
         if dcn is not None:
             assert isinstance(dcn, dict) and len(stage_with_dcn) == num_stages
             if dcn.get('deformable_groups', 1) != 1:
@@ -105,6 +133,10 @@ class ResNet(_EngineOnly):
         self.zero_init_residual = zero_init_residual
         self.dcn, self.stage_with_dcn = dcn, tuple(stage_with_dcn)
         self.dcn_cfg = None if dcn is None else dict(dcn)           # as given, before the blocks pop fallback_on_stride
+        self.gen_attention = None if gen_attention is None else dict(gen_attention)
+        self.stage_with_gen_attention = tuple(tuple(s) for s in stage_with_gen_attention)
+        if gen_attention is not None:
+            assert isinstance(gen_attention, dict) and len(self.stage_with_gen_attention) == num_stages
         self.conv1 = nn.Conv2d(in_channels, 64, 7, 2, 3, bias=False)
         self.add_module('bn1', build_norm_layer(norm_cfg, 64, 1)[1])
         inplanes = 64
@@ -116,7 +148,10 @@ class ResNet(_EngineOnly):
                 ds = None
                 if b == 0:
                     ds = nn.Sequential(nn.Conv2d(inplanes, planes * 4, 1, stride, bias=False), build_norm_layer(norm_cfg, planes * 4)[1])
-                blocks.append(Bottleneck(inplanes, planes, stride, ds, norm_cfg, conv_cfg, stage_dcn, **self._block_args()))
+                # make_res_layer (resnet.py:283-300): block b gets the dict when b is listed; an index past the stage builds nothing
+                ga = self.gen_attention if b in self.stage_with_gen_attention[i] else None
+                blocks.append(Bottleneck(inplanes, planes, stride, ds, norm_cfg, conv_cfg, stage_dcn, gen_attention=ga,
+                                         **self._block_args()))
                 inplanes = planes * 4
             self.add_module('layer%d' % (i + 1), nn.Sequential(*blocks))
 
@@ -130,6 +165,13 @@ class ResNet(_EngineOnly):
         return tuple(tuple(kinds[type(blk.conv2)] for blk in getattr(self, 'layer%d' % (i + 1)))
                      for i in range(len(self.arch_settings[self.depth])))
 
+    def gen_attention_layout(self):
+        """per stage, per block: None, or the spec (weights.gen_attention_spec) of that block's gen_attention_block - what the
+        engine builds after its conv2"""
+        return tuple(tuple(blk.gen_attention_block.spec if hasattr(blk, 'gen_attention_block') else None
+                           for blk in getattr(self, 'layer%d' % (i + 1)))
+                     for i in range(len(self.arch_settings[self.depth])))
+
 
 @BACKBONES.register_module
 class ResNeXt(ResNet):
@@ -139,6 +181,9 @@ class ResNeXt(ResNet):
 
     def __init__(self, groups=1, base_width=4, **kwargs):
         check_groups(groups, base_width)
+        if kwargs.get('gen_attention') is not None and any(len(s) for s in kwargs.get('stage_with_gen_attention', ())):
+            raise NotImplementedError("gen_attention on ResNeXt: the reference's ResNeXt rebuilds every stage without it "
+                                      "(resnext.py:196-216), so its checkpoints hold no attention blocks; liborp_b200 does not build them")
         if groups > 1 and kwargs.get('dcn') is not None and any(kwargs.get('stage_with_dcn', ())):
             raise NotImplementedError("dcn with groups=%d would be a grouped deformable convolution (resnext.py:56-66): "
                                       "liborp_b200 does not build it" % groups)
@@ -410,9 +455,11 @@ class OrientedRepPointsDetector(nn.Module):
         import os
         if isinstance(self.backbone, ResNet):
             from .weights import random_state_dict
+            ga = dict(gen_attention=self.backbone.gen_attention,
+                      stage_with_gen_attention=self.backbone.stage_with_gen_attention) if self.backbone.gen_attention else {}
             sd = random_state_dict(self.backbone.depth, seed=0, reference_init=True, num_classes=self.bbox_head.num_classes,
                                    dcn=self.backbone.dcn_cfg, stage_with_dcn=self.backbone.stage_with_dcn,
-                                   **self.backbone._block_args())
+                                   **self.backbone._block_args(), **ga)
         elif isinstance(self.backbone, HRNet):
             from .weights import random_hrnet_state_dict
             sd = random_hrnet_state_dict(self.backbone.arch, seed=0, reference_init=True, num_classes=self.bbox_head.num_classes,
@@ -442,6 +489,7 @@ class OrientedRepPointsDetector(nn.Module):
             self._engine = Engine({k: v.detach() for k, v in self.state_dict().items()}, depth, dev, self.precision,
                                   test_cfg=dict(self.test_cfg) if self.test_cfg else None,
                                   dcn=self.backbone.dcn_layout() if resnet else None,
+                                  gen_attention=self.backbone.gen_attention_layout() if resnet else None,
                                   pooling_type=self.neck.pooling_type if hr else 'AVG')
         return self._engine
 

@@ -72,6 +72,109 @@ def dcn_layout(depth, dcn=None, stage_with_dcn=(False, False, False, False)):
     return tuple(layout)
 
 
+# GeneralizedAttention's arguments and their defaults (generalized_attention.py:34-42)
+GEN_ATTENTION_DEFAULTS = dict(spatial_range=-1, num_heads=9, position_embedding_dim=-1, position_magnitude=1, kv_stride=2,
+                              q_stride=1, attention_type='1111')
+
+
+def gen_attention_spec(cfg, planes):
+    """the block that GeneralizedAttention(planes, **cfg) builds, as the engine runs it: dict(attention_type (four bools),
+    num_heads, head_dim, kv_stride, position_embedding_dim, position_magnitude, channels).  NotImplementedError for what the
+    kernels do not run (spatial_range >= 0, q_stride != 1, kv_stride other than 1 or 2, planes % num_heads, a head dimension
+    other than 32 or 64), ValueError where the reference itself fails (an attention_type that is not four 0/1 digits, a position
+    embedding that is not a positive multiple of 4 when the position terms use it), TypeError for an unknown argument"""
+    unknown = sorted(set(cfg) - set(GEN_ATTENTION_DEFAULTS))
+    if unknown:
+        raise TypeError("GeneralizedAttention got unexpected arguments %s" % unknown)
+    a = dict(GEN_ATTENTION_DEFAULTS, **cfg)
+    t = a['attention_type']
+    if not isinstance(t, str) or len(t) != 4 or any(ch not in '01' for ch in t):
+        raise ValueError("attention_type=%r: generalized_attention.py reads four 0/1 digits" % (t,))
+    t = tuple(ch == '1' for ch in t)
+    if t[1] and not t[3]:
+        raise NotImplementedError("gen_attention with attention_type=%r: without the geom_bias term the reference's query-position "
+                                  "branch (generalized_attention.py:308-326) pairs the y-offset features with the query at the "
+                                  "transposed position and fails on maps that are not square; liborp_b200 runs the '0100' term "
+                                  "together with '0001' only" % (a['attention_type'],))
+    if a['spatial_range'] >= 0:
+        raise NotImplementedError("gen_attention with spatial_range=%r: the reference's local mask is hard-coded for 256 / 512 "
+                                  "channels and maps up to 84 / 42; liborp_b200 runs spatial_range=-1" % (a['spatial_range'],))
+    if a['q_stride'] != 1:
+        raise NotImplementedError("gen_attention with q_stride=%r: liborp_b200 runs q_stride=1" % (a['q_stride'],))
+    if a['kv_stride'] not in (1, 2):
+        raise NotImplementedError("gen_attention with kv_stride=%r: liborp_b200 runs kv_stride 1 or 2" % (a['kv_stride'],))
+    heads = a['num_heads']
+    if not isinstance(heads, int) or heads < 1:
+        raise ValueError("gen_attention with num_heads=%r: needs a positive integer" % (heads,))
+    if planes % heads or planes // heads not in (32, 64):
+        raise NotImplementedError("gen_attention with num_heads=%d on %d channels: liborp_b200 runs head dimensions "
+                                  "(channels / num_heads) of 32 and 64 that divide the channels" % (heads, planes))
+    e = a['position_embedding_dim'] if a['position_embedding_dim'] > 0 else planes
+    if (t[1] or t[3]) and e % 4:
+        raise ValueError("gen_attention with position_embedding_dim=%r: the embedding (generalized_attention.py:182-194) has "
+                         "2 * ceil(dim / 4) features where appr_geom_fc takes dim // 2; dim must be a multiple of 4" % (e,))
+    return dict(attention_type=t, num_heads=heads, head_dim=planes // heads, kv_stride=a['kv_stride'],
+                position_embedding_dim=e, position_magnitude=a['position_magnitude'], channels=planes)
+
+
+def gen_attention_layout(depth, gen_attention=None, stage_with_gen_attention=((), (), (), ())):
+    """what ResNet(depth, gen_attention=..., stage_with_gen_attention=...) builds after each block's conv2, per stage and
+    block: None or the block's gen_attention_spec.  An index past the stage's last block builds nothing (resnet.py:283-300)"""
+    return tuple(tuple(gen_attention_spec(gen_attention, 64 << li) if gen_attention is not None and b in stage_with_gen_attention[li]
+                       else None for b in range(nblk))
+                 for li, nblk in enumerate(STAGE_BLOCKS[depth]))
+
+
+def gen_attention_keys(spec):
+    """the parameter names (after `gen_attention_block.`) of a block with this spec, with their shapes"""
+    t, c, e = spec['attention_type'], spec['channels'], spec['position_embedding_dim']
+    keys = {}
+    if t[0] or t[1]:
+        keys['query_conv.weight'] = (c, c, 1, 1)
+    if t[0] or t[2]:
+        keys['key_conv.weight'] = (c, c, 1, 1)
+    keys['value_conv.weight'] = (c, c, 1, 1)
+    if t[1] or t[3]:
+        keys['appr_geom_fc_x.weight'] = (c, e // 2)
+        keys['appr_geom_fc_y.weight'] = (c, e // 2)
+    if t[2]:
+        keys['appr_bias'] = (c,)
+    if t[3]:
+        keys['geom_bias'] = (c,)
+    keys['proj_conv.weight'] = (c, c, 1, 1)
+    keys['proj_conv.bias'] = (c,)
+    keys['gamma'] = (1,)
+    return keys
+
+
+def _draw_gen_attention(sd, p, spec, g, gamma):
+    """a gen_attention_block as the reference initialises it: ResNet.init_weights' kaiming (fan_out, normal, zero bias) on
+    its four convolutions (resnet.py:474-476 re-draws every nn.Conv2d), kaiming_uniform(a=1) on appr_geom_fc_{x,y}
+    (generalized_attention.py:374-383), appr_bias / geom_bias uniform in +-1/sqrt(2 d), gamma 0.
+    gamma > 0 (tests only): gamma is that value, and query_conv / key_conv / appr_geom_fc are drawn 1/d^(1/4) narrower, so
+    that content and position energies have about unit spread for unit-variance inputs instead of ~sqrt(d)"""
+    c, d = spec['channels'], spec['head_dim']
+    shrink = d ** -0.25 if gamma > 0 else 1.0
+    for name, shape in gen_attention_keys(spec).items():
+        k = p + '.gen_attention_block.' + name
+        w = torch.empty(shape)
+        if name.endswith('conv.weight'):
+            _kaiming_fan_out(w, g)
+            if name.startswith(('query', 'key')):
+                w *= shrink
+        elif name.startswith('appr_geom_fc'):
+            bound = math.sqrt(3.0 / shape[1])
+            w.uniform_(-bound, bound, generator=g).mul_(shrink)
+        elif name in ('appr_bias', 'geom_bias'):
+            stdv = 1.0 / math.sqrt(2 * d)
+            w.uniform_(-stdv, stdv, generator=g)
+        elif name == 'gamma':
+            w.fill_(gamma)
+        else:                                                          # proj_conv.bias
+            w.zero_()
+        sd[k] = w
+
+
 def _drawers(sd, g, reference_init, residual_gain):
     """the (conv, norm) draws of the random state dicts into sd from generator g"""
 
@@ -135,7 +238,8 @@ def _draw_head(sd, g, conv, norm, reference_init, num_classes, feat):
 
 
 def random_state_dict(depth=50, seed=0, reference_init=True, num_classes=16, feat=256, residual_gain=1.0, dcn=None,
-                      stage_with_dcn=(False, False, False, False), dcn_offset_scale=0.0, groups=1, base_width=4):
+                      stage_with_dcn=(False, False, False, False), dcn_offset_scale=0.0, groups=1, base_width=4,
+                      gen_attention=None, stage_with_gen_attention=((), (), (), ()), gen_attention_gamma=0.0):
     """reference_init=True reproduces the reference's init_weights (incl. zero_init_residual and all-ones
     norm scales); False randomises norm parameters / running statistics so that every branch of the graph
     carries signal (used by the parity tests); residual_gain scales the randomised scale of every block's last norm
@@ -147,13 +251,19 @@ def random_state_dict(depth=50, seed=0, reference_init=True, num_classes=16, fea
     instead, so that the samples leave the grid by about `scale` pixels per unit of input and the DCNv2 mask logits vary;
     with zero offsets a deformable layer is a plain convolution.
     groups / base_width: a ResNeXt (resnext.py): conv1 / conv2 / bn1 / bn2 are block_width() wide and conv2 has `groups` groups,
-    its kaiming fan_out width * 9 as for any nn.Conv2d.  groups=1 draws exactly the ResNet's tensors."""
+    its kaiming fan_out width * 9 as for any nn.Conv2d.  groups=1 draws exactly the ResNet's tensors.
+    gen_attention / stage_with_gen_attention: the blocks' gen_attention_block as ResNet takes them (gen_attention_layout),
+    drawn by _draw_gen_attention after the block's other tensors; gen_attention_gamma > 0 (tests only) makes them act (see
+    there).  Without attention blocks every draw is what it was without these arguments."""
     check_groups(groups, base_width)
     if groups > 1 and dcn is not None and any(stage_with_dcn):
         raise NotImplementedError("dcn with groups=%d would be a grouped deformable convolution (resnext.py:56-66): not built" % groups)
     g = torch.Generator().manual_seed(seed)
     sd = {}
     layout = dcn_layout(depth, dcn, stage_with_dcn)
+    ga_layout = gen_attention_layout(depth, gen_attention, stage_with_gen_attention)
+    if groups > 1 and any(sp is not None for st in ga_layout for sp in st):
+        raise NotImplementedError("gen_attention on ResNeXt: the reference's ResNeXt builds no attention blocks (resnext.py:196-216)")
     conv, norm = _drawers(sd, g, reference_init, residual_gain)
 
     # ---------------------------------------------------------------- backbone (resnet.py)
@@ -187,6 +297,8 @@ def random_state_dict(depth=50, seed=0, reference_init=True, num_classes=16, fea
             if b == 0:
                 conv(p + ".downsample.0", planes * 4, inplanes, 1, "kaiming")
                 norm(p + ".downsample.1", planes * 4, True)
+            if ga_layout[li][b] is not None:
+                _draw_gen_attention(sd, p, ga_layout[li][b], g, gen_attention_gamma)
             inplanes = planes * 4
     # ---------------------------------------------------------------- neck (fpn.py, start_level=1, 5 outs)
     for i, cin in enumerate((512, 1024, 2048)):
