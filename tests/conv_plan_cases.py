@@ -203,6 +203,137 @@ PARITY = [
     (('bf16', 0, 'bf16', 64, 1, 0, 0, 0, 0, 0, 1, 1, 6, 0, 0, 0, 0, 0, 0, 0), 'bf16', 'conv', 2048, 256, 3, 2, 0, 0, 0, 0, 1, [(5, 37, 43)]),
     # r50 p7
     (('bf16', 0, 'f32', 128, 0, 0, 0, 0, 0, 0, 1, 0, 5, 0, 0, 1, 0, 1, 0, 0), 'bf16', 'conv', 256, 256, 3, 2, 0, 0, 0, 0, 1, [(4, 33, 23)]),
+    # ---- the ResNeXt, HRNet + HRFPN, DCN-stage and GeneralizedAttention graphs (16 x 1024^2, 4 x 960^2): the layer names are
+    # the reference's module paths; HRNet's widths are padded to multiples of 8 (W18: 24 / 40 / 72 / 144), so each case keeps
+    # the Cin (partial 64-channel K block, or a Cin below one block) and Cout (padded up inside the BN tile) of its layers
+    # hrnet-w18 bf16 x16 fpn_convs.2: Cin 256 x Cout 256 k3 s2
+    (('bf16', 0, 'bf16', 256, 1, 0, 0, 0, 0, 0, 1, 0, 3, 0, 1, 0, 0, 0, 0, 0), 'bf16', 'conv', 256, 256, 3, 2, 1, 0, 0, 0, 0, [(6, 81, 123)]),
+    # r50-ga bf16 x16 layer4.*.att.kv: Cin 512 x Cout 1024 k1 s2
+    (('bf16', 0, 'bf16', 256, 1, 0, 0, 0, 0, 0, 2, 0, 3, 0, 0, 0, 0, 0, 0, 0), 'bf16', 'conv', 512, 1024, 1, 2, 0, 0, 0, 0, 0, [(6, 155, 15)]),
+    # r50-ga bf16 x16 layer3.*.att.kv: Cin 256 x Cout 512 k1 s2
+    (('bf16', 0, 'bf16', 256, 1, 0, 0, 0, 0, 0, 2, 0, 3, 0, 0, 0, 0, 1, 0, 0), 'bf16', 'conv', 256, 512, 1, 2, 0, 0, 0, 0, 0, [(6, 35, 139)]),
+    # x101-64x4d bf16 x16 layer1.*.c1: Cin 64 x Cout 256 k1 s1
+    (('bf16', 0, 'bf16', 256, 1, 0, 0, 0, 1, 0, 2, 0, 6, 1, 1, 0, 0, 1, 0, 0), 'bf16', 'conv', 64, 256, 1, 1, 1, 1, 0, 0, 0, [(1, 133, 129)]),
+    # hrnet-w18 bf16 x16 stage4.*.branches.3.*.conv1: Cin 144 x Cout 144 k3 s1 (the plan also runs Cin x Cout 256x24)
+    (('bf16', 0, 'bf16', 32, 0, 0, 0, 0, 0, 0, 1, 0, 6, 1, 1, 0, 0, 1, 1, 0), 'bf16', 'conv', 144, 144, 3, 1, 1, 1, 0, 0, 0, [(3, 33, 33)]),
+    # hrnet-w18 bf16 x16 stage3.*.branches.2.*.conv1, stage4.*.branches.2.*.conv1: Cin 72 x Cout 72 k3 s1 (the plan also runs Cin x Cout 72x144)
+    (('bf16', 0, 'bf16', 32, 0, 0, 0, 0, 1, 0, 1, 0, 6, 1, 1, 0, 0, 1, 1, 0), 'bf16', 'conv', 72, 72, 3, 1, 1, 1, 0, 0, 0, [(5, 33, 33)]),
+    # hrnet-w18 bf16 x16 stage4.*.fuse_layers.0.3.0: Cin 144 x Cout 24 k1 s1
+    (('bf16', 0, 'bf16', 32, 0, 0, 0, 0, 1, 0, 2, 0, 6, 0, 1, 0, 0, 0, 1, 0), 'bf16', 'conv', 144, 24, 1, 1, 1, 0, 0, 0, 0, [(1, 2, 2)]),
+    # hrnet-w18 bf16 x16 stage2.*.fuse_layers.0.1.0, stage3.*.fuse_layers.0.1.0, stage4.*.fuse_layers.0.1.0: Cin 40 x Cout 24 k1 s1 (the plan also runs Cin x Cout 72x24, 144x72)
+    (('bf16', 0, 'bf16', 32, 0, 0, 0, 0, 1, 0, 2, 0, 6, 0, 1, 0, 0, 1, 1, 0), 'bf16', 'conv', 40, 24, 1, 1, 1, 0, 0, 0, 0, [(1, 133, 129)]),
+    # hrnet-w18 bf16 x16 stage2.*.branches.0.*.conv1, stage3.*.branches.0.*.conv1, stage4.*.branches.0.*.conv1: Cin 24 x Cout 24 k3 s1 (the plan also runs Cin x Cout 40x72)
+    (('bf16', 0, 'bf16', 32, 0, 0, 0, 0, 1, 0, 2, 0, 6, 1, 1, 0, 0, 1, 1, 0), 'bf16', 'conv', 24, 24, 3, 1, 1, 1, 0, 0, 0, [(1, 133, 129)]),
+    # hrnet-w18 bf16 x16 stage4.*.branches.3.*.conv2: Cin 144 x Cout 144 k3 s1
+    (('bf16', 0, 'bf16', 32, 0, 0, 0, 1, 0, 0, 2, 0, 6, 1, 1, 0, 0, 1, 1, 0), 'bf16', 'conv', 144, 144, 3, 1, 1, 1, 0, 1, 0, [(3, 33, 33)]),
+    # hrnet-w18 bf16 x16 stage3.*.fuse_layers.2.0.1, stage4.*.fuse_layers.2.0.1: Cin 24 x Cout 72 k3 s2 (the plan also runs Cin x Cout 24x144, 40x72, 40x144)
+    (('bf16', 0, 'bf16', 32, 0, 0, 0, 1, 1, 0, 2, 0, 6, 0, 1, 0, 0, 1, 1, 0), 'bf16', 'conv', 24, 72, 3, 2, 1, 0, 0, 1, 0, [(5, 65, 65)]),
+    # hrnet-w18 bf16 x16 stage2.*.branches.0.*.conv2, stage3.*.branches.0.*.conv2, stage4.*.branches.0.*.conv2: Cin 24 x Cout 24 k3 s1 (the plan also runs Cin x Cout 40x72, 72x72, 72x144)
+    (('bf16', 0, 'bf16', 32, 0, 0, 0, 1, 1, 0, 2, 0, 6, 1, 1, 0, 0, 1, 1, 0), 'bf16', 'conv', 24, 24, 3, 1, 1, 1, 0, 1, 0, [(1, 133, 129)]),
+    # hrnet-w18 bf16 x16 transition1.1.0: Cin 256 x Cout 40 k3 s2
+    (('bf16', 0, 'bf16', 64, 0, 0, 0, 0, 0, 0, 1, 0, 6, 1, 1, 0, 0, 1, 1, 0), 'bf16', 'conv', 256, 40, 3, 2, 1, 1, 0, 0, 0, [(5, 105, 129)]),
+    # hrnet-w18 bf16 x16 stage4.*.fuse_layers.1.3.0: Cin 144 x Cout 40 k1 s1
+    (('bf16', 0, 'bf16', 64, 0, 0, 0, 0, 1, 0, 2, 0, 6, 0, 1, 0, 0, 0, 1, 0), 'bf16', 'conv', 144, 40, 1, 1, 1, 0, 0, 0, 0, [(1, 2, 2)]),
+    # hrnet-w18 bf16 x16 stage3.*.fuse_layers.1.2.0, stage4.*.fuse_layers.1.2.0: Cin 72 x Cout 40 k1 s1
+    (('bf16', 0, 'bf16', 64, 0, 0, 0, 0, 1, 0, 2, 0, 6, 0, 1, 0, 0, 1, 1, 0), 'bf16', 'conv', 72, 40, 1, 1, 1, 0, 0, 0, 0, [(1, 133, 129)]),
+    # hrnet-w18 bf16 x16 stage2.*.branches.1.*.conv1, stage3.*.branches.1.*.conv1, stage4.*.branches.1.*.conv1: Cin 40 x Cout 40 k3 s1
+    (('bf16', 0, 'bf16', 64, 0, 0, 0, 0, 1, 0, 2, 0, 6, 1, 1, 0, 0, 1, 1, 0), 'bf16', 'conv', 40, 40, 3, 1, 1, 1, 0, 0, 0, [(1, 133, 129)]),
+    # hrnet-w18 bf16 x16 stage3.*.fuse_layers.1.0.0, stage4.*.fuse_layers.1.0.0: Cin 24 x Cout 40 k3 s2
+    (('bf16', 0, 'bf16', 64, 0, 0, 0, 1, 1, 0, 2, 0, 6, 0, 1, 0, 0, 1, 1, 0), 'bf16', 'conv', 24, 40, 3, 2, 1, 0, 0, 1, 0, [(5, 105, 129)]),
+    # hrnet-w18 bf16 x16 stage2.*.branches.1.*.conv2, stage3.*.branches.1.*.conv2, stage4.*.branches.1.*.conv2: Cin 40 x Cout 40 k3 s1 (the plan also runs Cin x Cout 24x40)
+    (('bf16', 0, 'bf16', 64, 0, 0, 0, 1, 1, 0, 2, 0, 6, 1, 1, 0, 0, 1, 1, 0), 'bf16', 'conv', 40, 40, 3, 1, 1, 1, 0, 1, 0, [(1, 133, 129)]),
+    # hrnet-w18 bf16 x16 fpn_convs.3: Cin 256 x Cout 256 k3 s2
+    (('bf16', 0, 'bf16', 64, 1, 0, 0, 0, 0, 0, 1, 0, 6, 0, 1, 0, 0, 0, 0, 0), 'bf16', 'conv', 256, 256, 3, 2, 1, 0, 0, 0, 0, [(6, 11, 113)]),
+    # hrnet-w18 bf16 x16 reduction_conv.3: Cin 144 x Cout 256 k1 s1
+    (('bf16', 0, 'f32', 256, 0, 0, 0, 0, 0, 0, 2, 0, 3, 0, 0, 0, 0, 0, 0, 0), 'bf16', 'conv', 144, 256, 1, 1, 0, 0, 1, 0, 0, [(1, 120, 127)]),
+    # hrnet-w18 bf16 x16 reduction_conv.1: Cin 40 x Cout 256 k1 s1 (the plan also runs Cin x Cout 72x256)
+    (('bf16', 0, 'f32', 256, 0, 0, 0, 0, 1, 0, 2, 0, 6, 0, 0, 0, 0, 1, 0, 0), 'bf16', 'conv', 40, 256, 1, 1, 0, 0, 1, 0, 0, [(1, 133, 129)]),
+    # hrnet-w18 bf16 x16 reduction_conv.0: Cin 24 x Cout 256 k1 s1
+    (('bf16', 0, 'f32', 256, 0, 0, 0, 0, 1, 0, 2, 0, 6, 0, 1, 0, 0, 1, 0, 0), 'bf16', 'conv', 24, 256, 1, 1, 1, 0, 1, 0, 0, [(1, 133, 129)]),
+    # hrnet-w18 f16x3 x4@960 reduction_conv.2: Cin 72 x Cout 256 k1 s1
+    (('f16x3', 0, 'f32', 128, 0, 0, 0, 0, 1, 0, 2, 0, 6, 0, 0, 0, 0, 1, 0, 0), 'f16x3', 'conv', 72, 256, 1, 1, 0, 0, 1, 0, 0, [(1, 83, 91)]),
+    # hrnet-w18 f16x3 x16 reduction_conv.3: Cin 144 x Cout 256 k1 s1 (the plan also runs Cin x Cout 256x256)
+    (('f16x3', 0, 'f32', 256, 0, 0, 0, 0, 0, 0, 2, 0, 3, 0, 0, 0, 0, 0, 0, 0), 'f16x3', 'conv', 144, 256, 1, 1, 0, 0, 1, 0, 0, [(1, 120, 127)]),
+    # hrnet-w18 f16x3 x16 reduction_conv.2: Cin 72 x Cout 256 k1 s1 (the plan also runs Cin x Cout 128x256)
+    (('f16x3', 0, 'f32', 256, 0, 0, 0, 0, 0, 0, 2, 0, 3, 0, 0, 0, 0, 1, 0, 0), 'f16x3', 'conv', 72, 256, 1, 1, 0, 0, 1, 0, 0, [(1, 133, 129)]),
+    # hrnet-w18 f16x3 x16/f16x3 x4@960 reduction_conv.1: Cin 40 x Cout 256 k1 s1 (the plan also runs Cin x Cout 64x256)
+    (('f16x3', 0, 'f32', 256, 0, 0, 0, 0, 1, 0, 2, 0, 6, 0, 0, 0, 0, 1, 0, 0), 'f16x3', 'conv', 40, 256, 1, 1, 0, 0, 1, 0, 0, [(1, 133, 129)]),
+    # hrnet-w18 f16x3 x16/f16x3 x4@960 reduction_conv.0: Cin 24 x Cout 256 k1 s1 (the plan also runs Cin x Cout 32x256)
+    (('f16x3', 0, 'f32', 256, 0, 0, 0, 0, 1, 0, 2, 0, 6, 0, 1, 0, 0, 1, 0, 0), 'f16x3', 'conv', 24, 256, 1, 1, 1, 0, 1, 0, 0, [(1, 133, 129)]),
+    # r50-dcn f16x3 x16 layer4.*.off: Cin 512 x Cout 18 k3 s1 (the plan also runs Cin x Cout 512x27)
+    (('f16x3', 0, 'f32', 32, 0, 0, 0, 0, 0, 0, 1, 0, 6, 0, 1, 0, 0, 0, 1, 0), 'f16x3', 'conv', 512, 18, 3, 1, 1, 0, 1, 0, 0, [(1, 2, 2)]),
+    # r50-dcn f16x3 x16 layer3.*.off: Cin 256 x Cout 18 k3 s1 (the plan also runs Cin x Cout 128x18, 128x27, 256x27)
+    (('f16x3', 0, 'f32', 32, 0, 0, 0, 0, 0, 0, 1, 0, 6, 0, 1, 0, 0, 1, 1, 0), 'f16x3', 'conv', 256, 18, 3, 1, 1, 0, 1, 0, 0, [(1, 133, 129)]),
+    # hrnet-w18 f16x3 x4@960 reduction_conv.3: Cin 144 x Cout 256 k1 s1
+    (('f16x3', 0, 'f32', 64, 0, 0, 0, 0, 1, 0, 2, 0, 6, 0, 0, 0, 0, 0, 0, 0), 'f16x3', 'conv', 144, 256, 1, 1, 0, 0, 1, 0, 0, [(1, 2, 2)]),
+    # hrnet-w32 f16x3 x16 stage3.*.branches.2.*.conv2, stage4.*.branches.2.*.conv2: Cin 128 x Cout 128 k3 s1 (the plan also runs Cin x Cout 64x128)
+    (('f16x3', 0, 'split', 128, 1, 0, 0, 1, 0, 1, 2, 0, 3, 1, 1, 0, 0, 1, 0, 0), 'f16x3', 'conv', 128, 128, 3, 1, 1, 1, 0, 1, 0, [(1, 133, 129)]),
+    # hrnet-w18 f16x3 x16 stage3.*.branches.2.*.conv2, stage4.*.branches.2.*.conv2: Cin 72 x Cout 72 k3 s1 (the plan also runs Cin x Cout 40x72)
+    (('f16x3', 0, 'split', 128, 1, 0, 0, 1, 0, 1, 2, 0, 3, 1, 1, 0, 0, 1, 1, 0), 'f16x3', 'conv', 72, 72, 3, 1, 1, 1, 0, 1, 0, [(1, 133, 129)]),
+    # hrnet-w18 f16x3 x4@960 fpn_convs.1: Cin 256 x Cout 256 k3 s2
+    (('f16x3', 0, 'split', 128, 1, 1, 0, 0, 0, 0, 1, 0, 2, 0, 1, 0, 0, 1, 0, 0), 'f16x3', 'conv', 256, 256, 3, 2, 1, 0, 0, 0, 0, [(6, 35, 139)]),
+    # hrnet-w18 f16x3 x16 stage3.*.branches.2.*.conv1, stage4.*.branches.2.*.conv1: Cin 72 x Cout 72 k3 s1
+    (('f16x3', 0, 'split', 128, 1, 1, 0, 0, 0, 0, 1, 0, 2, 1, 1, 0, 0, 1, 1, 0), 'f16x3', 'conv', 72, 72, 3, 1, 1, 1, 0, 0, 0, [(1, 133, 129)]),
+    # r50-ga f16x3 x4@960 fpn1; x101-64x4d f16x3 x4@960 fpn1: Cin 256 x Cout 256 k3 s1 (the plan also runs Cin x Cout 1024x256)
+    (('f16x3', 0, 'split', 128, 1, 1, 0, 0, 0, 0, 1, 1, 2, 0, 0, 0, 0, 1, 0, 0), 'f16x3', 'conv', 256, 256, 3, 1, 0, 0, 0, 0, 1, [(1, 83, 91)]),
+    # hrnet-w32 f16x3 x16 stage4.*.fuse_layers.2.3.0: Cin 256 x Cout 128 k1 s1
+    (('f16x3', 0, 'split', 128, 1, 1, 0, 0, 0, 1, 1, 0, 2, 0, 1, 0, 0, 0, 0, 0), 'f16x3', 'conv', 256, 128, 1, 1, 1, 0, 0, 0, 0, [(1, 120, 127)]),
+    # hrnet-w18 f16x3 x16 stage4.*.fuse_layers.2.3.0: Cin 144 x Cout 72 k1 s1
+    (('f16x3', 0, 'split', 128, 1, 1, 0, 0, 0, 1, 1, 0, 2, 0, 1, 0, 0, 0, 1, 0), 'f16x3', 'conv', 144, 72, 1, 1, 1, 0, 0, 0, 0, [(1, 120, 127)]),
+    # hrnet-w18 f16x3 x16 transition2.2.0: Cin 40 x Cout 72 k3 s2
+    (('f16x3', 0, 'split', 128, 1, 1, 0, 0, 0, 1, 1, 0, 2, 1, 1, 0, 0, 1, 1, 0), 'f16x3', 'conv', 40, 72, 3, 2, 1, 1, 0, 0, 0, [(5, 105, 129)]),
+    # hrnet-w18 f16x3 x16 fpn_convs.2; hrnet-w32 f16x3 x16 fpn_convs.2: Cin 256 x Cout 256 k3 s2
+    (('f16x3', 0, 'split', 256, 1, 0, 0, 0, 0, 0, 1, 0, 3, 0, 1, 0, 0, 0, 0, 0), 'f16x3', 'conv', 256, 256, 3, 2, 1, 0, 0, 0, 0, [(6, 81, 123)]),
+    # hrnet-w18 f16x3 x16 stage4.*.branches.3.*.conv1: Cin 144 x Cout 144 k3 s1 (the plan also runs Cin x Cout 72x144)
+    (('f16x3', 0, 'split', 256, 1, 0, 0, 0, 0, 0, 1, 0, 3, 1, 1, 0, 0, 0, 1, 0), 'f16x3', 'conv', 144, 144, 3, 1, 1, 1, 0, 0, 0, [(1, 120, 127)]),
+    # r50-ga f16x3 x16 layer4.*.att.kv: Cin 512 x Cout 1024 k1 s2
+    (('f16x3', 0, 'split', 256, 1, 0, 0, 0, 0, 1, 1, 0, 3, 0, 0, 0, 0, 0, 0, 0), 'f16x3', 'conv', 512, 1024, 1, 2, 0, 0, 0, 0, 0, [(6, 155, 15)]),
+    # r50-ga f16x3 x16 layer3.*.att.kv: Cin 256 x Cout 512 k1 s2
+    (('f16x3', 0, 'split', 256, 1, 0, 0, 0, 0, 1, 1, 0, 3, 0, 0, 0, 0, 1, 0, 0), 'f16x3', 'conv', 256, 512, 1, 2, 0, 0, 0, 0, 0, [(6, 35, 139)]),
+    # x101-64x4d f16x3 x16/f16x3 x4@960 layer1.*.c1; x50-32x8d f16x3 x16 layer1.*.c1: Cin 64 x Cout 256 k1 s1
+    (('f16x3', 0, 'split', 256, 1, 0, 0, 0, 1, 1, 2, 0, 3, 1, 1, 0, 0, 1, 0, 0), 'f16x3', 'conv', 64, 256, 1, 1, 1, 1, 0, 0, 0, [(1, 133, 129)]),
+    # hrnet-w32 f16x3 x16 stage4.*.fuse_layers.3.0.2: Cin 32 x Cout 256 k3 s2 (the plan also runs Cin x Cout 64x256)
+    (('f16x3', 0, 'split', 256, 1, 0, 0, 1, 0, 1, 1, 0, 3, 0, 1, 0, 0, 0, 0, 0), 'f16x3', 'conv', 32, 256, 3, 2, 1, 0, 0, 1, 0, [(6, 81, 123)]),
+    # hrnet-w18 f16x3 x16 stage4.*.fuse_layers.3.0.2: Cin 24 x Cout 144 k3 s2 (the plan also runs Cin x Cout 40x144)
+    (('f16x3', 0, 'split', 256, 1, 0, 0, 1, 0, 1, 1, 0, 3, 0, 1, 0, 0, 0, 1, 0), 'f16x3', 'conv', 24, 144, 3, 2, 1, 0, 0, 1, 0, [(6, 81, 123)]),
+    # hrnet-w18 f16x3 x16 stage4.*.branches.3.*.conv2: Cin 144 x Cout 144 k3 s1 (the plan also runs Cin x Cout 72x144)
+    (('f16x3', 0, 'split', 256, 1, 0, 0, 1, 0, 1, 1, 0, 3, 1, 1, 0, 0, 0, 1, 0), 'f16x3', 'conv', 144, 144, 3, 1, 1, 1, 0, 1, 0, [(1, 120, 127)]),
+    # hrnet-w18 f16x3 x4@960 stage4.*.fuse_layers.3.0.2: Cin 24 x Cout 144 k3 s2 (the plan also runs Cin x Cout 40x144)
+    (('f16x3', 0, 'split', 64, 1, 0, 0, 1, 0, 1, 2, 0, 4, 0, 1, 0, 0, 0, 1, 0), 'f16x3', 'conv', 24, 144, 3, 2, 1, 0, 0, 1, 0, [(1, 2, 2)]),
+    # hrnet-w32 f16x3 x16 stage3.*.fuse_layers.1.0.0, stage4.*.fuse_layers.1.0.0: Cin 32 x Cout 64 k3 s2 (the plan also runs Cin x Cout 512x512)
+    (('f16x3', 0, 'split', 64, 1, 0, 0, 1, 0, 1, 2, 0, 4, 0, 1, 0, 0, 1, 0, 0), 'f16x3', 'conv', 32, 64, 3, 2, 1, 0, 0, 1, 0, [(5, 105, 129)]),
+    # hrnet-w18 f16x3 x16/f16x3 x4@960 stage3.*.fuse_layers.1.0.0, stage4.*.fuse_layers.1.0.0: Cin 24 x Cout 40 k3 s2 (the plan also runs Cin x Cout 24x72, 40x72)
+    (('f16x3', 0, 'split', 64, 1, 0, 0, 1, 0, 1, 2, 0, 4, 0, 1, 0, 0, 1, 1, 0), 'f16x3', 'conv', 24, 40, 3, 2, 1, 0, 0, 1, 0, [(5, 105, 129)]),
+    # hrnet-w18 f16x3 x4@960 stage4.*.branches.3.*.conv2: Cin 144 x Cout 144 k3 s1 (the plan also runs Cin x Cout 72x144)
+    (('f16x3', 0, 'split', 64, 1, 0, 0, 1, 0, 1, 2, 0, 4, 1, 1, 0, 0, 0, 1, 0), 'f16x3', 'conv', 144, 144, 3, 1, 1, 1, 0, 1, 0, [(1, 2, 2)]),
+    # hrnet-w32 f16x3 x16 stage2.*.fuse_layers.1.0.0: Cin 32 x Cout 64 k3 s2 (the plan also runs Cin x Cout 64x64)
+    (('f16x3', 0, 'split', 64, 1, 0, 0, 1, 0, 1, 2, 0, 4, 1, 1, 0, 0, 1, 0, 0), 'f16x3', 'conv', 32, 64, 3, 2, 1, 1, 0, 1, 0, [(5, 105, 129)]),
+    # hrnet-w18 f16x3 x16/f16x3 x4@960 stage2.*.branches.0.*.conv2, stage3.*.branches.0.*.conv2, stage4.*.branches.0.*.conv2: Cin 24 x Cout 24 k3 s1 (the plan also runs Cin x Cout 24x40, 32x32, 40x40, 40x72, 72x72)
+    (('f16x3', 0, 'split', 64, 1, 0, 0, 1, 0, 1, 2, 0, 4, 1, 1, 0, 0, 1, 1, 0), 'f16x3', 'conv', 24, 24, 3, 1, 1, 1, 0, 1, 0, [(1, 133, 129)]),
+    # hrnet-w18 f16x3 x4@960 fpn_convs.2; hrnet-w18 f16x3 x16 fpn_convs.3; hrnet-w32 f16x3 x16 fpn_convs.3: Cin 256 x Cout 256 k3 s2
+    (('f16x3', 0, 'split', 64, 1, 1, 0, 0, 0, 0, 1, 0, 3, 0, 1, 0, 0, 0, 0, 0), 'f16x3', 'conv', 256, 256, 3, 2, 1, 0, 0, 0, 0, [(6, 11, 113)]),
+    # hrnet-w18 f16x3 x4@960 stage4.*.branches.3.*.conv1: Cin 144 x Cout 144 k3 s1 (the plan also runs Cin x Cout 72x144)
+    (('f16x3', 0, 'split', 64, 1, 1, 0, 0, 0, 0, 1, 0, 3, 1, 1, 0, 0, 0, 1, 0), 'f16x3', 'conv', 144, 144, 3, 1, 1, 1, 0, 0, 0, [(1, 30, 94)]),
+    # hrnet-w18 f16x3 x4@960 stage3.*.branches.2.*.conv1, stage4.*.branches.2.*.conv1: Cin 72 x Cout 72 k3 s1 (the plan also runs Cin x Cout 256x24, 256x32, 256x40)
+    (('f16x3', 0, 'split', 64, 1, 1, 0, 0, 0, 0, 1, 0, 3, 1, 1, 0, 0, 1, 1, 0), 'f16x3', 'conv', 72, 72, 3, 1, 1, 1, 0, 0, 0, [(5, 13, 65)]),
+    # r50-ga f16x3 x4@960 layer4.*.att.kv: Cin 512 x Cout 1024 k1 s2
+    (('f16x3', 0, 'split', 64, 1, 1, 0, 0, 0, 1, 1, 0, 3, 0, 0, 0, 0, 0, 0, 0), 'f16x3', 'conv', 512, 1024, 1, 2, 0, 0, 0, 0, 0, [(1, 2, 2)]),
+    # r50-ga f16x3 x4@960 layer3.*.att.kv: Cin 256 x Cout 512 k1 s2
+    (('f16x3', 0, 'split', 64, 1, 1, 0, 0, 0, 1, 1, 0, 3, 0, 0, 0, 0, 1, 0, 0), 'f16x3', 'conv', 256, 512, 1, 2, 0, 0, 0, 0, 0, [(5, 17, 33)]),
+    # hrnet-w32 f16x3 x16 stage4.*.fuse_layers.1.3.0: Cin 256 x Cout 64 k1 s1
+    (('f16x3', 0, 'split', 64, 1, 1, 0, 0, 0, 1, 1, 0, 3, 0, 1, 0, 0, 0, 0, 0), 'f16x3', 'conv', 256, 64, 1, 1, 1, 0, 0, 0, 0, [(1, 2, 2)]),
+    # hrnet-w32 f16x3 x16 stage4.*.fuse_layers.0.3.0: Cin 256 x Cout 32 k1 s1
+    (('f16x3', 0, 'split', 64, 1, 1, 0, 0, 0, 1, 1, 0, 3, 0, 1, 0, 0, 0, 1, 0), 'f16x3', 'conv', 256, 32, 1, 1, 1, 0, 0, 0, 0, [(1, 2, 2)]),
+    # hrnet-w18 f16x3 x4@960 stage4.*.fuse_layers.3.0.1: Cin 24 x Cout 24 k3 s2 (the plan also runs Cin x Cout 40x40)
+    (('f16x3', 0, 'split', 64, 1, 1, 0, 0, 0, 1, 1, 0, 3, 1, 1, 0, 0, 0, 1, 0), 'f16x3', 'conv', 24, 24, 3, 2, 1, 1, 0, 0, 0, [(5, 43, 153)]),
+    # hrnet-w18 f16x3 x16/f16x3 x4@960 stage2.*.branches.0.*.conv1, stage3.*.branches.0.*.conv1, stage4.*.branches.0.*.conv1: Cin 24 x Cout 24 k3 s1 (the plan also runs Cin x Cout 32x32, 40x40, 40x72)
+    (('f16x3', 0, 'split', 64, 1, 1, 0, 0, 0, 1, 1, 0, 3, 1, 1, 0, 0, 1, 1, 0), 'f16x3', 'conv', 24, 24, 3, 1, 1, 1, 0, 0, 0, [(1, 133, 129)]),
+    # hrnet-w18 f16x3 x4@960 stage3.*.fuse_layers.0.2.0, stage4.*.fuse_layers.0.2.0: Cin 72 x Cout 24 k1 s1 (the plan also runs Cin x Cout 72x40, 144x24, 144x40, 144x72)
+    (('f16x3', 0, 'split', 64, 1, 1, 0, 0, 1, 1, 1, 0, 3, 0, 1, 0, 0, 0, 1, 0), 'f16x3', 'conv', 72, 24, 1, 1, 1, 0, 0, 0, 0, [(1, 2, 2)]),
+    # hrnet-w18 f16x3 x16/f16x3 x4@960 stage2.*.fuse_layers.0.1.0, stage3.*.fuse_layers.0.1.0, stage4.*.fuse_layers.0.1.0: Cin 40 x Cout 24 k1 s1 (the plan also runs Cin x Cout 64x32)
+    (('f16x3', 0, 'split', 64, 1, 1, 0, 0, 1, 1, 2, 0, 3, 0, 1, 0, 0, 1, 1, 0), 'f16x3', 'conv', 40, 24, 1, 1, 1, 0, 0, 0, 0, [(1, 133, 129)]),
+    # r50-dcn f16x3 x16 layer3.*.c2; r50-dcnv2 f16x3 x16 layer3.*.c2: Cin 256 x Cout 256 k3 s1 (the plan also runs Cin x Cout 128x128, 512x512)
+    (('f16x3', 1, 'split', 128, 1, 0, 1, 0, 0, 0, 1, 0, 2, 1, 1, 0, 0, 1, 0, 0), 'f16x3', 'deform', 256, 256, 3, 1, 1, 1, 0, 0, 0, [(4, 33, 65)]),
 ]
 
 
@@ -231,7 +362,12 @@ def planned(c, sms=132):
     split = prec == "f16x3"
     if kind == "stem":                                     # one launch per image batch: the last one's plan
         return _lib.tc_plan_for(probs[-1:], 64, 64, 4, 1, 64, 1, 0, bias=True, relu=1, split=split, stem=2, sms=sms)
-    cout_p = EngineTCSplit._pad_cout(cout) if split else (cout + 31) // 32 * 32
+    if not split:
+        cout_p = (cout + 31) // 32 * 32
+    elif kind == "conv" and not out_f32 and cout <= 32:
+        cout_p = 64                                        # EngineTCSplit._tc(out16=True): one 64-column TMA store tile
+    else:
+        cout_p = EngineTCSplit._pad_cout(cout)
     if kind == "deform":
         return _lib.tc_plan_for(probs, cout, cout_p, 3, 3, cin, 1, 1, bias=bias, relu=act, deform=True, split=split, sms=sms)
     pad = k // 2

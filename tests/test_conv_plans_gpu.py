@@ -162,7 +162,7 @@ class Case:
                     _lib.check(e.lib.orp_stem_conv_s2d_bf16(_lib.ptr(xs), n, h, w, _lib.ptr(ws), _lib.ptr(self.L.bias), 1,
                                                             _lib.ptr(y), st), "orp_stem_conv_s2d_bf16")
             return _lib.tc_last_plan()
-        tc = e._tc(self.L)
+        tc = e._tc(self.L, out16=self.kind == "conv" and not self.out_f32)     # the weights conv_multi packs for this layer
         if self.stats is not None:
             for t in self.stats:
                 t.zero_()
@@ -291,10 +291,11 @@ def test_conv_plan_vs_fp64(cuda, engines, c):
 
 
 DCN_CASES = [c for c in PARITY if c[2] == "deform"]
+DCN_IDS = [case_id(c) if c[7] else c[1] for c in DCN_CASES]    # the head's DCN (no bias) by its format, the backbone's by its case
 
 
 @pytest.mark.parametrize("mode", ["zero", "edges", "mask_binary", "mask_random", "edges_mask_random"])
-@pytest.mark.parametrize("c", DCN_CASES, ids=[c[1] for c in DCN_CASES])
+@pytest.mark.parametrize("c", DCN_CASES, ids=DCN_IDS)
 def test_deform_edges(cuda, engines, c, mode):
     offsets = "zero" if mode == "zero" else ("edges" if mode.startswith("edges") else "random")
     masks = "binary" if mode == "mask_binary" else ("random" if "mask_random" in mode else None)
@@ -307,7 +308,8 @@ def test_deform_edges(cuda, engines, c, mode):
         for i, ref in enumerate(case.refs):
             x = case.eng.to_float(case.xs[i]) if case.split else case.xs[i].float()
             plain = torch.relu(F.conv2d(_nchw(x).double(), case.L.w_raw.permute(0, 3, 1, 2).to(cuda).double()
-                                        if case.split else case.L.w_raw.permute(0, 3, 1, 2).to(cuda).bfloat16().double(), None, 1, 1))
+                                        if case.split else case.L.w_raw.permute(0, 3, 1, 2).to(cuda).bfloat16().double(),
+                                        None if case.L.bias is None else case.L.bias.double(), 1, 1))
             assert _rel(ref, plain) < 1e-6                      # the fp64 references agree (x rounded as the engine holds it)
     err = _check_values(case, plan)
     print("%s %s: %d tiles on %d CTAs, %d stages, rel err %.2e" % (c[1], mode, plan["num_tiles"], plan["grid"], plan["stages"], err))

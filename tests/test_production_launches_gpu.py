@@ -12,15 +12,17 @@ where they happen.
   config's test pipeline to 960^2, with the valid extents), the input the bench's own seeded uint8 tiles.  The weights are
   random_state_dict(reference_init=False) (randomised norm scales, so that no conv3 launch is trivially zero) and the Swin-T
   state dict of the bench; the launch plans must be those of the bench's detector, launch for launch.  The engine's
-  conv_multi, deform_conv_multi and _stem_conv_s2d are wrapped; after each real call the output is compared with an fp64
+  conv_multi, deform_conv_multi, _stem_conv_s2d and group_conv are wrapped; after each real call the output is compared with an fp64
   reference built from the exact operands (the input as the engine holds it, raw fp32 weights in f16x3 or bf16-rounded
   ones in bf16, bias, the 16-bit or fp32 residual, the activation, the production DCN offsets through deform_conv_ref, the
-  stem's image decoded from its space-to-depth operand), image by image relative to that image's max, with the tolerances
+  stem's image decoded from its space-to-depth operand and convolved at the stem layer's stride and padding: ResNet's 7x7 or
+  HRNet's 3x3 conv1), image by image relative to that image's max, with the tolerances
   of test_conv_plans_gpu.py; GroupNorm sums against fp64 sums.  The references are computed one image at a time on the
   device, so that the fp64 im2col of a 16 x 128^2 deformable convolution is never resident at once.  Then the call is
   launched twice more into guarded outputs prefilled with two NaN patterns: both results bitwise equal to the first output,
-  guards untouched.  Counters on _launch, _conv_splitk and the stem entry point make sure that no launch escapes the
-  checker.
+  guards untouched.  Counters on _launch, _conv_splitk and the stem and grouped entry points make sure that no launch
+  escapes the checker.  tests/test_backbone_launches_gpu.py runs the same checker on the ResNeXt, HRNet, DCN-stage and
+  GeneralizedAttention graphs.
 - test_benchmarked_step_r50_x16: the headline configuration exactly as bench_tile.run builds it, with the reference's
   initialisation and with randomised norm scales.  Graph replays equal the eager pass (1e-5) and each other; every tile
   of the 16-tile replay is within north_star's 1e-4 of the fp64 graph run on that tile alone (normalised in fp64 on the
@@ -31,6 +33,7 @@ where they happen.
   in the NMS, so that content match is not made there.)
 - test_benchmarked_step_other_workloads: R-101 f16x3 x4 and Swin-T f16x3 x8 as bench_tile.run_config builds them, every
   tile of the replay against the fp64 graph."""
+import ctypes
 import time
 
 import pytest
@@ -47,6 +50,7 @@ pytestmark = pytest.mark.gpu
 
 DENSE_TOL = 1e-4                                  # north_star: dense outputs within 1e-4 of the fp64 reference graph
 REPLAY_TOL = 1e-5                                 # graph replay against eager: GroupNorm sums are atomics, bits may differ
+GROUP_BF16_TOL = 1.5e-2                           # bf16 grouped conv2: the launch tolerance of tests/test_resnext_gpu.py
 TEST_SCALE = [("r101", "f16x3", 4), ("swin_tiny", "f16x3", 8)]     # bench_tile.run_test_scale
 
 
@@ -60,9 +64,38 @@ def _act(v, act):
     return torch.relu(v) if act is True or act == 1 else (F.gelu(v) if act == 2 else v)
 
 
+def _hrnet_names(hr, names):
+    """HRNetGraph's layers by the reference's module paths (hrnet.py), HRFPN's reduction slices and fpn_convs"""
+    names[id(hr.conv2)] = "conv2"
+    for b, blk in enumerate(hr.layer1):
+        for k, L in enumerate(blk["convs"]):
+            names[id(L)] = "layer1.%d.conv%d" % (b, k + 1)
+        if blk["ds"] is not None:
+            names[id(blk["ds"])] = "layer1.%d.downsample" % b
+    for s, (trans, mods) in enumerate(zip(hr.transitions, hr.stages), 1):
+        for i, chain in enumerate(trans):
+            for j, L in enumerate(chain or ()):
+                names[id(L)] = "transition%d.%d.%d" % (s, i, j)
+        for m, (branches, fuse) in enumerate(mods):
+            p = "stage%d.%d." % (s + 1, m)
+            for br, blocks in enumerate(branches):
+                for k, (c1, c2) in enumerate(blocks):
+                    names[id(c1)], names[id(c2)] = p + "branches.%d.%d.conv1" % (br, k), p + "branches.%d.%d.conv2" % (br, k)
+            for i, row in enumerate(fuse):
+                for j, path in enumerate(row):
+                    for k, L in enumerate(path or ()):
+                        names[id(L)] = p + "fuse_layers.%d.%d.%d" % (i, j, k)
+    for i, L in enumerate(hr.reduce):
+        names[id(L)] = "reduction_conv.%d" % i
+    for i, L in enumerate(hr.fpn):
+        names[id(L)] = "fpn_convs.%d" % i
+
+
 def _layer_names(det):
+    """id(ConvLayer) -> the layer's name, for every convolution of the detector: ResNet / ResNeXt (with deformable conv2 and
+    their conv_offset, and GeneralizedAttention blocks), Swin, HRNet + HRFPN, the FPN and the head"""
     names = {}
-    if det.depth == "swin_tiny":
+    if getattr(det, "swin", None) is not None:
         sw = det.swin
         names[id(sw.embed)] = "patch_embed"
         for i, stage in enumerate(sw.blocks):
@@ -73,14 +106,20 @@ def _layer_names(det):
             names[id(m["red"])] = "merge%d" % i
     else:
         names[id(det.stem)] = "stem"
-        for li, stage in enumerate(det.blocks):
-            for b, blk in enumerate(stage):
-                for k, L in blk.items():
-                    if L is not None:
-                        names[id(L)] = "layer%d.%d.%s" % (li + 1, b, k)
-    for i, (L, _) in enumerate(det.lat):
+    if getattr(det, "hrnet", None) is not None:
+        _hrnet_names(det.hrnet, names)
+    for li, stage in enumerate(getattr(det, "blocks", ())):
+        for b, blk in enumerate(stage):
+            for k in ("c1", "c2", "c3", "ds", "off"):
+                if blk.get(k) is not None:
+                    names[id(blk[k])] = "layer%d.%d.%s" % (li + 1, b, k)
+            att = blk.get("att")
+            for k in ("q", "kv", "proj"):
+                if att is not None and getattr(att, k) is not None:
+                    names[id(getattr(att, k))] = "layer%d.%d.att.%s" % (li + 1, b, k)
+    for i, (L, _) in enumerate(getattr(det, "lat", ())):
         names[id(L)] = "lateral%d" % i
-    for i, (L, _) in enumerate(det.fpn):
+    for i, (L, _) in enumerate(getattr(det, "fpn", ())):
         names[id(L)] = "fpn%d" % i
     for i, ((lc, _), (lr, _)) in enumerate(zip(det.cls_convs, det.reg_convs)):
         names[id(lc)], names[id(lr)] = "cls_convs%d" % i, "reg_convs%d" % i
@@ -104,6 +143,7 @@ def _where(y, ref, tol):
 class LaunchChecker:
     """wraps the tensor-core convolution methods of one detector's engine; every call is checked against fp64 and for
     write-once stores as it happens (see the module docstring)"""
+    conv_margin = 1.0                         # factor on the f16x3 convolution tolerance OP_TOL * max(1, K / 4096)
 
     def __init__(self, det, name):
         self.det, self.eng, self.name = det, det.eng, name
@@ -115,12 +155,14 @@ class LaunchChecker:
         self.low = 0                          # low-level launches of the forward pass
         self.escaped = []                     # ... made outside a checked call
         self.checked = 0
-        self.sigs = []                        # plan signature of every checked launch, in order
+        self.sigs = []                        # plan signature of every checked orp_conv2d / stem launch, in order
+        self.layers = []                      # ... and the name of its layer
         self.worst = {}                       # kind -> (rel err, tol, where)
         e = self.eng
-        self.orig = {m: getattr(e, m) for m in ("conv_multi", "deform_conv_multi", "_stem_conv_s2d", "_launch", "_conv_splitk",
-                                                "_call")}
+        self.orig = {m: getattr(e, m) for m in ("conv_multi", "deform_conv_multi", "_stem_conv_s2d", "group_conv", "_launch",
+                                                "_conv_splitk", "_call")}
         e.conv_multi, e.deform_conv_multi, e._stem_conv_s2d = self._conv_multi, self._deform_conv_multi, self._stem_conv_s2d
+        e.group_conv = self._group_conv
         e._launch, e._conv_splitk, e._call = self._counted("_launch"), self._counted("_conv_splitk"), self._call
 
     # ----------------------------------------------------------------------------------------------- counters
@@ -142,8 +184,8 @@ class LaunchChecker:
         return wrapper
 
     def _call(self, name, *args):
-        if name == "orp_stem_conv_s2d_%s":
-            self._saw("stem", (name,) + args, {})
+        if name in ("orp_stem_conv_s2d_%s", "orp_group_conv2d_%s"):
+            self._saw("stem" if name == "orp_stem_conv_s2d_%s" else "group", (name,) + args, {})
         return self.orig["_call"](name, *args)
 
     def _run(self, method, *a):
@@ -174,7 +216,7 @@ class LaunchChecker:
                 r = r + _nchw64(residual_f32[i][j:j + 1])
             return _act(r, relu)
         if self.split:
-            tol = OP_TOL * max(1.0, K / 4096.0)
+            tol = OP_TOL * max(1.0, K / 4096.0) * self.conv_margin
         else:
             tol = BF16_F32_TOL if out_f32 else BF16_TOL
         kind = "split-K" if low[0] == "_conv_splitk" else ("fp32-out" if out_f32 else "conv")
@@ -198,9 +240,20 @@ class LaunchChecker:
         y, plan, low = self._run("_stem_conv_s2d", xs, L, n, h, w)
         wd, bias = self._weights(L), L.bias.double()
 
-        def ref(i, j):
-            return torch.relu(F.conv2d(self._s2d_image(xs, n, h, w, j), wd, bias, 2, 3))
+        def ref(i, j):                        # ResNet's 7x7 / s2 / pad 3 conv1, or HRNet's 3x3 / s2 / pad 1
+            return torch.relu(F.conv2d(self._s2d_image(xs, n, h, w, j), wd, bias, L.stride, L.pad))
         self._check("stem", L, [y], ref, OP_TOL if self.split else BF16_TOL, plan, low)
+        return y
+
+    def _group_conv(self, x, L, groups, relu=False):
+        """ResNeXt's grouped conv2: its own walk over the groups (not an orp_conv2d plan, so no signature is recorded)"""
+        y, plan, low = self._run("group_conv", x, L, groups, relu)
+        wd, bias = self._weights(L), L.bias.double()
+
+        def ref(i, j):
+            return _act(F.conv2d(self._held(x[j:j + 1]), wd, bias, L.stride, 1, groups=groups), relu)
+        K = 9 * L.w_raw.shape[3]
+        self._check("grouped", L, [y], ref, OP_TOL * max(1.0, K / 4096.0) if self.split else GROUP_BF16_TOL, plan, low)
         return y
 
     # --------------------------------------------------------------------------------------------- operands
@@ -233,7 +286,9 @@ class LaunchChecker:
         k = self.checked
         what = "%s launch %d %s (%s, BN %d, %d tiles on %d CTAs)" % (self.name, k, self.names.get(id(L), "?"), kind, plan["BN"],
                                                                   plan["num_tiles"], plan["grid"])
-        self.sigs.append(signature(plan))
+        if kind != "grouped":
+            self.sigs.append(signature(plan))
+            self.layers.append(self.names.get(id(L), "?"))
         self._values(kind, what, ys, ref, tol, stats, K, out_f32, plan)
         if self.split:
             assert self.eng.overflow_count() == 0, "%s: f16 overflow" % what
@@ -292,6 +347,12 @@ class LaunchChecker:
             elif kind == "_conv_splitk":
                 (g,) = outs
                 self.orig["_conv_splitk"](a[0], g.t, *a[2:6], fresh(a[6]), *a[7:])
+            elif kind == "group":                                 # the same problem, its output the guarded buffer
+                (g,) = outs
+                q = _lib.TcProblem()
+                ctypes.pointer(q)[0] = a[1]._obj
+                q.out = g.t.data_ptr()
+                self.orig["_call"](a[0], ctypes.byref(q), *a[2:])
             else:
                 (g,) = outs
                 self.orig["_call"](*a[:-2], _lib.ptr(g.t), a[-1])
