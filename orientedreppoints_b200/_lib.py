@@ -1,5 +1,5 @@
 """ctypes binding of liborp_b200.so (include/orp_b200.h, orp_b200_dcnv2.h, orp_b200_swin.h, orp_b200_group.h,
-orp_b200_hrnet.h, orp_b200_attention.h).
+orp_b200_hrnet.h, orp_b200_attention.h, orp_b200_context.h).
 
 There is NO fallback: if the shared library is missing or a call fails, an exception is raised.
 The library is built in-tree by `python -m orientedreppoints_b200.build` (nvcc, sm_90a).
@@ -203,6 +203,31 @@ ATTENTION_SIGNATURES = {
     "orp_gen_attention_bcast_add_f32": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp]),
 }
 
+
+class ContextPlan(ctypes.Structure):
+    _fields_ = [(k, _i) for k in ("threads", "slots", "warps_per_slot", "chunks", "pixels_per_chunk", "grid_x", "grid_y")] + \
+              [("workspace_bytes", ctypes.c_longlong)]
+
+    def as_dict(self):
+        return {k: int(getattr(self, k)) for k, _ in self._fields_}
+
+
+class ContextMlp(ctypes.Structure):
+    _fields_ = [(k, _vp) for k in ("w1", "b1", "ln_w", "ln_b", "w2", "b2")]
+
+
+# name -> (restype, argtypes); every symbol include/orp_b200_context.h declares
+CONTEXT_SIGNATURES = {
+    "orp_context_make_plan": (_i, [_i, _i, _i, _i, _i, ctypes.POINTER(ContextPlan)]),
+    "orp_context_pool_bf16": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, ctypes.c_size_t, _vp]),
+    "orp_context_pool_f16x3": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, ctypes.c_size_t, _vp]),
+    "orp_context_pool_f32": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, ctypes.c_size_t, _vp]),
+    "orp_context_transform": (_i, [_vp, _i, _i, _i, _i, ctypes.POINTER(ContextMlp), ctypes.POINTER(ContextMlp), _vp, _vp, _vp]),
+    "orp_context_fuse_bf16": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
+    "orp_context_fuse_f16x3": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
+    "orp_context_fuse_f32": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
+}
+
 _LIB = None
 
 
@@ -220,7 +245,8 @@ def lib():
                 "(there is no CPU or PyTorch fallback for this path)" % LIB_PATH)
         l = ctypes.CDLL(LIB_PATH)
         for name, (res, args) in list(SIGNATURES.items()) + list(DCNV2_SIGNATURES.items()) + list(SWIN_SIGNATURES.items()) + \
-                list(GROUP_SIGNATURES.items()) + list(HRNET_SIGNATURES.items()) + list(ATTENTION_SIGNATURES.items()):
+                list(GROUP_SIGNATURES.items()) + list(HRNET_SIGNATURES.items()) + list(ATTENTION_SIGNATURES.items()) + \
+                list(CONTEXT_SIGNATURES.items()):
             fn = getattr(l, name)   # AttributeError if the symbol is not exported
             fn.restype = res
             fn.argtypes = args
@@ -335,6 +361,17 @@ def gen_attention_plan_for(fmt, N, H, W, C, heads, kv_stride, *, content=True, p
     a.ld_kv = 2 * C if ld_kv is None else ld_kv
     p = GenAttentionPlan()
     check(lib().orp_gen_attention_make_plan(ctypes.byref(a), GEN_ATTENTION_FORMATS[fmt], ctypes.byref(p)), "orp_gen_attention_make_plan")
+    return p.as_dict()
+
+
+CONTEXT_FORMATS = {"bf16": 0, "f16x3": 1, "fp32": 2}
+
+
+def context_plan_for(fmt, N, H, W, C):
+    """the plan orp_context_make_plan reports for the pool launch of format fmt ('bf16' / 'f16x3' / 'fp32') on x [N, H, W, C]
+    (no device needed)"""
+    p = ContextPlan()
+    check(lib().orp_context_make_plan(N, H, W, C, CONTEXT_FORMATS[fmt], ctypes.byref(p)), "orp_context_make_plan")
     return p.as_dict()
 
 

@@ -32,6 +32,7 @@ def _headers():
     hs.append(os.path.join(HERE, "..", "include", "orp_b200_group.h"))
     hs.append(os.path.join(HERE, "..", "include", "orp_b200_hrnet.h"))
     hs.append(os.path.join(HERE, "..", "include", "orp_b200_attention.h"))
+    hs.append(os.path.join(HERE, "..", "include", "orp_b200_context.h"))
     return hs
 
 

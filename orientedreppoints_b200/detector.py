@@ -152,12 +152,16 @@ class OrientedRepPointsDetector:
     inference only."""
 
     def __init__(self, state_dict, depth=50, device="cuda", precision="fp32", test_cfg=None, dcn=None, pooling_type='AVG',
-                 gen_attention=None):
+                 gen_attention=None, gcb=None):
         """depth: 50 / 101 / 152 (ResNet or ResNeXt: the groups of every conv2 come from the state dict's shapes), or a Swin backbone - "swin_tiny" (Swin-T, window 7), any key of swin.ARCHS
         ("swin_small", "swin_base_w12", ...) or a swin.SwinArch, or an HRNet backbone with the HRFPN neck (stride 2, five
         outputs) - a key of hrnet.ARCHS ("hrnetv2p_w18", ...) or an hrnet.HRNetArch.
         dcn: the ResNet's deformable conv2 layers per stage and block, None / 'DCN' / 'DCNv2' (models.ResNet.dcn_layout,
         weights.dcn_layout); None: every conv2 is a plain convolution.
+        gen_attention: the ResNet's attention blocks per stage and block, None or a weights.gen_attention_spec
+        (models.ResNet.gen_attention_layout, weights.gen_attention_layout).
+        gcb: the ResNet's / ResNeXt's context blocks per stage and block, None or a weights.gcb_spec (models.ResNet.gcb_layout,
+        weights.gcb_layout); each runs on bn3(conv3(.)) before the residual add (context_block.py).
         pooling_type: HRFPN's pooling, 'AVG' or 'MAX' (HRNet only)"""
         from . import hrnet
         from .swin import arch_of
@@ -172,6 +176,7 @@ class OrientedRepPointsDetector:
         self.pooling_type = pooling_type
         self.dcn = dcn
         self.gen_attention = gen_attention
+        self.gcb = gcb
         self.test_cfg = dict(nms_pre=2000, min_bbox_size=0, score_thr=0.05, nms=dict(type='rnms', iou_thr=0.4),
                              max_per_img=2000)                         # configs/dota/orientedrepoints_r50_demo.py:62-67
         if test_cfg:
@@ -200,6 +205,9 @@ class OrientedRepPointsDetector:
         d = self.device
         if self.gen_attention is not None and (self.swin_arch is not None or self.hr_arch is not None):
             raise ValueError("gen_attention describes the attention blocks of a ResNet backbone; %s has none"
+                             % ("the Swin backbone" if self.swin_arch is not None else "the HRNet backbone"))
+        if self.gcb is not None and (self.swin_arch is not None or self.hr_arch is not None):
+            raise ValueError("gcb describes the context blocks of a ResNet / ResNeXt backbone; %s has none"
                              % ("the Swin backbone" if self.swin_arch is not None else "the HRNet backbone"))
         if self.swin_arch is not None:
             if self.dcn is not None:
@@ -233,6 +241,10 @@ class OrientedRepPointsDetector:
         if self.groups > 1 and any(sp is not None for s in ga for sp in s):
             raise NotImplementedError("gen_attention on a ResNeXt: the reference's ResNeXt builds no attention blocks "
                                       "(resnext.py:196-216)")
+        gcb = self.gcb if self.gcb is not None else tuple((None,) * n for n in STAGE_BLOCKS[self.depth])
+        if tuple(len(s) for s in gcb) != STAGE_BLOCKS[self.depth] or \
+                any(sp is not None and not isinstance(sp, dict) for s in gcb for sp in s):
+            raise ValueError("gcb must give None or a gcb_spec for each of the %s blocks of R-%d" % (STAGE_BLOCKS[self.depth], self.depth))
         self.stem = folded("backbone.conv1", "backbone.bn1", 2, 3, pad_cin_to=4)
         self.blocks = []
         for li, nblk in enumerate(STAGE_BLOCKS[self.depth]):
@@ -246,6 +258,7 @@ class OrientedRepPointsDetector:
                 blk["dcn"] = layout[li][b]
                 blk["off"] = self._offset_conv(sd, p + ".conv2", blk["dcn"], 64 << li, s)
                 blk["att"] = self._gen_attention_block(sd, p, ga[li][b], 64 << li)
+                blk["gcb"] = self._context_block(sd, p, gcb[li][b], 256 << li)
                 stage.append(blk)
             self.blocks.append(stage)
         self.lat = [(ConvLayer(sd["neck.lateral_convs.%d.conv.weight" % i].float(), None, 1, 0, d),
@@ -316,6 +329,18 @@ class OrientedRepPointsDetector:
             raise ValueError("%s: the gen_attention spec is for %r channels where the block's conv2 has %d"
                              % (prefix, spec.get('channels'), planes))
         return GenAttentionBlock(sd, prefix, spec, self.device)
+
+    def _context_block(self, sd, prefix, spec, channels):
+        """the engine form of a block's context_block (context_block.ContextBlock), None without one; ValueError when the state
+        dict contradicts the layout"""
+        from .context_block import ContextBlock, check_block
+        if spec is None:
+            check_block(sd, prefix, None)
+            return None
+        if spec.get('channels') != channels:
+            raise ValueError("%s: the gcb spec is for %r channels where the block's conv3 has %d"
+                             % (prefix, spec.get('channels'), channels))
+        return ContextBlock(sd, prefix, spec, self.device)
 
     def _conv2(self, x, blk):
         """a block's 3x3 convolution + folded bn2 + ReLU.  Deformable (DCN / DCNv2): the offset convolution writes fp32 NHWC
@@ -437,7 +462,10 @@ class OrientedRepPointsDetector:
                 o = self._conv2(o, blk)
                 if blk["att"] is not None:                              # resnet.py:216-217, between relu(bn2) and conv3
                     o = blk["att"](e, o)
-                x = e.conv(o, blk["c3"], relu=True, residual=idt)
+                if blk["gcb"] is None:
+                    x = e.conv(o, blk["c3"], relu=True, residual=idt)
+                else:                                                   # resnet.py:219-230: on bn3(conv3(.)), then + identity, ReLU
+                    x = blk["gcb"](e, e.conv(o, blk["c3"]), idt)
             feats.append(x)
         c3, c4, c5 = feats[1], feats[2], feats[3]
         l2 = e.conv_gn(c5, *self.lat[2])

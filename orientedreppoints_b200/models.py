@@ -16,7 +16,7 @@ from .ops.conv_module import ConvModule
 from .ops.dcn import DeformConv, DeformConvPack, ModulatedDeformConvPack
 from .ops.norm import build_norm_layer
 from .utils.registry import Registry, build_from_cfg
-from .weights import STAGE_BLOCKS, block_width, check_groups, gen_attention_spec
+from .weights import STAGE_BLOCKS, block_width, check_groups, gcb_spec, gen_attention_spec
 
 BACKBONES = Registry('backbone')
 NECKS = Registry('neck')
@@ -82,6 +82,21 @@ class GeneralizedAttention(_EngineOnly):
         self.gamma = nn.Parameter(torch.zeros(1))
 
 
+class ContextBlock(_EngineOnly):
+    """the parameter tree of context_block.py:13-52 for a spec of weights.gcb_spec: conv_mask for 'att' pooling, and a
+    channel_{add,mul}_conv (1x1 C -> P, LayerNorm([P, 1, 1]), ReLU, 1x1 P -> C) for each fusion used"""
+
+    def __init__(self, inplanes, spec):
+        super().__init__()
+        c, p = inplanes, spec['planes']
+        self.spec = spec
+        if spec['pooling_type'] == 'att':
+            self.conv_mask = nn.Conv2d(c, 1, 1)
+        for f in spec['fusion_types']:
+            setattr(self, f + '_conv', nn.Sequential(nn.Conv2d(c, p, 1), nn.LayerNorm([p, 1, 1]), nn.ReLU(inplace=True),
+                                                     nn.Conv2d(p, c, 1)))
+
+
 class Bottleneck(_EngineOnly):
     """resnet.py:84-239 (style 'pytorch': the stride sits on the 3x3).  dcn: the conv2 config of resnet.py:146-168 - a
     DCN / DCNv2 layer (DeformConvPack / ModulatedDeformConvPack) unless `fallback_on_stride`, which is popped from the dict
@@ -90,7 +105,7 @@ class Bottleneck(_EngineOnly):
     expansion = 4
 
     def __init__(self, inplanes, planes, stride, downsample, norm_cfg, conv_cfg=None, dcn=None, groups=1, base_width=4,
-                 gen_attention=None):
+                 gen_attention=None, gcb=None):
         super().__init__()
         width = block_width(planes, groups, base_width)
         self.conv1 = nn.Conv2d(inplanes, width, 1, bias=False)
@@ -107,6 +122,8 @@ class Bottleneck(_EngineOnly):
         self.downsample = downsample
         if gen_attention is not None:                                 # resnet.py:186-189, applied after relu(bn2(conv2))
             self.gen_attention_block = GeneralizedAttention(planes, gen_attention_spec(gen_attention, planes))
+        if gcb is not None:                                           # resnet.py:182-184, applied to bn3(conv3(.))
+            self.context_block = ContextBlock(planes * 4, gcb_spec(gcb, planes * 4))
 
 
 @BACKBONES.register_module
@@ -120,10 +137,16 @@ class ResNet(_EngineOnly):
         super().__init__()
         if depth not in self.arch_settings:
             raise KeyError('invalid depth {} for resnet'.format(depth))
-        if style != 'pytorch' or num_stages != 4 or tuple(strides) != (1, 2, 2, 2) or tuple(dilations) != (1, 1, 1, 1) \
-                or gcb is not None:
+        if style != 'pytorch' or num_stages != 4 or tuple(strides) != (1, 2, 2, 2) or tuple(dilations) != (1, 1, 1, 1):
             raise NotImplementedError("liborp_b200 builds the configuration of configs/dota/*.py: 4 stages, style 'pytorch', "
-                                      "strides (1,2,2,2), no dilation / GCB in the backbone")
+                                      "strides (1,2,2,2), no dilation in the backbone")
+        if gcb is not None:
+            if len(stage_with_gcb) != num_stages:
+                raise ValueError("stage_with_gcb=%r: needs one entry per stage (%d), as resnet.py:397-398 asserts"
+                                 % (tuple(stage_with_gcb), num_stages))
+            if not any(stage_with_gcb):
+                raise NotImplementedError("gcb=%r selects no block: stage_with_gcb is all False, so the reference builds no "
+                                          "context block; set stage_with_gcb (e.g. (False, True, True, True)) or drop gcb" % (gcb,))
         if dcn is not None:
             assert isinstance(dcn, dict) and len(stage_with_dcn) == num_stages
             if dcn.get('deformable_groups', 1) != 1:
@@ -137,12 +160,15 @@ class ResNet(_EngineOnly):
         self.stage_with_gen_attention = tuple(tuple(s) for s in stage_with_gen_attention)
         if gen_attention is not None:
             assert isinstance(gen_attention, dict) and len(self.stage_with_gen_attention) == num_stages
+        self.gcb = None if gcb is None else dict(gcb)
+        self.stage_with_gcb = tuple(stage_with_gcb)
         self.conv1 = nn.Conv2d(in_channels, 64, 7, 2, 3, bias=False)
         self.add_module('bn1', build_norm_layer(norm_cfg, 64, 1)[1])
         inplanes = 64
         for i, nblk in enumerate(self.arch_settings[depth]):
             planes, blocks = 64 << i, []
             stage_dcn = dcn if self.stage_with_dcn[i] else None      # the one shared dict (resnet.py:402, 146-147)
+            stage_gcb = self.gcb if gcb is not None and self.stage_with_gcb[i] else None   # every block of the stage (resnet.py:411)
             for b in range(nblk):
                 stride = strides[i] if b == 0 else 1
                 ds = None
@@ -151,7 +177,7 @@ class ResNet(_EngineOnly):
                 # make_res_layer (resnet.py:283-300): block b gets the dict when b is listed; an index past the stage builds nothing
                 ga = self.gen_attention if b in self.stage_with_gen_attention[i] else None
                 blocks.append(Bottleneck(inplanes, planes, stride, ds, norm_cfg, conv_cfg, stage_dcn, gen_attention=ga,
-                                         **self._block_args()))
+                                         gcb=stage_gcb, **self._block_args()))
                 inplanes = planes * 4
             self.add_module('layer%d' % (i + 1), nn.Sequential(*blocks))
 
@@ -169,6 +195,13 @@ class ResNet(_EngineOnly):
         """per stage, per block: None, or the spec (weights.gen_attention_spec) of that block's gen_attention_block - what the
         engine builds after its conv2"""
         return tuple(tuple(blk.gen_attention_block.spec if hasattr(blk, 'gen_attention_block') else None
+                           for blk in getattr(self, 'layer%d' % (i + 1)))
+                     for i in range(len(self.arch_settings[self.depth])))
+
+    def gcb_layout(self):
+        """per stage, per block: None, or the spec (weights.gcb_spec) of that block's context_block - what the engine runs on
+        bn3(conv3(.)) before the residual add"""
+        return tuple(tuple(blk.context_block.spec if hasattr(blk, 'context_block') else None
                            for blk in getattr(self, 'layer%d' % (i + 1)))
                      for i in range(len(self.arch_settings[self.depth])))
 
@@ -457,6 +490,8 @@ class OrientedRepPointsDetector(nn.Module):
             from .weights import random_state_dict
             ga = dict(gen_attention=self.backbone.gen_attention,
                       stage_with_gen_attention=self.backbone.stage_with_gen_attention) if self.backbone.gen_attention else {}
+            if self.backbone.gcb is not None:
+                ga.update(gcb=self.backbone.gcb, stage_with_gcb=self.backbone.stage_with_gcb)
             sd = random_state_dict(self.backbone.depth, seed=0, reference_init=True, num_classes=self.bbox_head.num_classes,
                                    dcn=self.backbone.dcn_cfg, stage_with_dcn=self.backbone.stage_with_dcn,
                                    **self.backbone._block_args(), **ga)
@@ -490,6 +525,7 @@ class OrientedRepPointsDetector(nn.Module):
                                   test_cfg=dict(self.test_cfg) if self.test_cfg else None,
                                   dcn=self.backbone.dcn_layout() if resnet else None,
                                   gen_attention=self.backbone.gen_attention_layout() if resnet else None,
+                                  gcb=self.backbone.gcb_layout() if resnet else None,
                                   pooling_type=self.neck.pooling_type if hr else 'AVG')
         return self._engine
 

@@ -175,6 +175,97 @@ def _draw_gen_attention(sd, p, spec, g, gamma):
         sd[k] = w
 
 
+# ContextBlock's arguments besides inplanes (context_block.py:15-19) and the fusions it knows, in the order it applies them
+GCB_ARGS = ('ratio', 'pooling_type', 'fusion_types')
+GCB_FUSIONS = ('channel_add', 'channel_mul')
+GCB_MAX_PLANES = 2048
+
+
+def gcb_spec(cfg, channels):
+    """the block that ContextBlock(channels, **cfg) builds, as the engine runs it: dict(channels, planes = int(channels * ratio),
+    pooling_type, fusion_types - the fusions used, in GCB_FUSIONS order).  ValueError where the reference itself fails (a
+    pooling_type other than 'avg' / 'att', fusion_types that are not a non-empty list or tuple of known fusions, planes < 1),
+    NotImplementedError for more than GCB_MAX_PLANES planes, TypeError for a missing ratio or an unknown argument"""
+    if not isinstance(cfg, dict):
+        raise ValueError("gcb must be a dict of ContextBlock arguments, not %r" % (cfg,))
+    unknown = sorted(set(cfg) - set(GCB_ARGS))
+    if unknown:
+        raise TypeError("ContextBlock got unexpected arguments %s" % unknown)
+    if 'ratio' not in cfg:
+        raise TypeError("ContextBlock needs a ratio (context_block.py:15-19)")
+    pooling, fusions = cfg.get('pooling_type', 'att'), cfg.get('fusion_types', ('channel_add',))
+    if pooling not in ('avg', 'att'):
+        raise ValueError("gcb with pooling_type=%r: context_block.py:21 takes 'avg' or 'att'" % (pooling,))
+    if not isinstance(fusions, (list, tuple)) or not fusions or any(f not in GCB_FUSIONS for f in fusions):
+        raise ValueError("gcb with fusion_types=%r: context_block.py:22-25 needs a non-empty list or tuple of %s"
+                         % (fusions, GCB_FUSIONS))
+    planes = int(channels * cfg['ratio'])
+    if planes < 1:
+        raise ValueError("gcb with ratio=%r on %d channels gives int(%d * ratio) = %d planes: the MLP needs at least one"
+                         % (cfg['ratio'], channels, channels, planes))
+    if planes > GCB_MAX_PLANES:
+        raise NotImplementedError("gcb with ratio=%r on %d channels gives %d planes: liborp_b200 runs up to %d"
+                                  % (cfg['ratio'], channels, planes, GCB_MAX_PLANES))
+    return dict(channels=channels, planes=planes, pooling_type=pooling, fusion_types=tuple(f for f in GCB_FUSIONS if f in fusions))
+
+
+def gcb_layout(depth, gcb=None, stage_with_gcb=(False, False, False, False)):
+    """what ResNet(depth, gcb=..., stage_with_gcb=...) builds after each block's bn3, per stage and block: None or the block's
+    gcb_spec.  Every block of a selected stage has one (resnet.py:411, 282-298).  ValueError unless stage_with_gcb names the
+    four stages"""
+    if gcb is None:
+        return tuple((None,) * nblk for nblk in STAGE_BLOCKS[depth])
+    if len(stage_with_gcb) != len(STAGE_BLOCKS[depth]):
+        raise ValueError("stage_with_gcb=%r: needs one entry per stage (%d), as resnet.py:397-398 asserts"
+                         % (tuple(stage_with_gcb), len(STAGE_BLOCKS[depth])))
+    return tuple(tuple(gcb_spec(gcb, 256 << li) if stage_with_gcb[li] else None for _ in range(nblk))
+                 for li, nblk in enumerate(STAGE_BLOCKS[depth]))
+
+
+def gcb_keys(spec):
+    """the parameter names (after `context_block.`) of a block with this spec, with their shapes"""
+    c, p = spec['channels'], spec['planes']
+    keys = {}
+    if spec['pooling_type'] == 'att':
+        keys['conv_mask.weight'] = (1, c, 1, 1)
+        keys['conv_mask.bias'] = (1,)
+    for f in spec['fusion_types']:
+        keys[f + '_conv.0.weight'] = (p, c, 1, 1)
+        keys[f + '_conv.0.bias'] = (p,)
+        keys[f + '_conv.1.weight'] = (p, 1, 1)
+        keys[f + '_conv.1.bias'] = (p, 1, 1)
+        keys[f + '_conv.3.weight'] = (c, p, 1, 1)
+        keys[f + '_conv.3.bias'] = (c,)
+    return keys
+
+
+def _draw_gcb(sd, p, spec, g, gain):
+    """a context_block as the reference initialises it: ResNet.init_weights' kaiming (fan_out, normal, zero bias) on every
+    nn.Conv2d, conv_mask and the last convolution included (resnet.py:474-476 re-draws what ContextBlock.reset_parameters set),
+    LayerNorm weight 1 and bias 0.
+    gain > 0 (tests only): conv_mask from N(0, 1 / C) (logits of about unit spread for unit-variance inputs) with an N(0, 1)
+    bias, N(0, 0.1^2) biases on the first convolution, LayerNorm weight in [0.5, 1.5] and bias N(0, 0.1^2), and the last
+    convolution and its N(0, 0.1^2) bias times gain, so every term acts"""
+    c = spec['channels']
+    for name, shape in gcb_keys(spec).items():
+        w = torch.empty(shape)
+        if name == 'conv_mask.weight' and gain > 0:
+            w.normal_(0, math.sqrt(1.0 / c), generator=g)
+        elif name.endswith('weight') and len(shape) == 4:
+            _kaiming_fan_out(w, g)
+            if name.endswith('.3.weight') and gain > 0:
+                w *= gain
+        elif gain <= 0:
+            w.fill_(1.0 if name.endswith('.1.weight') else 0.0)
+        elif name.endswith('.1.weight'):
+            w.uniform_(0.5, 1.5, generator=g)
+        else:
+            w.normal_(0, 1.0 if name == 'conv_mask.bias' else 0.1, generator=g)
+            if name.endswith('.3.bias'):
+                w *= gain
+        sd[p + '.context_block.' + name] = w
+
+
 def _drawers(sd, g, reference_init, residual_gain):
     """the (conv, norm) draws of the random state dicts into sd from generator g"""
 
@@ -239,7 +330,8 @@ def _draw_head(sd, g, conv, norm, reference_init, num_classes, feat):
 
 def random_state_dict(depth=50, seed=0, reference_init=True, num_classes=16, feat=256, residual_gain=1.0, dcn=None,
                       stage_with_dcn=(False, False, False, False), dcn_offset_scale=0.0, groups=1, base_width=4,
-                      gen_attention=None, stage_with_gen_attention=((), (), (), ()), gen_attention_gamma=0.0):
+                      gen_attention=None, stage_with_gen_attention=((), (), (), ()), gen_attention_gamma=0.0, gcb=None,
+                      stage_with_gcb=(False, False, False, False), gcb_gain=0.0):
     """reference_init=True reproduces the reference's init_weights (incl. zero_init_residual and all-ones
     norm scales); False randomises norm parameters / running statistics so that every branch of the graph
     carries signal (used by the parity tests); residual_gain scales the randomised scale of every block's last norm
@@ -254,7 +346,10 @@ def random_state_dict(depth=50, seed=0, reference_init=True, num_classes=16, fea
     its kaiming fan_out width * 9 as for any nn.Conv2d.  groups=1 draws exactly the ResNet's tensors.
     gen_attention / stage_with_gen_attention: the blocks' gen_attention_block as ResNet takes them (gen_attention_layout),
     drawn by _draw_gen_attention after the block's other tensors; gen_attention_gamma > 0 (tests only) makes them act (see
-    there).  Without attention blocks every draw is what it was without these arguments."""
+    there).  Without attention blocks every draw is what it was without these arguments.
+    gcb / stage_with_gcb: the blocks' context_block as ResNet / ResNeXt take them (gcb_layout), drawn by _draw_gcb after the
+    block's other tensors; gcb_gain > 0 (tests only) makes every term act (see there; use it with reference_init=False and
+    a residual_gain).  Without context blocks every draw is what it was without these arguments."""
     check_groups(groups, base_width)
     if groups > 1 and dcn is not None and any(stage_with_dcn):
         raise NotImplementedError("dcn with groups=%d would be a grouped deformable convolution (resnext.py:56-66): not built" % groups)
@@ -264,6 +359,7 @@ def random_state_dict(depth=50, seed=0, reference_init=True, num_classes=16, fea
     ga_layout = gen_attention_layout(depth, gen_attention, stage_with_gen_attention)
     if groups > 1 and any(sp is not None for st in ga_layout for sp in st):
         raise NotImplementedError("gen_attention on ResNeXt: the reference's ResNeXt builds no attention blocks (resnext.py:196-216)")
+    gcb_lay = gcb_layout(depth, gcb, stage_with_gcb)
     conv, norm = _drawers(sd, g, reference_init, residual_gain)
 
     # ---------------------------------------------------------------- backbone (resnet.py)
@@ -299,6 +395,8 @@ def random_state_dict(depth=50, seed=0, reference_init=True, num_classes=16, fea
                 norm(p + ".downsample.1", planes * 4, True)
             if ga_layout[li][b] is not None:
                 _draw_gen_attention(sd, p, ga_layout[li][b], g, gen_attention_gamma)
+            if gcb_lay[li][b] is not None:
+                _draw_gcb(sd, p, gcb_lay[li][b], g, gcb_gain)
             inplanes = planes * 4
     # ---------------------------------------------------------------- neck (fpn.py, start_level=1, 5 outs)
     for i, cin in enumerate((512, 1024, 2048)):
