@@ -1,5 +1,5 @@
 """ctypes binding of liborp_b200.so (include/orp_b200.h, orp_b200_dcnv2.h, orp_b200_swin.h, orp_b200_group.h,
-orp_b200_hrnet.h, orp_b200_attention.h, orp_b200_context.h).
+orp_b200_hrnet.h, orp_b200_attention.h, orp_b200_context.h, orp_b200_carafe.h).
 
 There is NO fallback: if the shared library is missing or a call fails, an exception is raised.
 The library is built in-tree by `python -m orientedreppoints_b200.build` (nvcc, sm_90a).
@@ -228,6 +228,13 @@ CONTEXT_SIGNATURES = {
     "orp_context_fuse_f32": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
 }
 
+# name -> (restype, argtypes); every symbol include/orp_b200_carafe.h declares
+CARAFE_SIGNATURES = {
+    "orp_carafe_add_bf16": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _i, _vp, _i, _i, _vp, _vp]),
+    "orp_carafe_add_f16x3": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _i, _vp, _i, _i, _vp, _vp]),
+    "orp_carafe_add_f32": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _i, _vp, _i, _i, _vp, _vp]),
+}
+
 _LIB = None
 
 
@@ -246,7 +253,7 @@ def lib():
         l = ctypes.CDLL(LIB_PATH)
         for name, (res, args) in list(SIGNATURES.items()) + list(DCNV2_SIGNATURES.items()) + list(SWIN_SIGNATURES.items()) + \
                 list(GROUP_SIGNATURES.items()) + list(HRNET_SIGNATURES.items()) + list(ATTENTION_SIGNATURES.items()) + \
-                list(CONTEXT_SIGNATURES.items()):
+                list(CONTEXT_SIGNATURES.items()) + list(CARAFE_SIGNATURES.items()):
             fn = getattr(l, name)   # AttributeError if the symbol is not exported
             fn.restype = res
             fn.argtypes = args

@@ -33,6 +33,7 @@ def _headers():
     hs.append(os.path.join(HERE, "..", "include", "orp_b200_hrnet.h"))
     hs.append(os.path.join(HERE, "..", "include", "orp_b200_attention.h"))
     hs.append(os.path.join(HERE, "..", "include", "orp_b200_context.h"))
+    hs.append(os.path.join(HERE, "..", "include", "orp_b200_carafe.h"))
     return hs
 
 

@@ -148,11 +148,11 @@ class EngineF32:
 
 
 class OrientedRepPointsDetector:
-    """R-50 / R-101 / R-152, ResNeXt of those depths, or Swin-T/S/B/L + FPN(GN), or HRNet + HRFPN, + OrientedRepPointsHead,
-    inference only."""
+    """R-50 / R-101 / R-152, ResNeXt of those depths, or Swin-T/S/B/L + FPN(GN) or FPN_CARAFE, or HRNet + HRFPN,
+    + OrientedRepPointsHead, inference only."""
 
     def __init__(self, state_dict, depth=50, device="cuda", precision="fp32", test_cfg=None, dcn=None, pooling_type='AVG',
-                 gen_attention=None, gcb=None):
+                 gen_attention=None, gcb=None, neck=None):
         """depth: 50 / 101 / 152 (ResNet or ResNeXt: the groups of every conv2 come from the state dict's shapes), or a Swin backbone - "swin_tiny" (Swin-T, window 7), any key of swin.ARCHS
         ("swin_small", "swin_base_w12", ...) or a swin.SwinArch, or an HRNet backbone with the HRFPN neck (stride 2, five
         outputs) - a key of hrnet.ARCHS ("hrnetv2p_w18", ...) or an hrnet.HRNetArch.
@@ -162,7 +162,9 @@ class OrientedRepPointsDetector:
         (models.ResNet.gen_attention_layout, weights.gen_attention_layout).
         gcb: the ResNet's / ResNeXt's context blocks per stage and block, None or a weights.gcb_spec (models.ResNet.gcb_layout,
         weights.gcb_layout); each runs on bn3(conv3(.)) before the residual add (context_block.py).
-        pooling_type: HRFPN's pooling, 'AVG' or 'MAX' (HRNet only)"""
+        pooling_type: HRFPN's pooling, 'AVG' or 'MAX' (HRNet only).
+        neck: None (the FPN of configs/dota/*.py) or a weights.fpn_carafe_spec: the FPN_CARAFE neck of a ResNet / ResNeXt or
+        Swin backbone (carafe_fpn.py; models.FPN_CARAFE.spec); the state dict's neck.* tensors must be exactly its keys"""
         from . import hrnet
         from .swin import arch_of
         self.device = torch.device(device)
@@ -177,6 +179,8 @@ class OrientedRepPointsDetector:
         self.dcn = dcn
         self.gen_attention = gen_attention
         self.gcb = gcb
+        self.neck_spec = neck
+        self.neck = None                                   # carafe_fpn.CarafeFPN for FPN_CARAFE, None for FPN
         self.test_cfg = dict(nms_pre=2000, min_bbox_size=0, score_thr=0.05, nms=dict(type='rnms', iou_thr=0.4),
                              max_per_img=2000)                         # configs/dota/orientedrepoints_r50_demo.py:62-67
         if test_cfg:
@@ -209,6 +213,8 @@ class OrientedRepPointsDetector:
         if self.gcb is not None and (self.swin_arch is not None or self.hr_arch is not None):
             raise ValueError("gcb describes the context blocks of a ResNet / ResNeXt backbone; %s has none"
                              % ("the Swin backbone" if self.swin_arch is not None else "the HRNet backbone"))
+        if self.neck_spec is not None and self.hr_arch is not None:
+            raise NotImplementedError("FPN_CARAFE on an HRNet backbone: liborp_b200 builds HRNet with its HRFPN neck")
         if self.swin_arch is not None:
             if self.dcn is not None:
                 raise ValueError("dcn describes the deformable layers of a ResNet backbone; the Swin backbone has none")
@@ -261,6 +267,9 @@ class OrientedRepPointsDetector:
                 blk["gcb"] = self._context_block(sd, p, gcb[li][b], 256 << li)
                 stage.append(blk)
             self.blocks.append(stage)
+        if self.neck_spec is not None:
+            self._load_carafe_neck(sd, (512, 1024, 2048))
+            return self._load_head(sd)
         self.lat = [(ConvLayer(sd["neck.lateral_convs.%d.conv.weight" % i].float(), None, 1, 0, d),
                      Norm(sd, "neck.lateral_convs.%d.gn" % i, d)) for i in range(3)]
         self.fpn = [(ConvLayer(sd["neck.fpn_convs.%d.conv.weight" % i].float(), None, 2 if i >= 3 else 1, 1, d),
@@ -383,11 +392,22 @@ class OrientedRepPointsDetector:
         if self.eng.name not in ("bf16", "f16x3"):
             raise ValueError("the Swin backbones run on the tensor-core engines ('f16x3' or 'bf16')")
         self.swin = Swin(sd, d, self.eng, self.swin_arch)
+        if self.neck_spec is not None:
+            self._load_carafe_neck(sd, tuple(self.swin_arch.channels[1:]))
+            return self._load_head(sd)
         self.lat = [(ConvLayer(sd["neck.lateral_convs.%d.conv.weight" % i].float(), None, 1, 0, d),
                      Norm(sd, "neck.lateral_convs.%d.gn" % i, d)) for i in range(3)]
         self.fpn = [(ConvLayer(sd["neck.fpn_convs.%d.conv.weight" % i].float(), None, 1, 1, d),
                      Norm(sd, "neck.fpn_convs.%d.gn" % i, d)) for i in range(3)]
         self._load_head(sd)
+
+    def _load_carafe_neck(self, sd, widths):
+        """the FPN_CARAFE neck on the backbone's stride-8, -16 and -32 outputs of widths `widths`"""
+        from .carafe_fpn import CarafeFPN
+        if not isinstance(self.neck_spec, dict) or tuple(self.neck_spec.get('in_channels', ())) != widths:
+            raise ValueError("neck must be a weights.fpn_carafe_spec on the backbone's output widths %s, not %r"
+                             % (list(widths), self.neck_spec))
+        self.neck = CarafeFPN(sd, self.neck_spec, self.device)
 
     def _load_hrnet(self, sd):
         """HRNet + HRFPN (hrnet.HRNetGraph); conv1 (3x3 / s2 / pad 1) + bn1 + ReLU runs on the stem kernels"""
@@ -440,6 +460,8 @@ class OrientedRepPointsDetector:
         if self.swin_arch is not None:
             # decoded uint8 tiles: Normalize + ImageToTensor (+ the zero padding outside valid_hw) are fused into the patch gather
             c3, c4, c5 = self.swin.forward(img, self.img_norm_cfg, valid_hw)
+            if self.neck is not None:
+                return self.neck(e, [c3, c4, c5])
             l2 = e.conv_gn(c5, *self.lat[2])
             l1 = e.conv_gn(c4, *self.lat[1], up=l2)
             l0 = e.conv_gn(c3, *self.lat[0], up=l1)
@@ -468,6 +490,8 @@ class OrientedRepPointsDetector:
                     x = blk["gcb"](e, e.conv(o, blk["c3"]), idt)
             feats.append(x)
         c3, c4, c5 = feats[1], feats[2], feats[3]
+        if self.neck is not None:
+            return self.neck(e, [c3, c4, c5])
         l2 = e.conv_gn(c5, *self.lat[2])
         l1 = e.conv_gn(c4, *self.lat[1], up=l2)
         l0 = e.conv_gn(c3, *self.lat[0], up=l1)

@@ -1,7 +1,8 @@
 """Module-structure layer of the drop-in boundary (SURVEY.md 8(b), last row): the registries and the nn.Module parameter
 containers the reference's configs name - ResNet (mmdet/models/backbones/resnet.py:345-515), ResNeXt (resnext.py), SwinTransformer
 (backbones/swin_transformer.py:449-631), FPN (necks/fpn.py:50-136), OrientedRepPointsHead
-(anchor_heads/orientedreppoints_head.py:18-146), HRNet (backbones/hrnet.py) with HRFPN (necks/hrfpn.py), OrientedRepPointsDetector (detectors/orientedreppoints_detector.py,
+(anchor_heads/orientedreppoints_head.py:18-146), HRNet (backbones/hrnet.py) with HRFPN (necks/hrfpn.py), FPN_CARAFE
+(necks/fpn_carafe.py) with CARAFEPack (ops/carafe/carafe.py), OrientedRepPointsDetector (detectors/orientedreppoints_detector.py,
 single_stage.py) - with the reference's attribute names, so `build_detector(cfg.model, test_cfg=cfg.test_cfg)` builds from
 the reference's config dicts and `state_dict()` / `load_state_dict()` use the reference's keys (published checkpoints load).
 
@@ -16,7 +17,7 @@ from .ops.conv_module import ConvModule
 from .ops.dcn import DeformConv, DeformConvPack, ModulatedDeformConvPack
 from .ops.norm import build_norm_layer
 from .utils.registry import Registry, build_from_cfg
-from .weights import STAGE_BLOCKS, block_width, check_groups, gcb_spec, gen_attention_spec
+from .weights import STAGE_BLOCKS, block_width, check_groups, fpn_carafe_spec, gcb_spec, gen_attention_spec
 
 BACKBONES = Registry('backbone')
 NECKS = Registry('neck')
@@ -426,6 +427,54 @@ class FPN(_EngineOnly):
                 self.fpn_convs.append(ConvModule(cin, out_channels, 3, stride=2, padding=1, conv_cfg=conv_cfg, norm_cfg=norm_cfg, act_cfg=None, inplace=False))
 
 
+class CARAFEPack(_EngineOnly):
+    """the parameter tree of carafe.py:161-214 with scale factor 2: channel_compressor (1x1 C -> compressed_channels) and
+    content_encoder (encoder_kernel, C' -> up_kernel^2 * up_group * 4), both with a bias"""
+
+    def __init__(self, channels, up_kernel=5, up_group=1, encoder_kernel=3, compressed_channels=64):
+        super().__init__()
+        self.channels, self.up_kernel, self.up_group = channels, up_kernel, up_group
+        self.channel_compressor = nn.Conv2d(channels, compressed_channels, 1)
+        self.content_encoder = nn.Conv2d(compressed_channels, up_kernel * up_kernel * up_group * 4, encoder_kernel,
+                                         padding=(encoder_kernel - 1) // 2)
+
+
+@NECKS.register_module
+class FPN_CARAFE(_EngineOnly):
+    """fpn_carafe.py:34-200 with the reference's tree and keys.  Built: five outputs at the head's strides 8..128 - the
+    backbone's stride-8, -16 and -32 outputs (in_channels[start_level:], end_level=-1) and two extra levels - with
+    upsample_cfg type 'carafe' and the arguments weights.fpn_carafe_spec accepts; `spec` is that description"""
+
+    def __init__(self, in_channels, out_channels, num_outs, start_level=0, end_level=-1, norm_cfg=None, act_cfg=None,
+                 order=('conv', 'norm', 'act'),
+                 upsample_cfg=dict(type='carafe', up_kernel=5, up_group=1, encoder_kernel=3, encoder_dilation=1)):
+        super().__init__()
+        assert isinstance(in_channels, list)
+        if end_level != -1:
+            raise NotImplementedError("FPN_CARAFE end_level=%r: liborp_b200 builds end_level=-1, with two extra levels" % (end_level,))
+        if not 0 <= start_level < len(in_channels) or num_outs < len(in_channels) - start_level:
+            raise ValueError("FPN_CARAFE start_level=%r, num_outs=%r on %d inputs: the reference asserts num_outs >= %d inputs - "
+                             "start_level" % (start_level, num_outs, len(in_channels), len(in_channels)))
+        if len(in_channels) - start_level != 3 or num_outs != 5:
+            raise NotImplementedError("FPN_CARAFE start_level=%r, num_outs=%r on %d inputs: liborp_b200 builds three backbone "
+                                      "levels (strides 8, 16, 32) and num_outs=5" % (start_level, num_outs, len(in_channels)))
+        self.spec = fpn_carafe_spec(in_channels[start_level:], out_channels, norm_cfg, act_cfg, order, upsample_cfg)
+        self.in_channels, self.out_channels, self.num_ins, self.num_outs = in_channels, out_channels, len(in_channels), num_outs
+        self.start_level, self.end_level, self.norm_cfg, self.act_cfg, self.order = start_level, end_level, norm_cfg, act_cfg, order
+        sp = self.spec
+        kw = dict(norm_cfg=norm_cfg, bias=norm_cfg is None, act_cfg=act_cfg, inplace=False, order=tuple(order))
+        self.lateral_convs, self.fpn_convs, self.upsample_modules = nn.ModuleList(), nn.ModuleList(), nn.ModuleList()
+        for cin in sp['in_channels']:
+            self.lateral_convs.append(ConvModule(cin, out_channels, 1, **kw))
+        self.lateral_convs.append(ConvModule(sp['in_channels'][-1], out_channels, 3, stride=2, padding=1, **kw))
+        self.lateral_convs.append(ConvModule(out_channels, out_channels, 3, stride=2, padding=1, **kw))
+        for _ in range(5):
+            self.fpn_convs.append(ConvModule(out_channels, out_channels, 3, padding=1, **kw))
+        for _ in range(4):
+            self.upsample_modules.append(CARAFEPack(out_channels, sp['up_kernel'], sp['up_group'], sp['encoder_kernel'],
+                                                    sp['compressed_channels']))
+
+
 @HEADS.register_module
 class OrientedRepPointsHead(_EngineOnly):
     def __init__(self, num_classes, in_channels, feat_channels=256, point_feat_channels=256, stacked_convs=3, num_points=9,
@@ -468,7 +517,18 @@ class OrientedRepPointsDetector(nn.Module):
         self.bbox_head = build_head(bbox_head)
         if isinstance(self.backbone, HRNet) != isinstance(self.neck, HRFPN):
             raise NotImplementedError("%s with %s: liborp_b200 builds HRNet with the HRFPN neck, and the ResNet / Swin backbones "
-                                      "with FPN" % (type(self.backbone).__name__, type(self.neck).__name__))
+                                      "with FPN or FPN_CARAFE" % (type(self.backbone).__name__, type(self.neck).__name__))
+        if isinstance(self.neck, FPN_CARAFE):
+            if isinstance(self.backbone, ResNet):
+                widths = [256 << i for i in self.backbone.out_indices]
+            else:
+                widths = [self.backbone.embed_dim << i for i in self.backbone.out_indices]
+            if list(self.neck.in_channels) != widths or list(self.neck.spec['in_channels']) != widths[-3:]:
+                raise ValueError("FPN_CARAFE in_channels %s with start_level %d are not the backbone's outputs %s ending in its "
+                                 "stride-8, -16 and -32 levels" % (list(self.neck.in_channels), self.neck.start_level, widths))
+            if self.neck.out_channels != self.bbox_head.in_channels:
+                raise ValueError("FPN_CARAFE out_channels %d are not the head's in_channels %d"
+                                 % (self.neck.out_channels, self.bbox_head.in_channels))
         if isinstance(self.neck, HRFPN):
             if list(self.neck.in_channels) != list(self.backbone.arch.out_widths):
                 raise ValueError("HRFPN in_channels %s are not the HRNet's stage-4 widths %s"
@@ -492,6 +552,8 @@ class OrientedRepPointsDetector(nn.Module):
                       stage_with_gen_attention=self.backbone.stage_with_gen_attention) if self.backbone.gen_attention else {}
             if self.backbone.gcb is not None:
                 ga.update(gcb=self.backbone.gcb, stage_with_gcb=self.backbone.stage_with_gcb)
+            if isinstance(self.neck, FPN_CARAFE):
+                ga.update(neck=self.neck.spec)
             sd = random_state_dict(self.backbone.depth, seed=0, reference_init=True, num_classes=self.bbox_head.num_classes,
                                    dcn=self.backbone.dcn_cfg, stage_with_dcn=self.backbone.stage_with_dcn,
                                    **self.backbone._block_args(), **ga)
@@ -501,7 +563,8 @@ class OrientedRepPointsDetector(nn.Module):
                                          feat=self.neck.out_channels, zero_init_residual=self.backbone.zero_init_residual)
         else:
             from .swin import random_swin_state_dict
-            sd = random_swin_state_dict(0, num_classes=self.bbox_head.num_classes, arch=self.backbone.arch)
+            sd = random_swin_state_dict(0, num_classes=self.bbox_head.num_classes, arch=self.backbone.arch,
+                                        neck=self.neck.spec if isinstance(self.neck, FPN_CARAFE) else None)
         self.load_state_dict(sd, strict=True)
         if isinstance(pretrained, str) and os.path.isfile(pretrained):
             ck = torch.load(pretrained, map_location='cpu')
@@ -526,7 +589,8 @@ class OrientedRepPointsDetector(nn.Module):
                                   dcn=self.backbone.dcn_layout() if resnet else None,
                                   gen_attention=self.backbone.gen_attention_layout() if resnet else None,
                                   gcb=self.backbone.gcb_layout() if resnet else None,
-                                  pooling_type=self.neck.pooling_type if hr else 'AVG')
+                                  pooling_type=self.neck.pooling_type if hr else 'AVG',
+                                  neck=self.neck.spec if isinstance(self.neck, FPN_CARAFE) else None)
         return self._engine
 
     def extract_feat(self, img):

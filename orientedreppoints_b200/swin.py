@@ -78,11 +78,12 @@ def arch_of(depth):
     return None
 
 
-def random_swin_state_dict(seed=0, feat=256, num_classes=16, arch=SWIN_T):
+def random_swin_state_dict(seed=0, feat=256, num_classes=16, arch=SWIN_T, neck=None, carafe_gain=0.0):
     """trunc_normal(.02) linears, zero biases, unit LayerNorms (swin_transformer.py:571-579) - plus the FPN/head
     entries of weights.random_state_dict with the Swin neck shapes (in_channels 2E, 4E, 8E).  Biases/norms are randomised a
     little so that every term of the graph carries signal in the parity tests.  The draws are in parameter order, so Swin-T's
-    are those of every earlier version of this function."""
+    are those of every earlier version of this function.  neck: None (FPN) or a weights.fpn_carafe_spec, drawn by
+    weights._draw_fpn_carafe with randomised norms and biases (carafe_gain as there); without it the draws are unchanged."""
     from .weights import random_state_dict
     arch = arch_of(arch) if not isinstance(arch, str) else ARCHS[arch]
     embed, nb = arch.embed, (2 * arch.window - 1) ** 2
@@ -121,6 +122,10 @@ def random_swin_state_dict(seed=0, feat=256, num_classes=16, arch=SWIN_T):
     for k, v in base.items():
         if k.startswith("bbox_head."):
             sd[k] = v
+    if neck is not None:
+        from .weights import _draw_fpn_carafe
+        _draw_fpn_carafe(sd, g, neck, False, carafe_gain)
+        return sd
     for i, cin in enumerate(arch.channels[1:]):
         sd["neck.lateral_convs.%d.conv.weight" % i] = torch.empty(feat, cin, 1, 1).normal_(0, 1.0 / math.sqrt(cin), generator=g)
         sd["neck.fpn_convs.%d.conv.weight" % i] = torch.empty(feat, feat, 3, 3).normal_(0, 1.0 / math.sqrt(feat * 9), generator=g)

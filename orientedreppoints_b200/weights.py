@@ -6,6 +6,8 @@ Key names follow the reference modules so published checkpoints load unchanged (
   downsample.{0,1}.*            (mmdet/models/backbones/resnet.py:84-239, 345-515; ResNeXt: resnext.py:11-70, the same
                                  keys with conv1 / conv2 / bn1 / bn2 `width` wide and conv2 grouped)
   neck.lateral_convs.{i}.{conv,gn}.*, neck.fpn_convs.{i}.{conv,gn}.*   (necks/fpn.py:88-128)
+  or, for FPN_CARAFE, neck.lateral_convs.{0..4}.*, neck.fpn_convs.{0..4}.*, neck.upsample_modules.{0..3}.{channel_compressor,
+  content_encoder}.*                                                   (necks/fpn_carafe.py:34-200, ops/carafe/carafe.py:161-214)
   bbox_head.{cls,reg}_convs.{i}.{conv,gn}.*, bbox_head.reppoints_*     (orientedreppoints_head.py:91-132)
 Tensors are in the reference's layouts (conv weights [Cout, Cin, KH, KW]).
 """
@@ -266,6 +268,112 @@ def _draw_gcb(sd, p, spec, g, gain):
         sd[p + '.context_block.' + name] = w
 
 
+CARAFE_KERNELS = (1, 3, 5, 7)
+CARAFE_GROUPS = (1, 2, 4)
+
+
+def fpn_carafe_spec(in_channels, out_channels, norm_cfg=None, act_cfg=None, order=('conv', 'norm', 'act'),
+                    upsample_cfg=dict(type='carafe', up_kernel=5, up_group=1, encoder_kernel=3, encoder_dilation=1)):
+    """the engine's description of an FPN_CARAFE neck (fpn_carafe.py:34-200) on the backbone's stride-8, -16 and -32 outputs,
+    whose widths are `in_channels`, with two extra levels (3x3 stride-2 laterals): dict(in_channels, out_channels, norm
+    (None or 'GN'), relu, up_kernel, up_group, encoder_kernel, compressed_channels).  ValueError where the reference itself
+    fails, NotImplementedError (naming the argument) for what the engine does not build"""
+    if tuple(order) not in (('conv', 'norm', 'act'), ('act', 'conv', 'norm')):
+        raise ValueError("FPN_CARAFE order=%r: the reference accepts ('conv', 'norm', 'act') and ('act', 'conv', 'norm')" % (order,))
+    if act_cfg is not None:
+        if tuple(order) != ('conv', 'norm', 'act'):
+            raise NotImplementedError("FPN_CARAFE order=%r with an activation: liborp_b200 builds order ('conv', 'norm', 'act'), "
+                                      "or ('act', 'conv', 'norm') with act_cfg=None" % (order,))
+        if dict(act_cfg, inplace=None) != dict(type='ReLU', inplace=None):
+            raise NotImplementedError("FPN_CARAFE act_cfg=%r: liborp_b200 builds None or ReLU" % (act_cfg,))
+    if norm_cfg is not None:
+        n = dict(norm_cfg)
+        n.pop('requires_grad', None)
+        if n != dict(type='GN', num_groups=32):
+            raise NotImplementedError("FPN_CARAFE norm_cfg=%r: liborp_b200 builds None or GN with 32 groups" % (norm_cfg,))
+    if out_channels != 256:
+        raise NotImplementedError("FPN_CARAFE out_channels=%r: liborp_b200 builds the head's 256" % (out_channels,))
+    cfg = dict(upsample_cfg) if upsample_cfg is not None else dict(type=None)
+    kind = cfg.pop('type', None)
+    if kind in ('nearest', 'bilinear'):
+        raise NotImplementedError("FPN_CARAFE upsample_cfg type %r: liborp_b200 builds 'carafe'" % (kind,))
+    if kind != 'carafe':
+        raise ValueError("FPN_CARAFE upsample_cfg type %r: the reference fails on it (%s)"
+                         % (kind, "slice_as asserts on the un-upsampled lateral" if kind is None else
+                            "hasattr(dict, 'upsample_kernel') is False" if kind in ('deconv', 'pixel_shuffle') else
+                            "it is not one of its upsample types"))
+    args = dict(up_kernel=5, up_group=1, encoder_kernel=3, encoder_dilation=1, compressed_channels=64)
+    unknown = set(cfg) - set(args)
+    if unknown:
+        raise ValueError("FPN_CARAFE upsample_cfg: CARAFEPack takes no argument %s" % sorted(unknown))
+    args.update(cfg)
+    k, grp = args['up_kernel'], args['up_group']
+    if not isinstance(k, int) or k < 1 or k % 2 == 0:
+        raise ValueError("FPN_CARAFE up_kernel=%r: the carafe op asserts an odd kernel >= 1" % (k,))
+    if k not in CARAFE_KERNELS:
+        raise NotImplementedError("FPN_CARAFE up_kernel=%r: liborp_b200 builds %s" % (k, CARAFE_KERNELS))
+    if not isinstance(grp, int) or grp < 1 or out_channels % grp:
+        raise ValueError("FPN_CARAFE up_group=%r: the carafe op asserts that it divides the %d channels" % (grp, out_channels))
+    if grp not in CARAFE_GROUPS:
+        raise NotImplementedError("FPN_CARAFE up_group=%r: liborp_b200 builds %s" % (grp, CARAFE_GROUPS))
+    if args['encoder_kernel'] not in (1, 3):
+        raise NotImplementedError("FPN_CARAFE encoder_kernel=%r: liborp_b200 builds 1 and 3" % (args['encoder_kernel'],))
+    if args['encoder_dilation'] != 1:
+        raise NotImplementedError("FPN_CARAFE encoder_dilation=%r: liborp_b200 builds 1" % (args['encoder_dilation'],))
+    cc = args['compressed_channels']
+    if not isinstance(cc, int) or cc < 8 or cc % 8:
+        raise NotImplementedError("FPN_CARAFE compressed_channels=%r: liborp_b200 builds positive multiples of 8" % (cc,))
+    return dict(in_channels=tuple(in_channels), out_channels=out_channels, norm=None if norm_cfg is None else 'GN',
+                relu=act_cfg is not None, up_kernel=k, up_group=grp, encoder_kernel=args['encoder_kernel'], compressed_channels=cc)
+
+
+def fpn_carafe_keys(spec):
+    """{key: shape} of the neck.* parameters of an FPN_CARAFE of spec (fpn_carafe_spec): every ConvModule has a bias iff it
+    has no norm; laterals 0..2 are 1x1 on the backbone levels, 3 a 3x3 / s2 on the last of them, 4 a 3x3 / s2 on lateral 3"""
+    out, keys = spec['out_channels'], {}
+
+    def cm(name, cin, k):
+        keys[name + '.conv.weight'] = (out, cin, k, k)
+        if spec['norm'] is None:
+            keys[name + '.conv.bias'] = (out,)
+        else:
+            keys[name + '.gn.weight'] = keys[name + '.gn.bias'] = (out,)
+    for i, cin in enumerate(spec['in_channels']):
+        cm('neck.lateral_convs.%d' % i, cin, 1)
+    cm('neck.lateral_convs.3', spec['in_channels'][-1], 3)
+    cm('neck.lateral_convs.4', out, 3)
+    for i in range(5):
+        cm('neck.fpn_convs.%d' % i, out, 3)
+    cc, ek = spec['compressed_channels'], spec['encoder_kernel']
+    ce = spec['up_kernel'] ** 2 * spec['up_group'] * 4
+    for j in range(4):
+        p = 'neck.upsample_modules.%d.' % j
+        keys[p + 'channel_compressor.weight'], keys[p + 'channel_compressor.bias'] = (cc, out, 1, 1), (cc,)
+        keys[p + 'content_encoder.weight'], keys[p + 'content_encoder.bias'] = (ce, cc, ek, ek), (ce,)
+    return keys
+
+
+def _draw_fpn_carafe(sd, g, spec, reference_init, carafe_gain):
+    """FPN_CARAFE.init_weights (fpn_carafe.py:203-209): xavier-uniform on every conv with zero biases, then CARAFEPack's
+    normal_init(std=0.001) on content_encoder; norms 1 / 0.  reference_init=False randomises the norms and the biases.
+    carafe_gain > 0 (tests only) draws content_encoder from N(0, gain^2 / fan_in) with N(0, (gain / 2)^2) biases instead, so
+    that the logits spread over several units: with the reference's init the softmax is almost uniform"""
+    for k, shape in fpn_carafe_keys(spec).items():
+        if k.endswith('.gn.weight'):
+            sd[k] = torch.ones(shape) if reference_init else torch.empty(shape).uniform_(0.5, 1.5, generator=g)
+        elif k.endswith('.bias'):
+            sd[k] = torch.zeros(shape) if reference_init else torch.empty(shape).normal_(0, 0.1, generator=g)
+        elif 'content_encoder' in k:
+            fan_in = shape[1] * shape[2] * shape[3]
+            sd[k] = torch.empty(shape).normal_(0, carafe_gain / math.sqrt(fan_in) if carafe_gain > 0 else 0.001, generator=g)
+        else:
+            sd[k] = _xavier_uniform(torch.empty(shape), g)
+    if carafe_gain > 0:
+        for j in range(4):
+            b = 'neck.upsample_modules.%d.content_encoder.bias' % j
+            sd[b] = torch.empty(sd[b].shape).normal_(0, carafe_gain / 2, generator=g)
+
+
 def _drawers(sd, g, reference_init, residual_gain):
     """the (conv, norm) draws of the random state dicts into sd from generator g"""
 
@@ -331,7 +439,7 @@ def _draw_head(sd, g, conv, norm, reference_init, num_classes, feat):
 def random_state_dict(depth=50, seed=0, reference_init=True, num_classes=16, feat=256, residual_gain=1.0, dcn=None,
                       stage_with_dcn=(False, False, False, False), dcn_offset_scale=0.0, groups=1, base_width=4,
                       gen_attention=None, stage_with_gen_attention=((), (), (), ()), gen_attention_gamma=0.0, gcb=None,
-                      stage_with_gcb=(False, False, False, False), gcb_gain=0.0):
+                      stage_with_gcb=(False, False, False, False), gcb_gain=0.0, neck=None, carafe_gain=0.0):
     """reference_init=True reproduces the reference's init_weights (incl. zero_init_residual and all-ones
     norm scales); False randomises norm parameters / running statistics so that every branch of the graph
     carries signal (used by the parity tests); residual_gain scales the randomised scale of every block's last norm
@@ -349,7 +457,9 @@ def random_state_dict(depth=50, seed=0, reference_init=True, num_classes=16, fea
     there).  Without attention blocks every draw is what it was without these arguments.
     gcb / stage_with_gcb: the blocks' context_block as ResNet / ResNeXt take them (gcb_layout), drawn by _draw_gcb after the
     block's other tensors; gcb_gain > 0 (tests only) makes every term act (see there; use it with reference_init=False and
-    a residual_gain).  Without context blocks every draw is what it was without these arguments."""
+    a residual_gain).  Without context blocks every draw is what it was without these arguments.
+    neck: None (the FPN of configs/dota/*.py) or an fpn_carafe_spec, drawn by _draw_fpn_carafe in the FPN's place; carafe_gain
+    > 0 (tests only) spreads its encoder logits (see there).  Without `neck` every draw is what it was without these arguments."""
     check_groups(groups, base_width)
     if groups > 1 and dcn is not None and any(stage_with_dcn):
         raise NotImplementedError("dcn with groups=%d would be a grouped deformable convolution (resnext.py:56-66): not built" % groups)
@@ -399,6 +509,10 @@ def random_state_dict(depth=50, seed=0, reference_init=True, num_classes=16, fea
                 _draw_gcb(sd, p, gcb_lay[li][b], g, gcb_gain)
             inplanes = planes * 4
     # ---------------------------------------------------------------- neck (fpn.py, start_level=1, 5 outs)
+    if neck is not None:
+        _draw_fpn_carafe(sd, g, neck, reference_init, carafe_gain)
+        _draw_head(sd, g, conv, norm, reference_init, num_classes, feat)
+        return sd
     for i, cin in enumerate((512, 1024, 2048)):
         conv("neck.lateral_convs.%d.conv" % i, feat, cin, 1, "xavier")
         norm("neck.lateral_convs.%d.gn" % i, feat, False)
